@@ -1,9 +1,9 @@
-"""Builds libemotivoice_b200.so in-tree with nvcc for sm_100a (no torch involved).
+"""Builds libemotivoice_b200.so in-tree with nvcc for sm_90a (H100; no torch involved).
 
     python -m emotivoice_b200.build [--force]
 
 The shared library is the product's only compute path; there is no CPU or eager
-fallback.  It is git-ignored but travels to the GPU box with the snapshot.
+fallback.  It is git-ignored: build() makes it from the sources in every checkout.
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libemotivoice_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "-cudart", "static"]
 
 
@@ -29,7 +29,7 @@ def _digest():
     files = sources() + sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh"))
     files.append(os.path.join(INCLUDE, "emotivoice_b200.h"))
     for f in files:
-        h.update(os.path.basename(f).encode())      # names, not absolute paths: the tree is relocated on the GPU box
+        h.update(os.path.basename(f).encode())      # names, not absolute paths: a built tree may be moved
         with open(f, "rb") as fh:
             h.update(fh.read())
     h.update(" ".join(NVCC_FLAGS).encode())
@@ -45,8 +45,13 @@ def nvcc_path():
 
 def build(force=False, verbose=True):
     """Idempotent and safe to call from several processes at once (torchrun ranks): the check-and-compile
-    section runs under an exclusive file lock, so one process compiles and the others then find the stamp."""
+    section runs under an exclusive file lock, so one process compiles and the others then find the stamp.
+    A current library is found without writing anything, so a built tree may be read-only."""
     import fcntl
+    if not force and _up_to_date(_digest()):
+        if verbose:
+            print("emotivoice_b200.build: up to date, not recompiled", flush=True)
+        return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
     with open(os.path.join(LIB_DIR, ".build.lock"), "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)
@@ -56,10 +61,18 @@ def build(force=False, verbose=True):
             fcntl.flock(lock, fcntl.LOCK_UN)
 
 
+def _up_to_date(dig):
+    stamp = os.path.join(LIB_DIR, "build.stamp")
+    if not (os.path.exists(LIB_PATH) and os.path.exists(stamp)):
+        return False
+    with open(stamp) as f:
+        return f.read().strip() == dig
+
+
 def _build_locked(force, verbose):
     stamp = os.path.join(LIB_DIR, "build.stamp")
     dig = _digest()
-    if not force and os.path.exists(LIB_PATH) and os.path.exists(stamp) and open(stamp).read().strip() == dig:
+    if not force and _up_to_date(dig):
         if verbose:
             print("emotivoice_b200.build: up to date (sources digest %s), not recompiled" % dig[:12], flush=True)
         return LIB_PATH
@@ -80,14 +93,14 @@ def _build_locked(force, verbose):
         if verbose and out.strip():
             print(out.decode())
     cmd = [nvcc_path(), "-shared", "-o", LIB_PATH] + objs + ["-cudart", "static",
-                                                           "-gencode", "arch=compute_100a,code=sm_100a"]
+                                                           "-gencode", "arch=compute_90a,code=sm_90a"]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)
     with open(stamp, "w") as f:
         f.write(dig)
     if verbose:
-        print("emotivoice_b200.build: compiled %d sources with nvcc for sm_100a (digest %s)" % (len(objs), dig[:12]), flush=True)
+        print("emotivoice_b200.build: compiled %d sources with nvcc for sm_90a (digest %s)" % (len(objs), dig[:12]), flush=True)
     return LIB_PATH
 
 

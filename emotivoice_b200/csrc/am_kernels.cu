@@ -1,4 +1,4 @@
-// Acoustic-model kernels of the PromptTTS path (fp32, sm_100a): LayerNorm (+embedding/PE
+// Acoustic-model kernels of the PromptTTS path (fp32, sm_90a): LayerNorm (+embedding/PE
 // prologue), fused multi-head attention, conditioning gather, predictor heads, pitch/energy
 // embedding, duration scan and Gaussian upsampling.  Reference semantics are cited per kernel.
 #include "ev_common.cuh"
@@ -259,7 +259,7 @@ int launch_attention(const float* qkv, const int32_t* key_lens, float* ctx, int 
   EV_CHECK_ARG(B <= 65535 && heads <= 65535, "attention: grid too large");
   const int dk = H / heads;
   // 32-query tiles while 64-query tiles would leave SMs idle (batch 1), 64-query tiles otherwise
-  const bool small = (long long)((L + 63) / 64) * heads * B < 2 * 148;
+  const bool small = (long long)((L + 63) / 64) * heads * B < 2 * sm_count();
   if (dk == 48) return small ? launch_attention_dk<48, 32>(qkv, key_lens, ctx, B, L, H, heads, st)
                              : launch_attention_dk<48, 64>(qkv, key_lens, ctx, B, L, H, heads, st);
   if (dk == 64) return small ? launch_attention_dk<64, 32>(qkv, key_lens, ctx, B, L, H, heads, st)

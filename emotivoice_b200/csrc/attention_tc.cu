@@ -1,25 +1,24 @@
-// Multi-head self-attention on the 5th-gen tensor cores (sm_100a): S = Q K^T and O = P V are tcgen05.mma (kind::tf32, fp32
-// accumulation in TMEM), the softmax runs between two TMEM reads with thread = query row (a tcgen05.ld lane), so row maxima
-// and sums are thread-local -- no shuffles, no (L x L) tensor in memory.  Replaces encoder.py:84-109
-// (scores = q k^T / sqrt(d_k); key-padding mask; softmax; p v) for d_k = 48 (EmotiVoice: 384 / 8).
+// Multi-head self-attention on the Hopper tensor cores (sm_90a): S = Q K^T and O = P V are wgmma (tf32 operands from shared
+// memory, fp32 accumulators in registers); the softmax runs on the S accumulator fragments, so no (L x L) tensor is ever stored.
+// Replaces encoder.py:84-109 (scores = q k^T / sqrt(d_k); key-padding mask; softmax; p v) for d_k = 48 (EmotiVoice: 384 / 8).
 //
-// One CTA = 128 queries of one (batch item, head); keys are walked ONCE in tiles of 64 with a lazily rescaled online softmax:
+// One CTA = 128 queries of one (batch item, head), two consumer warpgroups of 64 query rows each; keys are walked ONCE in tiles of
+// 64 with a lazily rescaled online softmax:
 //   S_j = Q K_j^T  ->  P_j = exp(S_j / sqrt(d_k) - m), l += rowsum(P_j), O += P_j V_j
-// m is the running row maximum; it only moves (and O, l are only rescaled by exp(m_old - m_new), a TMEM load / multiply / store of
-// the row's 48 accumulator columns) when a tile's maximum exceeds it by more than 8: until then P_j <= e^8, harmless in fp32 and
-// in the relative precision of the tf32 operand.  Softmax is shift invariant, so the result is the reference's up to rounding.
-// Final: ctx = O / l.
+// m is the running row maximum; it only moves (and O, l are only rescaled by exp(m_old - m_new)) when a tile's maximum exceeds it
+// by more than 8: until then P_j <= e^8, harmless in fp32 and in the relative precision of the tf32 operand.  Softmax is shift
+// invariant, so the result is the reference's up to rounding.  Final: ctx = O / l.  A row's 64 scores of a tile are spread over
+// the four lanes of a quad (16 each): row maxima and sums take two xor-shuffles.
 //
-// Operands are staged in shared memory in the no-swizzle K-major UMMA layout of conv1d_tc.cu (element (row r, 16-byte
+// Operands are staged in shared memory in the no-swizzle K-major layout of conv1d_tc.cu (element (row r, 16-byte
 // granule g) at (g * rows_pad + r) * 16):  Q [12 granules][128 rows], K_j [12][64 rows] (B operand of S), V_j^T [16 key
 // granules][48 rows = d] (B operand of O: the loader warps transpose 4x4 blocks in registers), P_j [16 key granules][128 rows]
-// (A operand of O, written by the softmax threads: thread = row, 16 B per granule -> conflict free).
+// (A operand of O, written by each consumer warpgroup for its own 64 rows).
 // MODE 1 = 3xTF32 fp32 emulation (x = hi + lo, three MMAs per K step): the duration-critical encoder prefix and the "fp32"
 // precision; MODE 0 = one tf32 MMA per K step (operands rounded to nearest).
 //
-// Roles (288 threads): warps 0-3 softmax (warp w <-> TMEM lanes 32w..), warps 4-7 loaders, warp 8 TMEM alloc + MMA issue.
-// mbarriers: q_ready, kv_full/kv_empty[2], s_full/s_empty[2] (S is double buffered in TMEM: Q K_{j+1}^T runs under the
-// softmax of tile j), p_full/p_empty (the O rescale sits between p_empty -- P V_{j-1} has completed -- and p_full), o_full.
+// Roles (384 threads): warps 0-7 consumers (MMA issue, softmax, output), warps 8-11 loaders.  mbarriers: q_ready,
+// kv_full / kv_empty[2] (K and V^T double buffered: the loads of tile j+1 run under the MMAs and softmax of tile j).
 #include "ev_common.cuh"
 #include "tc_common.cuh"
 
@@ -29,9 +28,9 @@ namespace atc {
 using namespace tc;
 
 constexpr int BQ = 128, BKT = 64;
-constexpr int NSW = 4, NLW = 4;                  // softmax warps, loader warps
-constexpr int W_LOAD = NSW, W_MMA = NSW + NLW;
-constexpr int ATC_THREADS = (W_MMA + 1) * 32;    // 288
+constexpr int NCW = 8, NLW = 4;                  // consumer warps, loader warps
+constexpr int W_LOAD = NCW;
+constexpr int ATC_THREADS = (NCW + NLW) * 32;    // 384
 constexpr int QPAD = BQ + 1, KPAD = BKT + 1;     // rows_pad == 1 (mod 8): granule-fastest 16-byte stores are conflict free
 
 template <int DK>
@@ -54,6 +53,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const floa
   constexpr int PL = SPLIT3 ? 2 : 1;
   using S = Smem<DK>;
   constexpr int G = S::G, GK = S::GK, VPAD = S::VPAD;
+  constexpr int NS = BKT / 2, NO = DK / 2;        // accumulator registers per thread: S tile, O
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * BQ;
@@ -61,32 +61,21 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const floa
   const float* base = qkv + (size_t)b * L * ld;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_raw + 128);
   uint8_t* q_s = smem_raw + S::head;                       // [plane][G][QPAD][16]
   uint8_t* k_s = q_s + PL * S::q_plane;                    // [stage][plane][G][KPAD][16]
   uint8_t* v_s = k_s + 2 * PL * S::k_plane;                // [stage][plane][GK][VPAD][16]
   uint8_t* p_s = v_s + 2 * PL * S::v_plane;                // [plane][GK][BQ][16]
   const uint32_t bar_base = smem_u32(bars);
-  const uint32_t q_ready = bar_base, p_full = bar_base + 8, p_empty = bar_base + 16, o_full = bar_base + 24;
+  const uint32_t q_ready = bar_base;
   auto kv_full = [&](int s) { return bar_base + 32u + 8u * s; };
   auto kv_empty = [&](int s) { return bar_base + 48u + 8u * s; };
-  auto s_full = [&](int s) { return bar_base + 64u + 8u * s; };
-  auto s_empty = [&](int s) { return bar_base + 80u + 8u * s; };
 
   if (tid == 0) {
-    mbar_init(q_ready, NLW * 32); mbar_init(p_full, NSW * 32); mbar_init(p_empty, 1); mbar_init(o_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(kv_full(s), NLW * 32); mbar_init(kv_empty(s), 1); mbar_init(s_full(s), 1); mbar_init(s_empty(s), NSW * 32); }
+    mbar_init(q_ready, NLW * 32);
+    for (int s = 0; s < 2; ++s) { mbar_init(kv_full(s), NLW * 32); mbar_init(kv_empty(s), NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  constexpr uint32_t TMEM_COLS = 256;           // S0 [0,64) | S1 [64,128) | O [128, 128+DK)
-  if (warp == W_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // Programmatic dependent launch: the set-up above ran under the predecessor's tail; EVERY thread now waits for the preceding grids
   // before anything is read -- including key_lens, which in the encoder is written by validate_inputs_kernel a few launches upstream
   // (a role that decoded its tile count from stale lengths would desynchronise the pipeline).
@@ -94,97 +83,125 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const floa
   const int klen = key_lens ? min(L, key_lens[b]) : L;
   const int nkt = (klen + BKT - 1) / BKT;
 
-  if (warp < NSW) {
-    // ================================ softmax: thread = query row ================================================
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int r = warp * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
+  if (warp < NCW) {
+    // ================================ consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) ============================
+    const int wg = warp >> 2, wl = warp & 3;
+    const uint32_t wg_bar = 2u + (uint32_t)wg;            // named barrier of the warpgroup (P tile hand-over)
+    constexpr uint32_t q_lbo = QPAD * 16, k_lbo = KPAD * 16, v_lbo = VPAD * 16, p_lbo = BQ * 16;
+    const uint64_t q_desc = make_desc(smem_u32(q_s) + (uint32_t)(wg * 64) * 16u, q_lbo, 128u);
+    const uint64_t p_desc = make_desc(smem_u32(p_s) + (uint32_t)(wg * 64) * 16u, p_lbo, 128u);
+    const uint64_t k_desc0 = make_desc(0u, k_lbo, 128u), v_desc0 = make_desc(0u, v_lbo, 128u);
     const float inv_sqrt_dk = 1.0f / sqrtf((float)DK);
-    float m = -INFINITY, l = 0.f;
-    float v[64];
     constexpr float RESCALE_AT = 8.0f;
+    float sacc[NS], oacc[NO];
+#pragma unroll
+    for (int i = 0; i < NS; ++i) sacc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < NO; ++i) oacc[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};     // per fragment row (h = 0: row l/4, h = 1: row l/4 + 8); l: this thread's columns
+    mbar_wait(q_ready, 0);
     for (int j = 0; j < nkt; ++j) {
-      const int sb = j & 1;
-      mbar_wait(s_full(sb), (j >> 1) & 1);
-      tc_fence_after();
-      tmem_ld32(lane_addr + (uint32_t)(sb * BKT), 32, v);
-      tmem_ld32(lane_addr + (uint32_t)(sb * BKT + 32), 32, v + 32);
-      tc_fence_before();
-      mbar_arrive(s_empty(sb));                  // S_j is in registers: the buffer may take Q K_{j+2}^T
-      const int nvalid = min(BKT, klen - j * BKT);
-      float mt = -INFINITY;
+      const int s = j & 1;
+      mbar_wait(kv_full(s), (j >> 1) & 1);
+      // ---- S_j = Q K_j^T
+      const uint64_t k_desc = desc_advance(k_desc0, smem_u32(k_s + (size_t)s * PL * S::k_plane));
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < BKT; ++c) {
-        v[c] *= inv_sqrt_dk;
-        if (c < nvalid) mt = fmaxf(mt, v[c]);
-      }
-      mbar_wait(p_empty, ((j & 1) ^ 1));         // the MMAs of tile j-1 have read P and have finished accumulating into O
-      tc_fence_after();
-      // lazy rescale: tcgen05.ld / st are warp collectives, so the warp decides together and rows that need nothing scale by 1
-      const bool need = (j > 0) && (mt > m + RESCALE_AT);
-      if (j == 0) m = mt;
-      if (__any_sync(0xffffffffu, need)) {
-        const float f = need ? __expf(m - mt) : 1.0f;
-        if (need) { m = mt; l *= f; }
-        float o[64];
-        tmem_ld32(lane_addr + 128u, 32, o);
-        tmem_ld32(lane_addr + 160u, 16, o + 32);      // columns 32..47 (the helper zero-fills o[48..63])
-#pragma unroll
-        for (int c = 0; c < DK; ++c) o[c] *= f;
-        tmem_st32(lane_addr + 128u, o);
-        tmem_st16(lane_addr + 160u, o + 32);
-        tmem_st_wait();
-      }
-#pragma unroll
-      for (int g = 0; g < GK; ++g) {
-        float p[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int c = 4 * g + e;
-          const float x = v[c] - m;
-          p[e] = c < nvalid ? __expf(x) : 0.f;      // ex2.approx: relative error 2^-22, below the 3xTF32 product error; x <= 8
-        }
-        const float4 hi = make_float4(to_tf32(p[0]), to_tf32(p[1]), to_tf32(p[2]), to_tf32(p[3]));
-        // the denominator sums exactly what the tensor core multiplies: p (= hi + lo) in the 3xTF32 mode, the rounded hi otherwise
-        l += SPLIT3 ? (p[0] + p[1]) + (p[2] + p[3]) : (hi.x + hi.y) + (hi.z + hi.w);
-        *reinterpret_cast<float4*>(p_s + ((size_t)g * BQ + r) * 16) = hi;
+      for (int k8 = 0; k8 < G / 2; ++k8) {
+        const uint64_t a_hi = desc_advance(q_desc, (uint32_t)(2 * k8) * q_lbo);
+        const uint64_t b_hi = desc_advance(k_desc, (uint32_t)(2 * k8) * k_lbo);
         if (SPLIT3) {
-          const float4 lo = make_float4(to_tf32(p[0] - hi.x), to_tf32(p[1] - hi.y), to_tf32(p[2] - hi.z), to_tf32(p[3] - hi.w));
-          *reinterpret_cast<float4*>(p_s + S::p_plane + ((size_t)g * BQ + r) * 16) = lo;
+          wgmma_tf32_n64(sacc, desc_advance(a_hi, (uint32_t)S::q_plane), b_hi, k8 ? 1u : 0u);
+          wgmma_tf32_n64(sacc, a_hi, desc_advance(b_hi, (uint32_t)S::k_plane), 1u);
+          wgmma_tf32_n64(sacc, a_hi, b_hi, 1u);
+        } else {
+          wgmma_tf32_n64(sacc, a_hi, b_hi, k8 ? 1u : 0u);
         }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // ---- online softmax on the fragments
+      const int nvalid = min(BKT, klen - j * BKT);
+      float mt[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < NS; ++i) {
+        sacc[i] *= inv_sqrt_dk;
+        if (frag_col(i, lane) < nvalid) mt[(i >> 1) & 1] = fmaxf(mt[(i >> 1) & 1], sacc[i]);
+      }
+      float f[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mt[r] = fmaxf(mt[r], __shfl_xor_sync(0xffffffffu, mt[r], 1));
+        mt[r] = fmaxf(mt[r], __shfl_xor_sync(0xffffffffu, mt[r], 2));
+        const bool need = (j > 0) && (mt[r] > m[r] + RESCALE_AT);
+        if (j == 0) m[r] = mt[r];
+        f[r] = 1.0f;
+        if (need) { f[r] = __expf(m[r] - mt[r]); m[r] = mt[r]; l[r] *= f[r]; }
+      }
+      if (f[0] != 1.0f || f[1] != 1.0f) {
+#pragma unroll
+        for (int i = 0; i < NO; ++i) oacc[i] *= f[(i >> 1) & 1];
+      }
+      // the PV MMAs of tile j-1 of the whole warpgroup have completed (every warp passed its wait): P may be overwritten
+      bar_sync(wg_bar, 128);
+#pragma unroll
+      for (int i = 0; i < NS; i += 2) {
+        const int c = frag_col(i, lane), hr = (i >> 1) & 1;
+        const float p0 = c < nvalid ? __expf(sacc[i] - m[hr]) : 0.f;          // ex2.approx: relative error 2^-22; x <= 8
+        const float p1 = c + 1 < nvalid ? __expf(sacc[i + 1] - m[hr]) : 0.f;
+        const float2 hi = make_float2(to_tf32(p0), to_tf32(p1));
+        // the denominator sums exactly what the tensor core multiplies: p (= hi + lo) in the 3xTF32 mode, the rounded hi otherwise
+        l[hr] += SPLIT3 ? (p0 + p1) : (hi.x + hi.y);
+        const int r = wg * 64 + frag_row(i, lane, wl);
+        uint8_t* d = p_s + ((size_t)(c >> 2) * BQ + r) * 16 + (c & 3) * 4;
+        *reinterpret_cast<float2*>(d) = hi;
+        if (SPLIT3) *reinterpret_cast<float2*>(d + S::p_plane) = make_float2(to_tf32(p0 - hi.x), to_tf32(p1 - hi.y));
       }
       fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(p_full);
+      bar_sync(wg_bar, 128);           // the warpgroup's P rows are complete
+      // ---- O += P_j V_j
+      const uint64_t v_desc = desc_advance(v_desc0, smem_u32(v_s + (size_t)s * PL * S::v_plane));
+      wgmma_fence();
+#pragma unroll
+      for (int k8 = 0; k8 < GK / 2; ++k8) {
+        const uint64_t a_hi = desc_advance(p_desc, (uint32_t)(2 * k8) * p_lbo);
+        const uint64_t b_hi = desc_advance(v_desc, (uint32_t)(2 * k8) * v_lbo);
+        const uint32_t acc = (j | k8) ? 1u : 0u;
+        if (SPLIT3) {
+          wgmma_tf32_n48(oacc, desc_advance(a_hi, (uint32_t)S::p_plane), b_hi, acc);
+          wgmma_tf32_n48(oacc, a_hi, desc_advance(b_hi, (uint32_t)S::v_plane), 1u);
+          wgmma_tf32_n48(oacc, a_hi, b_hi, 1u);
+        } else {
+          wgmma_tf32_n48(oacc, a_hi, b_hi, acc);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(kv_empty(s));     // K_j and V_j have been read
     }
     // ctx = O / l   (an item without keys -- rejected by the module's input validation -- yields zeros instead of a hang)
-    float o[64];
-    if (nkt > 0) {
-      mbar_wait(o_full, 0);
-      tc_fence_after();
-      tmem_ld32(lane_addr + 128u, 32, o);
-      if (DK > 32) tmem_ld32(lane_addr + 160u, DK - 32, o + 32);
-    } else {
+    float inv[2];
 #pragma unroll
-      for (int c = 0; c < 64; ++c) o[c] = 0.f;
-      l = 1.f;
+    for (int r = 0; r < 2; ++r) {
+      float lr = l[r];
+      lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+      lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+      inv[r] = nkt > 0 ? 1.0f / lr : 0.f;
     }
-    const int row = q0 + r;
-    if (row < L) {
-      const float inv = 1.0f / l;
-      float* ob = ctx + ((size_t)b * L + row) * H + h * DK;
 #pragma unroll
-      for (int c = 0; c < DK; c += 4)
-        *reinterpret_cast<float4*>(ob + c) = make_float4(o[c] * inv, o[c + 1] * inv, o[c + 2] * inv, o[c + 3] * inv);
+    for (int i = 0; i < NO; i += 2) {
+      const int row = q0 + wg * 64 + frag_row(i, lane, wl);
+      if (row < L) {
+        const float iv = inv[(i >> 1) & 1];
+        *reinterpret_cast<float2*>(ctx + ((size_t)b * L + row) * H + h * DK + frag_col(i, lane)) = make_float2(oacc[i] * iv, oacc[i + 1] * iv);
+      }
     }
-    tc_fence_before();
-  } else if (warp < W_MMA) {
+  } else {
     // ================================ loaders =====================================================================
-    asm volatile("griddepcontrol.wait;" ::: "memory");
     const int lt = (warp - W_LOAD) * 32 + lane;        // 0..127
     // Every tile is loaded in batches of independent 16-byte loads issued back to back (memory-level parallelism: one latency
-    // per batch instead of one per element -- the first version of this loop serialised them and was loader bound), then
-    // rounded / split and stored in operand layout.
+    // per batch instead of one per element), then rounded / split and stored in operand layout.
     auto store_split = [&](uint8_t* dst, int plane_bytes, const float4& t) {
       const float4 hi = make_float4(to_tf32(t.x), to_tf32(t.y), to_tf32(t.z), to_tf32(t.w));
       *reinterpret_cast<float4*>(dst) = hi;
@@ -268,84 +285,6 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const floa
       fence_proxy_async();
       mbar_arrive(kv_full(s));
     }
-  } else {
-    // ================================ MMA issuer ===================================================================
-    // all 32 lanes run the warp-uniform control flow and the barrier waits; one elected lane issues the tcgen05 instructions
-    {
-      // instruction descriptors: D=F32, A=B=TF32, K-major, N>>3 at [17,23), M>>4 at [24,29)
-      const uint32_t idesc_s = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BKT >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-      const uint32_t idesc_o = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(DK >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-      constexpr uint32_t q_lbo = QPAD * 16, k_lbo = KPAD * 16, v_lbo = VPAD * 16, p_lbo = BQ * 16;
-      const uint64_t q_desc = make_desc(smem_u32(q_s), q_lbo, 128u), p_desc = make_desc(smem_u32(p_s), p_lbo, 128u);
-      const uint64_t k_desc0 = make_desc(0u, k_lbo, 128u), v_desc0 = make_desc(0u, v_lbo, 128u);
-      mbar_wait(q_ready, 0);
-      tc_fence_after();
-      auto issue_qk = [&](int c, bool release_kv) {       // S[c & 1] = Q K^T with the K tile in stage c & 1
-        const int s = c & 1;
-        mbar_wait(kv_full(s), (c >> 1) & 1);
-        mbar_wait(s_empty(s), ((c >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint64_t k_desc = desc_advance(k_desc0, smem_u32(k_s + (size_t)s * PL * S::k_plane));
-        const uint32_t d = tmem_base + (uint32_t)(s * BKT);
-        if (elect_one()) {
-#pragma unroll
-          for (int k8 = 0; k8 < G / 2; ++k8) {
-            const uint64_t a_hi = desc_advance(q_desc, (uint32_t)(2 * k8) * q_lbo);
-            const uint64_t b_hi = desc_advance(k_desc, (uint32_t)(2 * k8) * k_lbo);
-            if (SPLIT3) {
-              const uint64_t a_lo = desc_advance(a_hi, (uint32_t)S::q_plane);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)S::k_plane);
-              umma_tf32(d, a_lo, b_hi, idesc_s, k8 ? 1u : 0u);
-              umma_tf32(d, a_hi, b_lo, idesc_s, 1u);
-              umma_tf32(d, a_hi, b_hi, idesc_s, 1u);
-            } else {
-              umma_tf32(d, a_hi, b_hi, idesc_s, k8 ? 1u : 0u);
-            }
-          }
-          umma_commit(s_full(s));
-          if (release_kv) umma_commit(kv_empty(s));
-        }
-        __syncwarp();
-      };
-      int cnt = 0;
-      if (nkt > 0) issue_qk(cnt, false);
-      for (int j = 0; j < nkt; ++j) {
-        const int c = cnt + j, s = c & 1;
-        if (j + 1 < nkt) issue_qk(c + 1, false);          // runs under the softmax of tile j
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint64_t v_desc = desc_advance(v_desc0, smem_u32(v_s + (size_t)s * PL * S::v_plane));
-        const uint32_t d = tmem_base + 128u;
-        if (elect_one()) {
-#pragma unroll
-          for (int k8 = 0; k8 < GK / 2; ++k8) {
-            const uint64_t a_hi = desc_advance(p_desc, (uint32_t)(2 * k8) * p_lbo);
-            const uint64_t b_hi = desc_advance(v_desc, (uint32_t)(2 * k8) * v_lbo);
-            const uint32_t acc = (j | k8) ? 1u : 0u;
-            if (SPLIT3) {
-              const uint64_t a_lo = desc_advance(a_hi, (uint32_t)S::p_plane);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)S::v_plane);
-              umma_tf32(d, a_lo, b_hi, idesc_o, acc);
-              umma_tf32(d, a_hi, b_lo, idesc_o, 1u);
-              umma_tf32(d, a_hi, b_hi, idesc_o, 1u);
-            } else {
-              umma_tf32(d, a_hi, b_hi, idesc_o, acc);
-            }
-          }
-          umma_commit(p_empty);
-          umma_commit(kv_empty(s));
-          if (j == nkt - 1) umma_commit(o_full);
-        }
-        __syncwarp();
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
   }
 }
 

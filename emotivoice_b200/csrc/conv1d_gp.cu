@@ -1,25 +1,25 @@
-// HiFi-GAN convolutions on "granule-planar" activations (sm_100a): tcgen05.mma implicit GEMM whose A operand is fed by
-// bulk async copies (cp.async.bulk -> mbarrier complete_tx) instead of a register round trip, and whose epilogue stores
-// straight from the TMEM lane layout with fully coalesced 16-byte accesses -- no shared-memory transpose on either side.
+// HiFi-GAN convolutions on "granule-planar" activations (sm_90a): wgmma implicit GEMM whose A operand is fed by bulk async
+// copies (cp.async.bulk -> mbarrier complete_tx) instead of a register round trip, and whose epilogue stores straight from the
+// accumulator fragments -- no shared-memory transpose on either side.
 //
 // Layout (GP): an activation tensor (B, L, C) is stored as [b][g = C / cpg][l][cpg] with 16-byte granules
 // (cpg = 4 fp32 or 8 bf16 channels): every granule is a contiguous plane of L x 16 bytes.  That is exactly the no-swizzle
-// K-major UMMA operand layout of conv1d_tc.cu (element (row r, granule g) at (g * rows_pad + r) * 16), so
+// K-major operand layout of conv1d_tc.cu (element (row r, granule g) at (g * rows_pad + r) * 16), so
 //   * the A stage of a tile = KBG contiguous runs of `rows x 16 B`  -> KBG bulk copies issued by ONE thread, as many stages
-//     in flight as shared memory holds (the round-1 kernel had six warps doing ldg -> cvt -> st.shared, 86 % no-eligible);
+//     in flight as shared memory holds;
 //   * tap j of a dilated convolution is still the same staged tile with the descriptor start advanced by j*dil rows;
-//   * tcgen05.ld gives thread = row, registers = consecutive channels: 4 (fp32) / 8 (bf16) consecutive registers are one
-//     granule, consecutive lanes are consecutive rows -> each st.global.v4 of a warp covers 512 contiguous bytes.
+//   * an accumulator register pair is two adjacent channels of one row: one 8-byte (fp32) or 4-byte (bf16) store, and the four
+//     lanes of a quad together with the eight rows of a warp cover whole 128-byte granule runs.
 // What still has to touch the operand between the copy and the MMA -- LeakyReLU of the input, zeroing of rows outside
 // [0, len) (the convolution's zero padding and the batch-invariant contract), round-to-nearest tf32 and the hi/lo split of
 // the 3xTF32 fp32 emulation -- is an IN-PLACE pass over the staged tile by four "transform" warps: shared memory to shared
-// memory (29-cycle latency instead of a global-memory round trip), conflict-free (consecutive lanes = consecutive 16 B).
+// memory, conflict-free (consecutive lanes = consecutive 16 B).
 // HBM therefore holds plain activation values (fp32, or bf16 in the bf16 mode): residuals stay exact, one copy per tensor.
 //
-// Roles (480 threads): warps 0-7 epilogue, 8-11 transform, 12 A loader (one lane), 13 weight loader (one lane),
-// 14 TMEM allocation + MMA issue (one lane).  mbarrier pipelines: a_full (copy landed) -> a_ready (transformed) -> a_empty
-// (tcgen05.commit), b_full / b_empty, acc_full / acc_empty (two accumulator sets in TMEM: epilogue of tile i overlaps the
-// main loop of tile i+1).  Persistent CTAs, static round-robin tile order.
+// Roles (448 threads): warps 0-7 two consumer warpgroups (wgmma issue for rows [64 w, 64 w + 64) of every 128-row accumulator,
+// fp32 accumulators in registers, epilogue), 8-11 transform, 12 A loader (one lane), 13 weight loader (one lane).  mbarrier
+// pipelines: a_full (copy landed) -> a_ready (transformed) -> a_empty (every consumer warp has seen the MMAs that read the stage
+// complete), b_full / b_empty.  Persistent CTAs, static round-robin tile order.
 //
 // out[b, m*rate + n / CoutR, n % CoutR] = epi( bias[n] + sum_j sum_ci w[j][ci][n] * act_in(x[b, m + (j-(K-1)/2)*dil, ci]) )
 // rate > 1 is the polyphase form of ConvTranspose1d (packing.polyphase_pack): the GEMM's N = rate * CoutR columns are the
@@ -32,15 +32,14 @@ namespace gp {
 
 using namespace tc;
 
-constexpr int NEPI_WARPS = 8;
+constexpr int NCW = 8;                       // consumer warps (two warpgroups)
 constexpr int NTW = 4;                       // transform warps
-constexpr int W_XFORM = NEPI_WARPS;          // warps 8..11
+constexpr int W_XFORM = NCW;                 // warps 8..11
 constexpr int W_ALOAD = W_XFORM + NTW;       // 12
 constexpr int W_BLOAD = W_ALOAD + 1;         // 13
-constexpr int W_MMA = W_BLOAD + 1;           // 14
-constexpr int GP_THREADS = (W_MMA + 1) * 32; // 480
+constexpr int GP_THREADS = (W_BLOAD + 1) * 32; // 448
 constexpr int MAX_A = 8, MAX_B = 8;
-constexpr int SMEM_HEAD = 1024;              // barriers + TMEM slot
+constexpr int SMEM_HEAD = 1024;              // barriers
 constexpr int XF_UNROLL = 4;
 
 struct GPlan {
@@ -48,7 +47,7 @@ struct GPlan {
   int rows_pad;
   int a_plane_bytes, b_plane_bytes, a_stage_bytes, b_stage_bytes;
   int a_stages, b_stages;
-  int tmem_cols;
+  int acc_cols;        // MT * BN <= 2 * ACC_REGS
   int tiles_m, tiles_n, total_tiles;
   int smem_total;
 };
@@ -63,9 +62,8 @@ __host__ __device__ inline bool make_gplan(const GpConvParams& p, int mode, int 
   const int cpg = mode == 2 ? 8 : 4;     // channels per 16-byte granule of the ACTIVATIONS
   const int wcpg = mode >= 2 ? 8 : 4;    // channels per 16-byte granule of the WEIGHTS (bf16 operands: 8)
   q.kbg = kbg; q.mt = mt; q.BN = BN;
-  if (2 * mt * BN > 512) return false;
-  q.tmem_cols = 32;
-  while (q.tmem_cols < 2 * mt * BN) q.tmem_cols <<= 1;
+  if (mt * BN > 2 * ACC_REGS) return false;
+  q.acc_cols = mt * BN;
   const int rows = BM * mt + span;
   q.rows_pad = (rows + 7) / 8 * 8;
   q.a_plane_bytes = kbg * q.rows_pad * 16;
@@ -97,20 +95,21 @@ __host__ __device__ inline bool make_gplan(const GpConvParams& p, int mode, int 
 __device__ __forceinline__ float lrelu_f(float v, float slope) { return fmaxf(v, v * slope); }
 
 // MODE 0: one tf32 MMA per K step; 1: 3xTF32 fp32 emulation (hi/lo planes, three MMAs per K step); 2: bf16 operands,
-// bf16 activations in HBM (kind::f16, 8 channels per granule); 3: "bf16x3": fp32 activations in HBM, every operand split
-// into bf16 hi + lo (16 significant bits), three kind::f16 MMAs per K = 16 step -- an fp32-class result (~1e-5 relative) at
-// half the tensor-core and shared-memory cost of 3xTF32.  Accumulation is fp32 in TMEM in every mode.
+// bf16 activations in HBM (8 channels per granule); 3: "bf16x3": fp32 activations in HBM, every operand split
+// into bf16 hi + lo (16 significant bits), three bf16 MMAs per K = 16 step -- an fp32-class result (~1e-5 relative) at
+// half the tensor-core and shared-memory cost of 3xTF32.  Accumulation is fp32 in every mode.
 template <int MODE, int MT, int KBG>
 __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_constant__ GpConvParams p, const __grid_constant__ GPlan pl,
                                                                   const __grid_constant__ GpGroups gs) {
   constexpr bool SPLIT3 = (MODE == 1);     // 3xTF32: hi / lo tf32 planes
   constexpr bool BF16 = (MODE == 2);       // bf16 activations in HBM, bf16 operands
-  constexpr bool X3B = (MODE == 3);        // fp32 activations in HBM, operands split into bf16 hi + lo: three kind::f16 MMAs per K=16 step
+  constexpr bool X3B = (MODE == 3);        // fp32 activations in HBM, operands split into bf16 hi + lo: three bf16 MMAs per K=16 step
   constexpr bool OP16 = BF16 || X3B;       // the MMA operands are bf16
   constexpr int BPLANES = (SPLIT3 || X3B) ? 2 : 1;
   constexpr int CPG = BF16 ? 8 : 4;        // channels per 16-byte granule of the activations (HBM and the staged tile)
   constexpr int WCPG = OP16 ? 8 : 4;       // channels per 16-byte granule of the weights
   constexpr int KB = CPG * KBG;
+  constexpr int NA = ACC_REGS / MT;
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules (16 channels) per MMA K step");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
@@ -119,7 +118,6 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   const int BN = pl.BN;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_raw + 512);     // barriers occupy [0, 8 * 44) = 352 B
   uint8_t* a_tiles = smem_raw + SMEM_HEAD;
   uint8_t* b_tiles = a_tiles + pl.a_stages * pl.a_stage_bytes;
   const uint32_t bar_base = smem_u32(bars);
@@ -128,26 +126,16 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   auto a_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (3 * MAX_A + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (3 * MAX_A + MAX_B + s); };
-  auto acc_full = [&](int s) { return bar_base + 8u * (3 * MAX_A + 2 * MAX_B + s); };
-  auto acc_empty = [&](int s) { return bar_base + 8u * (3 * MAX_A + 2 * MAX_B + 2 + s); };
 
   if (tid == 0) {
-    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(acc_full(s), 1); mbar_init(acc_empty(s), NEPI_WARPS); }
+    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), NCW); }
+    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == W_MMA) {   // TMEM allocation by one full warp; the same warp frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(pl.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Programmatic dependent launch: harmless without the launch attribute.  With it, the next kernel in the stream may start
-  // its set-up (barriers, TMEM, first weight stages) while this grid's tail is still running; everything that touches
+  // its set-up (barriers, first weight stages) while this grid's tail is still running; everything that touches
   // activations executes griddepcontrol.wait first (returns once the preceding grid has completed and flushed).
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
@@ -167,120 +155,114 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
     len = p.lens ? min(p.L, p.lens[b] * p.lens_mul) : p.L;
   };
 
-  if (warp < NEPI_WARPS) {
-    // ============================ epilogue warps ==============================================
+  if (warp < NCW) {
+    // ============================ consumers: MMA issue + epilogue ==============================================
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int quad = warp & 3, half = warp >> 2;
-    const int nchunks = BN / 32;
+    const int wg = warp >> 2, wl = warp & 3;
     const int coutR = p.Cout / p.rate;
     const int gout = coutR / CPG;              // output granule planes per item
     const size_t Lout = (size_t)p.L * p.rate;
     const int accm = p.acc;
-    int tile_cnt = 0;
+    const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
+    // bf16x3: the two K granules of one MMA are two slots apart (hi in the even slots, lo in the odd ones), one K step = 4 slots
+    const uint64_t a_desc0 = make_desc(0u, X3B ? 2u * a_lbo : a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
+    const uint32_t a_k8 = (X3B ? 4u : 2u) * a_lbo, b_k8 = 2u * b_lbo;   // bytes per K step
+    const uint32_t a_lo_off = X3B ? a_lbo : (uint32_t)pl.a_plane_bytes;
+    float acc[MT][NA];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
+    auto release = [&](int sb, int sa) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(b_empty(sb));
+        if (sa >= 0) mbar_arrive(a_empty(sa));
+      }
+    };
+    int a_cnt = 0, b_cnt = 0;
     for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
       int gi, b, t0, n0, len;
       decode(tile, gi, b, t0, n0, len);
-      if (t0 >= len) continue;                 // padding tile: no MMA work was issued, nothing is stored (rows >= len are undefined)
-      const int buf = tile_cnt & 1;
+      if (t0 >= len) continue;                 // padding tile: no MMA work is issued, nothing is stored (rows >= len are undefined)
       const GpGroup& G = gs.g[gi];
+      const int K = G.K;
+      const uint32_t a_tap = (uint32_t)G.dil * 16u;          // bytes per tap shift
+      int prev_sb = -1, prev_sa = -1;
+      for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
+        const int sa = a_cnt % pl.a_stages;
+        const int nk8 = min(KB, p.Cin - cb * KB) / (2 * WCPG);  // MMA K steps: two 16-byte operand granules each
+        mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
+        const uint64_t a_hi0 = desc_advance(a_desc0, smem_u32(a_tiles + sa * pl.a_stage_bytes) + (uint32_t)(wg * 64) * 16u);
+        for (int j = 0; j < K; ++j, ++b_cnt) {
+          const int sb = b_cnt % pl.b_stages;
+          mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+          const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
+          const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
+          wgmma_fence();
+          for (int k8 = 0; k8 < nk8; ++k8) {
+            const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
+            const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
+            const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
+            const uint32_t first = (cb | j | k8) != 0 ? 1u : 0u;
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
+              const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
+              mma_step<MODE, NA>(BN, acc[mt], a_hi, desc_advance(a_hi, a_lo_off), b_hi, b_lo, first);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();          // the previous step's MMAs have completed: its stages may be refilled
+          if (prev_sb >= 0) release(prev_sb, prev_sa);
+          prev_sb = sb;
+          prev_sa = j == K - 1 ? sa : -1;
+        }
+      }
+      wgmma_wait<0>();
+      release(prev_sb, prev_sa);
+
+      // epilogue: register pair i, i+1 = channels n, n+1 of one row (one granule)
       const bool has_res = G.res != nullptr;
-      bool waited = false;
-#pragma unroll 1
-      for (int item = half; item < MT * nchunks; item += 2) {
-        const int mt = item / nchunks, c = (item - mt * nchunks) * 32;
-        const int row = t0 + mt * BM + quad * 32 + lane;         // this thread's GEMM row (input-resolution time step)
-        const bool ok = row < len;
-        const int n = n0 + c;                                     // first of this thread's 32 columns
-        const int phase = n / coutR, co = n - phase * coutR;
-        const size_t orow = (size_t)row * p.rate + phase;
-        // 16-byte granule q of this chunk lives at plane (co/CPG + q), row orow
-        const size_t gbase = ((size_t)b * gout + co / CPG) * Lout + orow;
-        constexpr int NG = 32 / CPG;                              // granules per 32-column chunk: 8 (fp32) / 4 (bf16)
-        uint4 rq[NG];
-        if (has_res) {
 #pragma unroll
-          for (int q = 0; q < NG; ++q) {
-            rq[q] = make_uint4(0u, 0u, 0u, 0u);
-            if (ok) rq[q] = *(reinterpret_cast<const uint4*>(G.res) + gbase + (size_t)q * Lout);
-          }
-        }
-        if (!waited) {
-          mbar_wait(acc_full(buf), (tile_cnt >> 1) & 1);
-          tc_fence_after();
-          waited = true;
-        }
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * MT * BN + mt * BN + c), 32, v);
-        if (ok) {
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int i = 0; i < NA; i += 2) {
+          const int c = frag_col(i, lane);
+          const int row = t0 + mt * BM + wg * 64 + frag_row(i, lane, wl);    // this GEMM row (input-resolution time step)
+          if (c >= BN || row >= len) continue;
+          const int n = n0 + c;
+          const int phase = n / coutR, co = n - phase * coutR;
+          const size_t e = (((size_t)b * gout + co / CPG) * Lout + (size_t)row * p.rate + phase) * CPG + (co % CPG);   // element index
+          float v0 = acc[mt][i], v1 = acc[mt][i + 1];
           if (G.bias) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 b4 = __ldg(reinterpret_cast<const float4*>(G.bias + n) + q);
-              v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
-            }
+            const float2 b2 = __ldg(reinterpret_cast<const float2*>(G.bias + n));
+            v0 += b2.x; v1 += b2.y;
           }
-          if (has_res) {
-#pragma unroll
-            for (int q = 0; q < NG; ++q) {
-              if (BF16) {
-                const uint32_t w4[4] = {rq[q].x, rq[q].y, rq[q].z, rq[q].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  v[8 * q + 2 * e] += __uint_as_float(w4[e] << 16);
-                  v[8 * q + 2 * e + 1] += __uint_as_float(w4[e] & 0xffff0000u);
-                }
-              } else {
-                v[4 * q] += __uint_as_float(rq[q].x); v[4 * q + 1] += __uint_as_float(rq[q].y);
-                v[4 * q + 2] += __uint_as_float(rq[q].z); v[4 * q + 3] += __uint_as_float(rq[q].w);
-              }
+          if (BF16) {
+            if (has_res) {
+              const uint32_t r = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.res) + e);
+              v0 += __uint_as_float(r << 16); v1 += __uint_as_float(r & 0xffff0000u);
             }
-          }
-          if (accm != EV_ACC_STORE) {     // the xs += / xs /= n accumulation of the last layer of a ResBlock (2 launches in 18): loaded late to keep
-            uint4 oq[NG];                 // the common path's register footprint small
-#pragma unroll
-            for (int q = 0; q < NG; ++q) oq[q] = *(reinterpret_cast<const uint4*>(G.out) + gbase + (size_t)q * Lout);
-#pragma unroll
-            for (int q = 0; q < NG; ++q) {
-              if (BF16) {
-                const uint32_t w4[4] = {oq[q].x, oq[q].y, oq[q].z, oq[q].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  v[8 * q + 2 * e] += __uint_as_float(w4[e] << 16);
-                  v[8 * q + 2 * e + 1] += __uint_as_float(w4[e] & 0xffff0000u);
-                }
-              } else {
-                v[4 * q] += __uint_as_float(oq[q].x); v[4 * q + 1] += __uint_as_float(oq[q].y);
-                v[4 * q + 2] += __uint_as_float(oq[q].z); v[4 * q + 3] += __uint_as_float(oq[q].w);
-              }
+            if (accm != EV_ACC_STORE) {
+              const uint32_t q = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.out) + e);
+              v0 += __uint_as_float(q << 16); v1 += __uint_as_float(q & 0xffff0000u);
+              if (accm == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
             }
-            if (accm == EV_ACC_ADD_DIV) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] /= p.div;
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(G.out) + e) = pack_bf16(v0, v1);
+          } else {
+            if (has_res) {
+              const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.res) + e);
+              v0 += r.x; v1 += r.y;
             }
-          }
-#pragma unroll
-          for (int q = 0; q < NG; ++q) {
-            uint4 o;
-            if (BF16) {
-              o.x = pack_bf16(v[8 * q], v[8 * q + 1]); o.y = pack_bf16(v[8 * q + 2], v[8 * q + 3]);
-              o.z = pack_bf16(v[8 * q + 4], v[8 * q + 5]); o.w = pack_bf16(v[8 * q + 6], v[8 * q + 7]);
-            } else {
-              o.x = __float_as_uint(v[4 * q]); o.y = __float_as_uint(v[4 * q + 1]);
-              o.z = __float_as_uint(v[4 * q + 2]); o.w = __float_as_uint(v[4 * q + 3]);
+            if (accm != EV_ACC_STORE) {
+              const float2 q = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.out) + e);
+              v0 += q.x; v1 += q.y;
+              if (accm == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
             }
-            *(reinterpret_cast<uint4*>(G.out) + gbase + (size_t)q * Lout) = o;
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(G.out) + e) = make_float2(v0, v1);
           }
         }
       }
-      if (!waited) {     // a warp without work items in this tile still follows the accumulator phases
-        mbar_wait(acc_full(buf), (tile_cnt >> 1) & 1);
-        tc_fence_after();
-      }
-      // all TMEM reads of this buffer are complete (tcgen05.wait::ld inside tmem_ld32): hand it back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty(buf));
-      ++tile_cnt;
     }
   } else if (warp < W_ALOAD) {
     // ============================ transform warps: in-place pass over the landed A stage =======================
@@ -398,7 +380,7 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp == W_BLOAD) {
+  } else {
     // ============================ weight loader (weights are constants: no dependency wait) ========================
     if (lane == 0) {
       // w layout: [plane (hi, lo)][N tile of BNp = min(Cout,128)][tap][Cin/WCPG granules][BNp][16 bytes] (fp32 or bf16 granules)
@@ -436,86 +418,6 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
       }
     }
     __syncwarp();
-  } else {
-    // ============================ MMA issuer =====================================================
-    // All 32 lanes run the (warp-uniform) control flow and the barrier waits; one elected lane issues the tcgen05 instructions.
-    {
-      const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
-      const uint32_t fmt = OP16 ? 1u : 2u;      // instruction descriptor: D=F32 [4,6)=1, A/B format [7,10) / [10,13), N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      // bf16x3: the two K granules of one MMA are two slots apart (hi in the even slots, lo in the odd ones), one K step = 4 slots
-      const uint64_t a_desc0 = make_desc(0u, X3B ? 2u * a_lbo : a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
-      const uint32_t a_k8 = (X3B ? 4u : 2u) * a_lbo, b_k8 = 2u * b_lbo;   // bytes per K step
-      const uint32_t a_lo_off = X3B ? a_lbo : (uint32_t)pl.a_plane_bytes;
-      int a_cnt = 0, b_cnt = 0, tile_cnt = 0;
-      for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
-        int gi, b, t0, n0, len;
-        decode(tile, gi, b, t0, n0, len);
-        if (t0 >= len) continue;
-        const int K = gs.g[gi].K;
-        const uint32_t a_tap = (uint32_t)gs.g[gi].dil * 16u;          // bytes per tap shift
-        const int buf = tile_cnt & 1;
-        mbar_wait(acc_empty(buf), ((tile_cnt >> 1) & 1) ^ 1);     // epilogue has drained this accumulator set
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + (uint32_t)(buf * MT * BN);
-        for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-          const int sa = a_cnt % pl.a_stages;
-          const int nk8 = min(KB, p.Cin - cb * KB) / (2 * WCPG);  // MMA K steps: two 16-byte operand granules each
-          mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
-          const uint64_t a_hi0 = desc_advance(a_desc0, smem_u32(a_tiles + sa * pl.a_stage_bytes));
-          for (int j = 0; j < K; ++j, ++b_cnt) {
-            const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
-            tc_fence_after();
-            const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
-            if (elect_one()) {
-              for (int k8 = 0; k8 < nk8; ++k8) {
-                const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
-                const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
-                const uint32_t first = (cb | j | k8) != 0 ? 1u : 0u;
-#pragma unroll
-                for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
-                  const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                  const uint32_t d = d_base + (uint32_t)(mt * BN);
-                  if (SPLIT3 || X3B) {
-                    const uint64_t a_lo = desc_advance(a_hi, a_lo_off);
-                    const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-                    if (X3B) {
-                      umma_bf16(d, a_lo, b_hi, idesc, first);     // small terms first
-                      umma_bf16(d, a_hi, b_lo, idesc, 1u);
-                      umma_bf16(d, a_hi, b_hi, idesc, 1u);
-                    } else {
-                      umma_tf32(d, a_lo, b_hi, idesc, first);
-                      umma_tf32(d, a_hi, b_lo, idesc, 1u);
-                      umma_tf32(d, a_hi, b_hi, idesc, 1u);
-                    }
-                  } else if (BF16) {
-                    umma_bf16(d, a_hi, b_hi, idesc, first);
-                  } else {
-                    umma_tf32(d, a_hi, b_hi, idesc, first);
-                  }
-                }
-              }
-              umma_commit(b_empty(sb));               // weight stage free once these MMAs have read it
-              if (j == K - 1) {
-                umma_commit(a_empty(sa));             // activation stage free
-                if (cb == n_cb - 1) umma_commit(acc_full(buf));   // accumulators of this tile complete -> epilogue
-              }
-            }
-            __syncwarp();
-          }
-        }
-        ++tile_cnt;
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(pl.tmem_cols));
   }
 }
 
@@ -769,7 +671,7 @@ static int plan_gp(const GpConvParams& p, int mode, gp::GPlan* out, int ng = 1, 
       if (cost < best * 0.97) { best = cost; best_pl = pl; found = true; }     // widest N / most accumulators first; 3 % hysteresis
     }
   }
-  if (!found) { set_error("conv1d_gp: tile does not fit in shared memory / TMEM (K=%d dil=%d Cout=%d)", p.K, p.dil, p.Cout); return EV_EINVAL; }
+  if (!found) { set_error("conv1d_gp: tile does not fit in shared memory / accumulator registers (K=%d dil=%d Cout=%d)", p.K, p.dil, p.Cout); return EV_EINVAL; }
   *out = best_pl;
   return EV_OK;
 }
@@ -784,7 +686,7 @@ int debug_gp_plan(const GpConvParams& p, int mode, int* v) {
   const int rc = plan_gp(p, mode, &pl);
   if (rc != EV_OK) return rc;
   v[0] = pl.BN; v[1] = pl.mt; v[2] = pl.kbg; v[3] = pl.a_stages; v[4] = pl.b_stages; v[5] = gp::NTW;
-  v[6] = pl.planes; v[7] = pl.tmem_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
+  v[6] = pl.planes; v[7] = pl.acc_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
   return EV_OK;
 }
 
@@ -860,7 +762,7 @@ int debug_gp_group_plan(const GpConvParams* ps, int n, int mode, int* v) {
   gp::GPlan pl;
   EV_TRY(plan_group(ps, n, mode, &gs, &pl));
   v[0] = pl.BN; v[1] = pl.mt; v[2] = pl.kbg; v[3] = pl.a_stages; v[4] = pl.b_stages; v[5] = gp::NTW;
-  v[6] = pl.planes; v[7] = pl.tmem_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
+  v[6] = pl.planes; v[7] = pl.acc_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
   return EV_OK;
 }
 int launch_conv1d_gp_group(const GpConvParams* ps, int n, int mode, cudaStream_t st) {

@@ -1,15 +1,14 @@
-// Time-major 1-D convolution as an implicit GEMM on the 5th-gen tensor cores (sm_100a):
-// tcgen05.mma (kind::tf32, fp32 accumulate in TMEM), operands staged in shared memory, weights
-// streamed by bulk async copies (cp.async.bulk -> mbarrier complete_tx), accumulators read back
-// with tcgen05.ld by dedicated epilogue warps.  Same contract as conv1d_tm.cu (see ev_common.cuh):
+// Time-major 1-D convolution as an implicit GEMM on the Hopper tensor cores (sm_90a):
+// wgmma (tf32 or bf16 operands from shared memory, fp32 accumulators in registers), weights streamed
+// by bulk async copies (cp.async.bulk -> mbarrier complete_tx).  Same contract as conv1d_tm.cu (see ev_common.cuh):
 //
 //   out[b,t,co] = epi( bias[co] + sum_j sum_ci w[j][ci][co] * act_in( x[b, t + (j-(K-1)/2)*dil, ci] ) )
 //
-// GEMM view: M = time (128 rows per accumulator, MT accumulators per tile), N = C_out tile (<= 128),
+// GEMM view: M = time (128 rows per accumulator tile, MT tiles per CTA tile), N = C_out tile (<= 128),
 // K = taps x C_in.
 //
 // * ONE activation fetch per tile for all k taps: the A operand lives in shared memory in the
-//   no-swizzle K-major UMMA layout with the 8-row-group stride (SBO) set to 128 B, i.e. element
+//   no-swizzle K-major layout with the 8-row-group stride (SBO) set to 128 B, i.e. element
 //   (row r, 16-byte K-granule g) sits at  A + (g * rows_pad + r) * 16 bytes.  Consecutive rows are
 //   16 B apart for the whole tile, so tap j of a dilated convolution is the same staged tile with the
 //   descriptor start address advanced by j*dil rows, and accumulator mt by 128*mt rows.  The producer
@@ -17,14 +16,13 @@
 //   hi-lo split and the layout change while staging, so activations stay plain fp32 time-major in HBM
 //   and no tensor map is needed.
 // * One weight tile from L2 feeds MT accumulators (MT x fewer weight bytes per output row).
-// * Persistent CTAs (one per SM) loop over tiles; the accumulators are double buffered in TMEM so
-//   the epilogue of tile i (TMEM -> registers -> swizzled smem -> fully coalesced 128-byte global
-//   rows, residual/accumulate operands prefetched) overlaps the main loop of tile i+1.
+// * Persistent CTAs (one per SM) loop over tiles.
 //
-// Roles (512 threads): warps 0-7 epilogue (warp e <-> TMEM lanes 32(e%4).., alternate 32-column
-// chunks), warps 8-13 stage A, warp 14 allocates TMEM and its elected lane issues every tcgen05.mma,
-// warp 15's elected lane streams the weight tiles.  mbarrier pipelines: A ring (a_full/a_empty), B ring (b_full/b_empty,
-// released by tcgen05.commit), accumulators (acc_full/acc_empty).
+// Roles (480 threads): warps 0-7 are two consumer warpgroups: warpgroup w issues the wgmma for rows [64 w, 64 w + 64) of every
+// 128-row accumulator, keeps those accumulators in registers and stores them; warps 8-13 stage A; warp 14's first lane streams
+// the weight tiles.  mbarrier pipelines: A ring (a_full/a_empty), B ring (b_full/b_empty); a consumer warp releases a stage once
+// wgmma.wait_group has seen the MMAs that read it complete (one step behind the issue, so the tensor core always has the next
+// step queued).
 #include <cstdio>
 #include <cstdlib>
 
@@ -43,12 +41,12 @@ struct Plan {
   int ngroups;         // producer groups: largest of {6,3,2,1} that is <= a_stages
   int ksplit;          // K-split factor S: S CTAs share one output tile, each reducing a slice of the C_in blocks
                        // into a private partial buffer; splitk_reduce_kernel sums them in a fixed order
-  int tmem_cols;
+  int acc_cols;        // accumulator columns per consumer thread's 64-row slices: MT * BN <= 2 * ACC_REGS
   int tiles_m, tiles_n, total_tiles;
   int smem_total;
 };
 
-// smem map: [0,288) barriers | [512,516) tmem base | 1024: epilogue staging (8 warps x 4 KB) | A ring | B ring
+// smem map: [0,256) barriers | 1024: A ring | B ring
 __host__ __device__ inline bool make_plan(const ConvParams& p, int mode, int BN, int mt, int kbg, int min_b_stages, Plan* o, int b_target = 4) {
   Plan q;
   q.planes = (mode == 1 || mode == 3) ? 2 : 1;
@@ -56,16 +54,15 @@ __host__ __device__ inline bool make_plan(const ConvParams& p, int mode, int BN,
   q.kbg = kbg;
   q.mt = mt;
   q.BN = BN;
-  if (2 * mt * q.BN > 512) return false;
-  q.tmem_cols = 32;
-  while (q.tmem_cols < 2 * mt * q.BN) q.tmem_cols <<= 1;
+  if (mt * q.BN > 2 * ACC_REGS) return false;
+  q.acc_cols = mt * q.BN;
   const int rows = BM * mt + (p.K - 1) * p.dil;
   q.rows_pad = ((rows + 7) / 8) * 8 + 8 / q.kbg;
   q.a_plane_bytes = q.kbg * q.rows_pad * 16;
   q.b_plane_bytes = q.kbg * q.BN * 16;
   q.a_stage_bytes = q.planes * q.a_plane_bytes;
   q.b_stage_bytes = q.planes * q.b_plane_bytes;
-  const int budget = 227 * 1024 - 1024 - STAGING_BYTES;
+  const int budget = 227 * 1024 - 1024;
   const int n_cb = (p.Cin + cpg * q.kbg - 1) / (cpg * q.kbg);
   // at least 2 + 2 stages; then grow the weight ring first (it turns over K times per A stage)
   if (min_b_stages > n_cb * p.K) min_b_stages = n_cb * p.K;
@@ -86,7 +83,7 @@ __host__ __device__ inline bool make_plan(const ConvParams& p, int mode, int BN,
   q.tiles_n = (p.Cout + q.BN - 1) / q.BN;
   q.ksplit = 1;
   q.total_tiles = p.B * q.tiles_m * q.tiles_n;
-  q.smem_total = 1024 + STAGING_BYTES + q.a_stages * q.a_stage_bytes + q.b_stages * q.b_stage_bytes;
+  q.smem_total = 1024 + q.a_stages * q.a_stage_bytes + q.b_stages * q.b_stage_bytes;
   *o = q;
   return true;
 }
@@ -122,25 +119,25 @@ __device__ __forceinline__ void splitk_reduce_store(const ConvParams& p, int S, 
 }
 
 // MODE 0: one tf32 MMA per K step (operands rounded to nearest tf32).
-// MODE 2: bf16 operands (rounded to nearest even by the producers / the host), kind::f16, 8 channels per granule.
-// MODE 3: "bf16x3" fp32-class emulation: x = hi + lo with hi = bf16(x), lo = bf16(x - hi) (16 significant bits), three kind::f16 MMAs per
-//                 K = 16 step (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi): ~1e-5 relative at half the tensor-core / weight-stream cost of 3xTF32.
-// MODE 1: "3xTF32" fp32 emulation: x = hi + lo with hi = tf32(x), lo = tf32(x - hi);
-//                 a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the dropped lo*lo term is 2^-22 relative),
-//                 three MMAs per K step into the same fp32 TMEM accumulator.  Weights arrive pre-split
-//                 (two planes, packing.to_tc_layout); activations are split by the producer warps.
-// MT: 128-row accumulators per tile.  KBG: 16-byte K granules (4 tf32 or 8 bf16 channels each) per pipeline stage.
+// MODE 2: bf16 operands (rounded to nearest even by the producers / the host), 8 channels per granule.
+// MODE 3: "bf16x3" fp32-class emulation: x = hi + lo with hi = bf16(x), lo = bf16(x - hi) (16 significant bits), three bf16 MMAs per
+//                 K = 16 step: ~1e-5 relative at half the tensor-core / weight-stream cost of 3xTF32.
+// MODE 1: "3xTF32" fp32 emulation: x = hi + lo with hi = tf32(x), lo = tf32(x - hi), three MMAs per K step into the same fp32
+//                 accumulator.  Weights arrive pre-split (two planes, packing.to_tc_layout); activations are split by the producer warps.
+// MT: 128-row accumulator tiles per CTA tile.  KBG: 16-byte K granules (4 tf32 or 8 bf16 channels each) per pipeline stage.
 // PDLM: programmatic dependent launch mode (EV_PDL): 0 = plain launch (no extra instructions),
 //       1 = convolutions only, 2 = every kernel of the engine launches this way (see the note after the set-up below).
 template <int MODE, int MT, int KBG, int PDLM>
 __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Plan pl) {
   constexpr bool SPLIT3 = (MODE == 1);
-  constexpr bool X3B = (MODE == 3);       // "bf16x3": fp32 operands split into bf16 hi + lo planes, three kind::f16 MMAs per K = 16 step
+  constexpr bool X3B = (MODE == 3);       // "bf16x3": fp32 operands split into bf16 hi + lo planes, three bf16 MMAs per K = 16 step
   constexpr bool BF16 = (MODE == 2) || X3B;      // the staged operands are bf16 (8 channels per granule)
   constexpr int PLANES = (SPLIT3 || X3B) ? 2 : 1;
   constexpr int CPG = BF16 ? 8 : 4;       // channels per 16-byte granule
   constexpr int KB = CPG * KBG;
   constexpr int GSH = (KBG == 8 ? 3 : 2);
+  constexpr int NA = ACC_REGS / MT;       // accumulator registers per 128-row tile
+  constexpr int NCW = NCONS / 32;         // consumer warps: every one of them releases each stage
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
@@ -148,43 +145,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
   const int BN = pl.BN;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_raw + 512);   // barriers occupy [0, 8*(2*MAX_A+2*MAX_B+4)) = 288 B
-  uint8_t* staging = smem_raw + 1024;
-  uint8_t* a_tiles = staging + STAGING_BYTES;
+  uint8_t* a_tiles = smem_raw + 1024;
   uint8_t* b_tiles = a_tiles + pl.a_stages * pl.a_stage_bytes;
   const uint32_t bar_base = smem_u32(bars);
   auto a_full = [&](int s) { return bar_base + 8u * s; };
   auto a_empty = [&](int s) { return bar_base + 8u * (MAX_A_STAGES + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (2 * MAX_A_STAGES + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A_STAGES + MAX_B_STAGES + s); };
-  auto acc_full = [&](int s) { return bar_base + 8u * (2 * MAX_A_STAGES + 2 * MAX_B_STAGES + s); };
-  auto acc_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A_STAGES + 2 * MAX_B_STAGES + 2 + s); };
 
   if (tid == 0) {
-    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), (NPWARPS / pl.ngroups) * 32); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(acc_full(s), 1); mbar_init(acc_empty(s), NEPI / 32); }
+    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), (NPWARPS / pl.ngroups) * 32); mbar_init(a_empty(s), NCW); }
+    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {   // TMEM allocation by one full warp; the same warp frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(pl.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Programmatic dependent launch (EV_PDL, default 2).  The grid is persistent (<= one CTA per SM, all resident), so it lets
-  // the NEXT launch in the stream start as soon as SMs free up: that kernel's CTAs run their set-up (barriers, TMEM) while
-  // this grid's tail is still running.  Everything that touches activations (producers: x; epilogue: res / out / split-K
+  // the NEXT launch in the stream start as soon as SMs free up: that kernel's CTAs run their set-up (barriers) while
+  // this grid's tail is still running.  Everything that touches activations (producers: x; consumers: res / out / split-K
   // partials) first executes griddepcontrol.wait, which returns once the preceding grid has completed and its writes are
   // visible.  PDLM == 1 (only the convolutions launch this way, so the launch before a convolution's predecessor has fully
-  // completed): the loader and the MMA issuer, which read only weights and p.lens, do not wait and the first weight stages
+  // completed): the weight loader, which reads only weights and p.lens, does not wait and the first weight stages
   // are prefetched under the predecessor's tail.  PDLM == 2 (every kernel launches this way): p.lens may come from a grid that
   // is still running TWO launches upstream (validate_inputs_kernel writes the int32 lengths, LayerNorm starts early and waits,
   // this kernel starts early too) -- a role that decoded tiles from stale lengths would walk a different tile sequence than
-  // the others and the pipeline would deadlock (seen once: a bench run whose batches had different lengths hung).  Every role waits.
+  // the others and the pipeline would deadlock.  Every role waits.
   if (PDLM) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   const int n_cb = (p.Cin + KB - 1) / KB;
@@ -206,107 +191,106 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
     len = p.lens ? min(p.L, p.lens[b] * p.lens_mul) : p.L;
   };
 
-  if (warp < NEPI / 32) {
-    // ============================ epilogue warps ==============================================
+  if (warp < NCW) {
+    // ============================ consumers: MMA issue + epilogue ==================================
     if (PDLM) asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int quad = warp & 3, chalf = warp >> 2;
-    float* stg = reinterpret_cast<float*>(staging + warp * (32 * 32 * 4));
-    const int rr = lane >> 3, cq = lane & 7;         // coalesced phase: 4 rows x 8 float4 per instruction
+    const int wg = warp >> 2, wl = warp & 3;
     const bool split = pl.ksplit > 1;           // K-split: raw partial sums, the fused epilogue runs in the reduce kernel
     const bool has_res = p.res != nullptr && !split;
     const int oact = split ? EV_ACT_NONE : p.out_act, accm = split ? EV_ACC_STORE : p.acc;
-    int tile_cnt = 0;
+    const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
+    const uint64_t a_desc0 = make_desc(0u, a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
+    const uint32_t a_tap = (uint32_t)p.dil * 16u, a_k8 = 2u * a_lbo, b_k8 = 2u * b_lbo;
+    float acc[MT][NA];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
+    auto release = [&](int sb, int sa) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(b_empty(sb));
+        if (sa >= 0) mbar_arrive(a_empty(sa));
+      }
+    };
+    int a_cnt = 0, b_cnt = 0;
     for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
       int b, t0, n0, nt, len;
       decode(tile, b, t0, n0, nt, len);
       float* ob = (split ? p.splitk_ws + (size_t)z_cur * p.B * p.L * p.Cout : p.out) + (size_t)b * p.L * p.Cout;   // may alias p.res
       const float* rb = has_res ? p.res + (size_t)b * p.L * p.Cout : nullptr;
-      if (t0 >= len) {   // padding tile: the batch-invariant contract stores zeros (no MMA work was issued)
-        for (int mt = 0; mt < MT; ++mt)
-          for (int c = chalf * 32; c < nt; c += 64)
-            for (int it = 0; it < 8; ++it) {
-              const int row = t0 + mt * BM + quad * 32 + it * 4 + rr;
-              if (row < p.L && c + cq * 4 < nt)
-                *reinterpret_cast<float4*>(ob + (size_t)row * p.Cout + n0 + c + cq * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      const bool active = t0 < len;      // padding tile: the batch-invariant contract stores zeros (no MMA work is issued)
+      if (active) {
+        const int cb_lo = (z_cur * n_cb) / pl.ksplit, cb_hi = ((z_cur + 1) * n_cb) / pl.ksplit;
+        int prev_sb = -1, prev_sa = -1;
+        for (int cb = cb_lo; cb < cb_hi; ++cb, ++a_cnt) {
+          const int sa = a_cnt % pl.a_stages;
+          const int nk8 = min(KB, p.Cin - cb * KB) / (2 * CPG);   // MMA K steps: two 16-byte granules each
+          mbar_wait(a_full(sa), (a_cnt / pl.a_stages) & 1);
+          const uint64_t a_hi0 = desc_advance(a_desc0, smem_u32(a_tiles + sa * pl.a_stage_bytes) + (uint32_t)(wg * 64) * 16u);
+          for (int j = 0; j < p.K; ++j, ++b_cnt) {
+            const int sb = b_cnt % pl.b_stages;
+            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+            const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
+            const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
+            wgmma_fence();
+            for (int k8 = 0; k8 < nk8; ++k8) {
+              const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
+              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
+              const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
+              const uint32_t first = ((cb - cb_lo) | j | k8) != 0 ? 1u : 0u;
+#pragma unroll
+              for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
+                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
+                mma_step<MODE, NA>(nt, acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a_plane_bytes), b_hi, b_lo, first);
+              }
             }
-        continue;
+            wgmma_commit();
+            wgmma_wait<1>();          // the previous step's MMAs have completed: its stages may be refilled
+            if (prev_sb >= 0) release(prev_sb, prev_sa);
+            prev_sb = sb;
+            prev_sa = j == p.K - 1 ? sa : -1;
+          }
+        }
+        wgmma_wait<0>();
+        release(prev_sb, prev_sa);
       }
-      const int buf = tile_cnt & 1;
+      // epilogue straight from the accumulator fragments: two adjacent columns per register pair (8-byte accesses)
       const float* __restrict__ bias = (p.bias && !split) ? p.bias + (size_t)b * p.bias_bs + n0 : nullptr;
-      bool waited = false;
-#pragma unroll 1
+#pragma unroll
       for (int mt = 0; mt < MT; ++mt) {
-        const int row_base = t0 + mt * BM + quad * 32;
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * MT * BN + mt * BN);
-#pragma unroll 1
-        for (int c = chalf * 32; c < nt; c += 64) {
-          const int cw = min(32, nt - c);
-          const bool col_ok = cq * 4 < cw;
-          // residual / accumulate operands and the bias: coalesced loads issued before the accumulator is needed
-          float4 rq[8], oq[8];
 #pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int row = row_base + it * 4 + rr;
-            const size_t off = (size_t)row * p.Cout + n0 + c + cq * 4;
-            rq[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (has_res && col_ok && row < len) rq[it] = *reinterpret_cast<const float4*>(rb + off);
+        for (int i = 0; i < NA; i += 2) {
+          const int c = frag_col(i, lane);
+          const int row = t0 + mt * BM + wg * 64 + frag_row(i, lane, wl);
+          if (c >= nt || row >= p.L) continue;
+          const size_t off = (size_t)row * p.Cout + n0 + c;
+          float2 o = make_float2(0.f, 0.f);
+          if (active && row < len) {
+            o = make_float2(acc[mt][i], acc[mt][i + 1]);
+            if (bias) {
+              const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + c));
+              o.x += b2.x; o.y += b2.y;
+            }
+            if (oact != EV_ACT_NONE) { o.x = act_apply(o.x, oact, 0.f); o.y = act_apply(o.y, oact, 0.f); }
+            if (has_res) {
+              const float2 r2 = *reinterpret_cast<const float2*>(rb + off);
+              o.x += r2.x; o.y += r2.y;
+            }
             if (accm != EV_ACC_STORE) {
-              oq[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (col_ok && row < len) oq[it] = *reinterpret_cast<const float4*>(ob + off);
+              const float2 q2 = *reinterpret_cast<const float2*>(ob + off);
+              o.x += q2.x; o.y += q2.y;
+              if (accm == EV_ACC_ADD_DIV) { o.x /= p.div; o.y /= p.div; }
             }
           }
-          float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (bias && col_ok) b4 = __ldg(reinterpret_cast<const float4*>(bias + c + cq * 4));
-          if (!waited) {
-            mbar_wait(acc_full(buf), (tile_cnt >> 1) & 1);
-            tc_fence_after();
-            waited = true;
-          }
-          float v[32];
-          tmem_ld32(taddr + (uint32_t)c, cw, v);      // thread = row (TMEM lane), 32 consecutive columns
-          // registers -> smem, 16-byte chunks XOR-swizzled by the row so both phases are conflict free
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(stg + lane * 32 + ((q ^ (lane & 7)) << 2)) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int r = it * 4 + rr;
-            const int row = row_base + r;
-            float4 o = *reinterpret_cast<const float4*>(stg + r * 32 + ((cq ^ (r & 7)) << 2));
-            if (row < len) {
-              o.x += b4.x; o.y += b4.y; o.z += b4.z; o.w += b4.w;
-              if (oact != EV_ACT_NONE) {
-                o.x = act_apply(o.x, oact, 0.f); o.y = act_apply(o.y, oact, 0.f);
-                o.z = act_apply(o.z, oact, 0.f); o.w = act_apply(o.w, oact, 0.f);
-              }
-              o.x += rq[it].x; o.y += rq[it].y; o.z += rq[it].z; o.w += rq[it].w;
-              if (accm != EV_ACC_STORE) {
-                o.x += oq[it].x; o.y += oq[it].y; o.z += oq[it].z; o.w += oq[it].w;
-                if (accm == EV_ACC_ADD_DIV) { o.x /= p.div; o.y /= p.div; o.z /= p.div; o.w /= p.div; }
-              }
-            } else {
-              o = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            if (col_ok && row < p.L) *reinterpret_cast<float4*>(ob + (size_t)row * p.Cout + n0 + c + cq * 4) = o;
-          }
-          __syncwarp();
+          *reinterpret_cast<float2*>(ob + off) = o;
         }
       }
-      if (!waited) {     // a warp without columns in this tile (N <= 32) still follows the accumulator phases
-        mbar_wait(acc_full(buf), (tile_cnt >> 1) & 1);
-        tc_fence_after();
-      }
-      // all TMEM reads of this buffer are complete (tcgen05.wait::ld inside tmem_ld32): hand it back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty(buf));
-      ++tile_cnt;
     }
-  } else if (warp < MMA_WARP) {
+  } else if (warp < W_WLOAD) {
     // ============================ A producers ===================================================
     if (PDLM) asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int pwarp = warp - NEPI / 32;
+    const int pwarp = warp - NCW;
     const int wpg = NPWARPS / pl.ngroups;          // warps per group
     const int grp = pwarp / wpg;
     const int gt = (pwarp - grp * wpg) * 32 + lane;  // thread index inside the group
@@ -391,81 +375,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
         mbar_arrive(a_full(s));
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ============================ MMA issuer =====================================================
-    // All 32 lanes run the (warp-uniform) control flow and the barrier waits; one elected lane issues the tcgen05 instructions
-    // (descriptors stay in uniform registers: no vote loop / R2UR per MMA, see tc_common.cuh: elect_one).
-    {
-      if (PDLM == 2) asm volatile("griddepcontrol.wait;" ::: "memory");      // p.lens (see the note after the set-up)
-      const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
-      const uint64_t a_desc0 = make_desc(0u, a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
-      const uint32_t a_tap = (uint32_t)p.dil * 16u, a_k8 = 2u * a_lbo, b_k8 = 2u * b_lbo;
-      int a_cnt = 0, b_cnt = 0, tile_cnt = 0;
-      for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
-        int b, t0, n0, nt, len;
-        decode(tile, b, t0, n0, nt, len);
-        if (t0 >= len) continue;
-        // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32 [10,13)=2,
-        // A/B K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-        // (bf16 mode: A = B = BF16, format code 1)
-        const uint32_t fmt = BF16 ? 1u : 2u;
-        const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(nt >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const int buf = tile_cnt & 1;
-        mbar_wait(acc_empty(buf), ((tile_cnt >> 1) & 1) ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + (uint32_t)(buf * MT * BN);
-        const int cb_lo = (z_cur * n_cb) / pl.ksplit, cb_hi = ((z_cur + 1) * n_cb) / pl.ksplit;
-        for (int cb = cb_lo; cb < cb_hi; ++cb, ++a_cnt) {
-          const int sa = a_cnt % pl.a_stages;
-          const int nk8 = min(KB, p.Cin - cb * KB) / (2 * CPG);   // MMA K steps: two 16-byte granules each
-          mbar_wait(a_full(sa), (a_cnt / pl.a_stages) & 1);
-          const uint64_t a_hi0 = desc_advance(a_desc0, smem_u32(a_tiles + sa * pl.a_stage_bytes));
-          for (int j = 0; j < p.K; ++j, ++b_cnt) {
-            const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
-            tc_fence_after();
-            const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
-            if (elect_one()) {
-              for (int k8 = 0; k8 < nk8; ++k8) {
-                const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
-                const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
-                const uint32_t first = ((cb - cb_lo) | j | k8) != 0 ? 1u : 0u;
-#pragma unroll
-                for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
-                  const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                  const uint32_t d = d_base + (uint32_t)(mt * BN);
-                  if (SPLIT3) {
-                    const uint64_t a_lo = desc_advance(a_hi, (uint32_t)pl.a_plane_bytes);
-                    const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-                    umma_tf32(d, a_lo, b_hi, idesc, first);     // small terms first
-                    umma_tf32(d, a_hi, b_lo, idesc, 1u);
-                    umma_tf32(d, a_hi, b_hi, idesc, 1u);
-                  } else if (X3B) {
-                    const uint64_t a_lo = desc_advance(a_hi, (uint32_t)pl.a_plane_bytes);
-                    const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-                    umma_bf16(d, a_lo, b_hi, idesc, first);
-                    umma_bf16(d, a_hi, b_lo, idesc, 1u);
-                    umma_bf16(d, a_hi, b_hi, idesc, 1u);
-                  } else if (BF16) {
-                    umma_bf16(d, a_hi, b_hi, idesc, first);
-                  } else {
-                    umma_tf32(d, a_hi, b_hi, idesc, first);
-                  }
-                }
-              }
-              umma_commit(b_empty(sb));     // weight stage free once these MMAs have read it
-              if (j == p.K - 1) {
-                umma_commit(a_empty(sa));   // activation stage free
-                if (cb == cb_hi - 1) umma_commit(acc_full(buf));       // accumulators of this tile complete -> epilogue
-              }
-            }
-            __syncwarp();
-          }
-        }
-        ++tile_cnt;
-      }
-    }
   } else {
     // ============================ weight loader ==================================================
     if (lane == 0) {
@@ -506,13 +415,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
       }
     }
     __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(pl.tmem_cols));
   }
 }
 
@@ -635,7 +537,7 @@ static int plan_conv1d_tc(const ConvParams& p, int mode, tc::Plan* out) {
   //    launches with a handful of tiles (measured: finer N splitting costs more in per-granule copies and
   //    replicated A staging than it gains in parallelism).
   //  * rows per tile: as many 128-row accumulators as still leave about one tile per SM (every weight tile
-  //    fetched from L2 then feeds MT MMAs), limited by TMEM (2 x MT x BN <= 512 columns) and smem.
+  //    fetched from L2 then feeds MT MMAs), limited by the accumulator registers (MT x BN <= 128) and smem.
   static const int bn_thresh = env_int("EV_TC_BN_TILES", 24);     // tuning knobs (tile shape only: results are unaffected)
   static const int mt_thresh = env_int("EV_TC_MT_TILES", 120);
   const long long tiles128 = (long long)((p.L + tc::BM - 1) / tc::BM) * p.B;
@@ -647,7 +549,7 @@ static int plan_conv1d_tc(const ConvParams& p, int mode, tc::Plan* out) {
   for (;; mt >>= 1) {
     if (tc::make_plan(p, mode, BN, mt, kbg, 4, &pl)) break;
     if (tc::make_plan(p, mode, BN, mt, kbg, 2, &pl)) break;
-    if (mt == 1) { set_error("conv1d_tc: tile does not fit in shared memory / TMEM (K=%d dil=%d Cout=%d)", p.K, p.dil, p.Cout); return EV_EINVAL; }
+    if (mt == 1) { set_error("conv1d_tc: tile does not fit in shared memory / accumulator registers (K=%d dil=%d Cout=%d)", p.K, p.dil, p.Cout); return EV_EINVAL; }
   }
   EV_TRY(apply_ksplit(p, mode, &pl));
   *out = pl;
@@ -659,7 +561,7 @@ int debug_tc_plan(const ConvParams& p, int mode, int* v) {
   const int rc = plan_conv1d_tc(p, mode, &pl);
   if (rc != EV_OK) return rc;
   v[0] = pl.BN; v[1] = pl.mt; v[2] = pl.kbg; v[3] = pl.a_stages; v[4] = pl.b_stages; v[5] = pl.ngroups;
-  v[6] = pl.ksplit; v[7] = pl.tmem_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
+  v[6] = pl.ksplit; v[7] = pl.acc_cols; v[8] = pl.smem_total; v[9] = pl.total_tiles; v[10] = pl.rows_pad;
   return EV_OK;
 }
 

@@ -1,4 +1,4 @@
-// Generic time-major 1-D convolution as an implicit GEMM, fp32 FFMA path (sm_100a).
+// Generic time-major 1-D convolution as an implicit GEMM, fp32 FFMA path (sm_90a).
 //
 //   out[b,t,co] = epi( bias[co] + sum_j sum_ci w[j][ci][co] * act_in( x[b, t + (j-(K-1)/2)*dil, ci] ) )
 //
@@ -244,10 +244,10 @@ int launch_conv1d(const ConvParams& p, cudaStream_t st) {
   if (p.Cout <= 32) return launch_variant<8, 1, 8>(p, st);
   const long long tiles_big = (long long)((p.L + 127) / 128) * ((p.Cout + 127) / 128) * p.B;
   if (p.Cout <= 64) {
-    if ((long long)((p.L + 127) / 128) * p.B < 148) return launch_variant<16, 1, 4>(p, st);
+    if ((long long)((p.L + 127) / 128) * p.B < sm_count()) return launch_variant<16, 1, 4>(p, st);
     return launch_variant<16, 1, 8>(p, st);
   }
-  if (tiles_big < 148) return launch_variant<16, 1, 4>(p, st);
+  if (tiles_big < sm_count()) return launch_variant<16, 1, 4>(p, st);
   return launch_variant<16, 2, 8>(p, st);
 }
 

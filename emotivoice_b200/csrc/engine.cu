@@ -1,5 +1,5 @@
 // libemotivoice_b200.so -- context, weight binding, layer orchestration and the C ABI
-// (include/emotivoice_b200.h).  All math runs in the hand-written sm_100a kernels of
+// (include/emotivoice_b200.h).  All math runs in the hand-written sm_90a kernels of
 // conv1d_tm.cu / am_kernels.cu / voc_kernels.cu; this file only sequences launches on the
 // caller's stream and carves the caller-provided workspace.
 #include <atomic>
@@ -51,7 +51,7 @@ int sm_count() {
   int n = cache[dev & 63].load(std::memory_order_relaxed);
   if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
     cache[dev & 63].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -493,7 +493,7 @@ static bool try_gp_pair(int mode, const ConvW& c1, const ConvW& c2, const void* 
 
 // One HiFi-GAN stage's ResBlocks (hifigan/models.py:120-126) with the three parallel blocks advancing together: the same-index
 // convolutions of the blocks (different taps / dilations / weights, one shape) are ONE launch.  Used while a single convolution has
-// fewer than two waves of tiles (batch 1: 68 / 135 tiles on 148 SMs); every tile is computed as in the ungrouped launches, so the
+// fewer than two waves of tiles (batch 1: 68 / 135 tiles on 132 SMs); every tile is computed as in the ungrouped launches, so the
 // result is bitwise the same.  The last c2 of each block accumulates into xs in block order (three plain launches).
 // Returns false (nothing launched) when the stage does not qualify.
 static bool try_grouped_stage(ev_ctx* ctx, const VocBufs& v, int mode, size_t rb0, int B, int L, int C, const int32_t* lens, int mul, cudaStream_t st, int* rc) {
@@ -631,7 +631,7 @@ static int run_stack(const ev_ctx* c, const StackW& s, float* x, float* y, float
     g_split_ws.ksplit = sp.qkv;
     EV_TRY(conv_x(mode, l.wqkv_tc, l.wqkv_h, y, l.wqkv, l.bqkv, 0, nullptr, qkv, B, L, H, 3 * H, 1, 1, conv_lens, 1, EV_ACT_NONE, 0.f,
                   EV_ACT_NONE, EV_ACC_STORE, 1.f, st, l.wqkv_x2));
-    // QK^T / softmax / PV: tcgen05 (3xTF32 where the layer runs fp32-accurate, one tf32 MMA otherwise) for d_k = 48; the fp32 FFMA
+    // QK^T / softmax / PV: tensor cores (3xTF32 where the layer runs fp32-accurate, one tf32 MMA otherwise) for d_k = 48; the fp32 FFMA
     // flash kernel in the "fp32_ffma" mode, for other head sizes, or with EV_ATTN=ffma (A/B measurements)
     if (mode != 0 && H / heads == 48 && attn_tc_enabled())
       EV_TRY(launch_attention_tc(qkv, key_lens, ctxb, B, L, H, heads, mode == 3 ? 1 : 0, st));
@@ -685,8 +685,8 @@ int ev_create(ev_ctx** out, int device, const ev_config* cfg) {
   cudaDeviceProp prop;
   cudaError_t e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) { set_error("ev_create: cudaGetDeviceProperties(%d): %s", device, cudaGetErrorString(e)); return EV_ECUDA; }
-  if (prop.major != 10) {
-    set_error("ev_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_error("ev_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     return EV_EARCH;
   }
   EV_CHECK_ARG(cfg->hidden % 128 == 0 && cfg->hidden <= 512, "ev_create: hidden=%d unsupported", cfg->hidden);
@@ -699,7 +699,7 @@ int ev_create(ev_ctx** out, int device, const ev_config* cfg) {
   ev_ctx* c = new ev_ctx();
   c->cfg = *cfg;
   c->device = device;
-  {   // CUDA loads kernel code lazily at first launch; for the large tcgen05 kernels that is tens of milliseconds each, which would
+  {   // CUDA loads kernel code lazily at first launch; for the large tensor-core kernels that is tens of milliseconds each, which would
       // land on whichever utterance first needs a new tile shape.  Load them now, once per device.
     static std::atomic<uint64_t> loaded{0};
     int prev = -1;

@@ -1,4 +1,4 @@
-// Shared declarations of the sm_100a engine (internal; the public ABI is include/emotivoice_b200.h).
+// Shared declarations of the sm_90a engine (internal; the public ABI is include/emotivoice_b200.h).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,7 +27,7 @@ inline bool first_use_on_device(std::atomic<uint64_t>& mask) {
   return true;
 }
 int sm_count();                          // SMs of the CURRENT device (cached per device)
-// eager loading of the big tcgen05 kernels' code on the current device (ev_create calls them once per device)
+// eager loading of the big tensor-core kernels' code on the current device (ev_create calls them once per device)
 void preload_conv1d_gp();
 void preload_resblock_gp();
 void preload_attention_tc();
@@ -65,7 +65,7 @@ int use_device_of(const void* dev_ptr);  // cudaSetDevice(the device that owns d
 // griddepcontrol.launch_dependents (the next launch in the stream may be scheduled as soon as every CTA of this grid
 // has started) followed by griddepcontrol.wait (returns once the preceding grid has completed and its writes are
 // visible) -- before its first memory access, so stream order semantics are unchanged; what is gained is the launch
-// latency and, for the convolutions, the set-up (barriers, TMEM allocation, first weight stages) that runs before the wait.
+// latency and, for the convolutions, the set-up (barriers, first weight stages) that runs before the wait.
 // Transitivity: every kernel has at least one thread that waits unconditionally, so "grid N complete" implies "grid N-1 complete".
 // ---------------------------------------------------------------------------------
 template <bool PDL>
@@ -124,7 +124,7 @@ struct ConvParams {
                        // summation order, hence every output bit, independent of how utterances are batched)
 };
 int launch_conv1d(const ConvParams& p, cudaStream_t st);
-// tcgen05 variant (conv1d_tc.cu); p.w in the tensor-core layout [plane hi|lo][Cout/BNp][K][Cin/4][BNp][4], BNp = min(Cout,128);
+// tensor-core variant (conv1d_tc.cu); p.w in the tensor-core layout [plane hi|lo][Cout/BNp][K][Cin/4][BNp][4], BNp = min(Cout,128);
 // mode 0: one tf32 MMA per K step; 1: 3xTF32 fp32 emulation (three MMAs per K step); 2: bf16 operands
 // (p.w then in the bf16 layout [Cout/BNp][K][Cin/8][BNp][8 bf16]).
 int launch_conv1d_tc(const ConvParams& p, int mode, cudaStream_t st);
@@ -133,7 +133,7 @@ int tc_shape_kbg(const ConvParams& p, int mode);               // K granules per
 
 // ---------------------------------------------------------------------------------
 // HiFi-GAN convolutions on granule-planar activations (conv1d_gp.cu): [b][C/cpg][L][cpg], 16-byte granules of 4 fp32 or
-// 8 bf16 channels; the A operand is bulk-copied, the epilogue stores straight from the TMEM lane layout.
+// 8 bf16 channels; the A operand is bulk-copied, the epilogue stores straight from the accumulator registers.
 // ---------------------------------------------------------------------------------
 struct GpConvParams {
   const void* x;       // GP (B, Cin/cpg, L, cpg)
@@ -226,7 +226,7 @@ int launch_layernorm(const float* x, const int64_t* ids, const float* emb, const
                      cudaStream_t st, int n_emb = 0);
 int launch_attention(const float* qkv, const int32_t* key_lens, float* ctx, int B, int L, int H, int heads,
                      cudaStream_t st);
-// tcgen05 variant (attention_tc.cu), d_k = 48 only; tc_mode 1: 3xTF32 fp32 emulation, 0: one tf32 MMA per K step
+// tensor-core variant (attention_tc.cu), d_k = 48 only; tc_mode 1: 3xTF32 fp32 emulation, 0: one tf32 MMA per K step
 int launch_attention_tc(const float* qkv, const int32_t* key_lens, float* ctx, int B, int L, int H, int heads, int tc_mode, cudaStream_t st);
 int launch_cond_gather(const int64_t* spk, const float* spk_emb, const float* style, const float* content,
                        float* out, int B, int H, int bert, int n_spk, cudaStream_t st);

@@ -1,8 +1,8 @@
-// One ResBlock1 layer of HiFi-GAN as ONE kernel on granule-planar activations (sm_100a):
+// One ResBlock1 layer of HiFi-GAN as ONE kernel on granule-planar activations (sm_90a):
 //     out = [acc]( x + c2( lrelu( c1( lrelu(x), dilation d ) ), dilation 1 ) )            (hifigan/models.py:50-57)
 // The intermediate xt = c1(lrelu(x)) never leaves the SM: c1's epilogue writes lrelu(acc1 + b1) -- rounded / split exactly like
-// conv1d_gp.cu's transform warps would after a round trip through HBM -- straight from the TMEM lane layout (thread = row) into
-// a shared-memory tile that already has the K-major UMMA operand layout, and c2's taps are descriptor shifts over that tile.
+// conv1d_gp.cu's transform warps would after a round trip through HBM -- straight from the accumulator registers into a
+// shared-memory tile that already has the K-major operand layout, and c2's taps are descriptor shifts over that tile.
 // Per layer the activation traffic drops from 5 passes (x, xt write, xt read, x residual, out) to 2 (x, out; the residual
 // re-read hits L2) and the launches halve.  Same reduction orders and roundings as two conv1d_gp launches: BITWISE equal to them.
 //
@@ -11,12 +11,10 @@
 // tile (its last K-1 rows per tile are surplus and discarded).  xt rows outside [0, len) are written as zeros: the reference
 // pads c2's input with zeros, it does not convolve c1 over the padding.
 //
-// Unlike the round-1 fused kernel (which lost 10-21 %: one accumulator set, c1's epilogue, c2 and c2's epilogue serialised per
-// tile) everything is double buffered and the two epilogues are separate warp groups:
-//   MMA order   C1(0) | C1(i+1), C2(i) | ...        acc1[2], acc2[2] in TMEM (4*MT*C <= 512 columns)
-//   warps 4-7   epi1: acc1 -> xt tile (shared memory)         warps 0-3   epi2: acc2 + b2 + x (+ accumulate modes) -> HBM
-//   warps 8-11  transform the landed x stages in place; warp 12 x loader; warp 13 weight loader; warp 14 TMEM alloc + MMA issue
-// so c1 of the next tile runs under c2 / both epilogues of the current one and the x ring prefetches across tiles.
+// Roles (448 threads): warps 0-7 two consumer warpgroups -- per tile: c1 (wgmma, accumulators in registers), epi1 into the xt tile,
+// a named barrier over both warpgroups, c2 over the xt tile, epi2 (+ b2 + x, accumulate modes) to HBM; warps 8-11 transform the
+// landed x stages in place; warp 12 x loader; warp 13 weight loader (w1 then w2 of every tile, the order the consumers read them).
+// The x ring and the weight ring prefetch across tiles, so the loads of tile i+1 run under c2 and the epilogues of tile i.
 #include "ev_common.cuh"
 #include "tc_common.cuh"
 
@@ -25,9 +23,9 @@ namespace gpp {
 
 using namespace tc;
 
-constexpr int NTW = 4;
-constexpr int W_EPI1 = 4, W_XFORM = 8, W_ALOAD = 12, W_BLOAD = 13, W_MMA = 14;
-constexpr int GPP_THREADS = 15 * 32;
+constexpr int NCW = 8, NTW = 4;
+constexpr int W_XFORM = 8, W_ALOAD = 12, W_BLOAD = 13;
+constexpr int GPP_THREADS = 14 * 32;
 constexpr int MAX_A = 6, MAX_B = 8;
 constexpr int SMEM_HEAD = 1024;
 
@@ -36,7 +34,7 @@ struct PPlan {
   int rows1_pad, rows2_pad, R;
   int x_plane_bytes, x_stage_bytes, a2_plane_bytes, a2_bytes, b_plane_bytes, b_stage_bytes;
   int a_stages, b_stages;
-  int tmem_cols;
+  int acc_cols;        // MT * C <= 2 * ACC_REGS
   int tiles_m, total_tiles;
   int smem_total;
 };
@@ -48,7 +46,7 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
   PPlan q;
   q.mt = mt; q.kbg = kbg;
   const int C = p.C;
-  if (C > 128 || C % 32 || 4 * mt * C > 512) return false;
+  if (C > 128 || C % 32 || mt * C > 2 * ACC_REGS) return false;
   const int cpg = mode == 2 ? 8 : 4;            // activation granule (HBM / x tile)
   const int ocpg = mode >= 2 ? 8 : 4;           // operand granule of the xt tile and the weights
   const int xplanes = mode == 1 ? 2 : 1;
@@ -72,8 +70,7 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
   while (q.a_stages < 4 && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
   while (q.b_stages < MAX_B && fits(q.a_stages, q.b_stages + 1)) ++q.b_stages;
   while (q.a_stages < MAX_A && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
-  q.tmem_cols = 32;
-  while (q.tmem_cols < 4 * mt * C) q.tmem_cols <<= 1;
+  q.acc_cols = mt * C;
   q.tiles_m = (p.L + q.R - 1) / q.R;
   q.total_tiles = p.B * q.tiles_m;
   q.smem_total = SMEM_HEAD + q.a2_bytes + q.a_stages * q.x_stage_bytes + q.b_stages * q.b_stage_bytes;
@@ -95,13 +92,13 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
   constexpr int OCPG = OP16 ? 8 : 4;
   constexpr int KB = CPG * KBG;
   constexpr int KBGW = KBG * CPG / OCPG;        // operand granules (weights, xt tile) per channel block
+  constexpr int NA = ACC_REGS / MT;
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules per MMA K step");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int C = p.C;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_raw + 768);
   uint8_t* a2_tile = smem_raw + SMEM_HEAD;
   uint8_t* x_tiles = a2_tile + pl.a2_bytes;
   uint8_t* b_tiles = x_tiles + pl.a_stages * pl.x_stage_bytes;
@@ -111,33 +108,17 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
   auto a_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (3 * MAX_A + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (3 * MAX_A + MAX_B + s); };
-  const uint32_t misc = bar_base + 8u * (3 * MAX_A + 2 * MAX_B);
-  auto acc1_full = [&](int s) { return misc + 8u * s; };
-  auto acc1_empty = [&](int s) { return misc + 8u * (2 + s); };
-  auto acc2_full = [&](int s) { return misc + 8u * (4 + s); };
-  auto acc2_empty = [&](int s) { return misc + 8u * (6 + s); };
-  const uint32_t a2_full = misc + 64u, a2_empty = misc + 72u;
 
   if (tid == 0) {
-    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(acc1_full(s), 1); mbar_init(acc1_empty(s), 4); mbar_init(acc2_full(s), 1); mbar_init(acc2_empty(s), 4); }
-    mbar_init(a2_full, 128); mbar_init(a2_empty, 1);
+    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), NCW); }
+    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), NCW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == W_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(pl.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   const int n_cb = (C + KB - 1) / KB;
   const int gC = C / CPG;                      // activation granule planes per item
-  // TMEM columns: acc1[buf] at buf*MT*C, acc2[buf] at (2 + buf)*MT*C
   // A launch carries up to three layers of one shape (the same-index layers of HiFi-GAN's parallel ResBlocks: their own taps,
   // dilation, weights, tensors, hence their own rows per tile and tile count); tiles are numbered member after member.
   auto group_of = [&](int tile) { return (gs.ng > 1 && tile >= gs.g[1].tile0) ? ((gs.ng > 2 && tile >= gs.g[2].tile0) ? 2 : 1) : 0; };
@@ -154,160 +135,168 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
     return tile;
   };
 
-  if (warp < W_EPI1) {
-    // ============================ epi2: acc2 + b2 + x (+ accumulate) -> out ================================
+  if (warp < NCW) {
+    // ============================ consumers: c1 -> epi1 (xt tile) -> c2 -> epi2 ================================
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int quad = warp;
-    const int nchunks = C / 32;
-    constexpr int NG = 32 / CPG;
-    int cnt = 0;
-    for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x), ++cnt) {
+    const int wg = warp >> 2, wl = warp & 3;
+    const float slope = p.slope;
+    const uint32_t x_lbo = (uint32_t)pl.rows1_pad * 16u, a2_lbo = (uint32_t)pl.rows2_pad * 16u, b_lbo = (uint32_t)C * 16u;
+    const uint64_t x_desc0 = make_desc(0u, X3B ? 2u * x_lbo : x_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
+    const uint64_t a2_desc0 = make_desc(smem_u32(a2_tile) + (uint32_t)(wg * 64) * 16u, a2_lbo, 128u);
+    const uint32_t x_k = (X3B ? 4u : 2u) * x_lbo, x_lo_off = X3B ? x_lbo : (uint32_t)pl.x_plane_bytes;
+    float acc[MT][NA];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
+    auto release = [&](int sb, int sa) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(b_empty(sb));
+        if (sa >= 0) mbar_arrive(a_empty(sa));
+      }
+    };
+    int a_cnt = 0, b_cnt = 0;
+    for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
       int gi, b, t0;
       const int len = tile_len(tile, gi, b, t0);
       const GpPairGroup& G = gs.g[gi];
-      const int R = G.R;
-      const int buf = cnt & 1;
-      bool waited = false;
-#pragma unroll 1
-      for (int item = 0; item < MT * nchunks; ++item) {
-        const int mt = item / nchunks, c = (item - mt * nchunks) * 32;
-        const int rl = mt * BM + quad * 32 + lane;              // row inside the tile
-        const int row = t0 + rl;
-        const bool ok = rl < R && row < len;
-        const size_t gbase = ((size_t)b * gC + c / CPG) * p.L + row;
-        uint4 rq[NG];
+      const int K = G.K, dil = G.dil, R = G.R;
+      const int h2 = (K - 1) / 2;
+      // ---- c1 over the staged x tile
+      {
+        int prev_sb = -1, prev_sa = -1;
+        for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
+          const int sa = a_cnt % pl.a_stages;
+          const int nk = min(KB, C - cb * KB) / (2 * OCPG);
+          mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
+          const uint64_t x0 = desc_advance(x_desc0, smem_u32(x_tiles + sa * pl.x_stage_bytes) + (uint32_t)(wg * 64) * 16u);
+          for (int j = 0; j < K; ++j, ++b_cnt) {
+            const int sb = b_cnt % pl.b_stages;
+            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+            const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
+            const uint64_t xj = desc_advance(x0, (uint32_t)(j * dil) * 16u);
+            wgmma_fence();
+            for (int k = 0; k < nk; ++k) {
+              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
+              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
+              const uint64_t a_k = desc_advance(xj, (uint32_t)k * x_k);
+              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
 #pragma unroll
-        for (int q = 0; q < NG; ++q) {
-          rq[q] = make_uint4(0u, 0u, 0u, 0u);
-          if (ok) rq[q] = *(reinterpret_cast<const uint4*>(G.x) + gbase + (size_t)q * p.L);       // the residual: L2 hit (the x tile was just staged)
-        }
-        if (!waited) {
-          mbar_wait(acc2_full(buf), (cnt >> 1) & 1);
-          tc_fence_after();
-          waited = true;
-        }
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((2 + buf) * MT * C + mt * C + c), 32, v);
-        if (ok) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(G.b2 + c) + q);
-            v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
-          }
-#pragma unroll
-          for (int q = 0; q < NG; ++q) {
-            if (BF16) {
-              const uint32_t w4[4] = {rq[q].x, rq[q].y, rq[q].z, rq[q].w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) { v[8 * q + 2 * e] += __uint_as_float(w4[e] << 16); v[8 * q + 2 * e + 1] += __uint_as_float(w4[e] & 0xffff0000u); }
-            } else {
-              v[4 * q] += __uint_as_float(rq[q].x); v[4 * q + 1] += __uint_as_float(rq[q].y);
-              v[4 * q + 2] += __uint_as_float(rq[q].z); v[4 * q + 3] += __uint_as_float(rq[q].w);
-            }
-          }
-          if (p.acc != EV_ACC_STORE) {
-            uint4 oq[NG];
-#pragma unroll
-            for (int q = 0; q < NG; ++q) oq[q] = *(reinterpret_cast<const uint4*>(G.out) + gbase + (size_t)q * p.L);
-#pragma unroll
-            for (int q = 0; q < NG; ++q) {
-              if (BF16) {
-                const uint32_t w4[4] = {oq[q].x, oq[q].y, oq[q].z, oq[q].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) { v[8 * q + 2 * e] += __uint_as_float(w4[e] << 16); v[8 * q + 2 * e + 1] += __uint_as_float(w4[e] & 0xffff0000u); }
-              } else {
-                v[4 * q] += __uint_as_float(oq[q].x); v[4 * q + 1] += __uint_as_float(oq[q].y);
-                v[4 * q + 2] += __uint_as_float(oq[q].z); v[4 * q + 3] += __uint_as_float(oq[q].w);
+              for (int mt = 0; mt < MT; ++mt) {
+                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
+                mma_step<MODE, NA>(C, acc[mt], a_hi, desc_advance(a_hi, x_lo_off), b_hi, b_lo, first);
               }
             }
-            if (p.acc == EV_ACC_ADD_DIV) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] /= p.div;
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < NG; ++q) {
-            uint4 o;
-            if (BF16) {
-              o.x = pack_bf16(v[8 * q], v[8 * q + 1]); o.y = pack_bf16(v[8 * q + 2], v[8 * q + 3]);
-              o.z = pack_bf16(v[8 * q + 4], v[8 * q + 5]); o.w = pack_bf16(v[8 * q + 6], v[8 * q + 7]);
-            } else {
-              o.x = __float_as_uint(v[4 * q]); o.y = __float_as_uint(v[4 * q + 1]); o.z = __float_as_uint(v[4 * q + 2]); o.w = __float_as_uint(v[4 * q + 3]);
-            }
-            *(reinterpret_cast<uint4*>(G.out) + gbase + (size_t)q * p.L) = o;
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev_sb >= 0) release(prev_sb, prev_sa);
+            prev_sb = sb;
+            prev_sa = j == K - 1 ? sa : -1;
           }
         }
+        wgmma_wait<0>();
+        release(prev_sb, prev_sa);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc2_empty(buf));
-    }
-  } else if (warp < W_XFORM) {
-    // ============================ epi1: acc1 + b1 -> lrelu -> operand format -> xt tile in shared memory ===================
-    const int quad = warp - W_EPI1;
-    const int nchunks = C / 32;
-    const float slope = p.slope;
-    int cnt = 0;
-    for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x), ++cnt) {
-      int gi, b, t0;
-      const int len = tile_len(tile, gi, b, t0);
-      const int h2 = (gs.g[gi].K - 1) / 2;
-      const float* b1 = gs.g[gi].b1;
-      const int buf = cnt & 1;
-      mbar_wait(acc1_full(buf), (cnt >> 1) & 1);
-      mbar_wait(a2_empty, (cnt & 1) ^ 1);                 // c2 of the previous tile has read the xt tile
-      tc_fence_after();
-#pragma unroll 1
-      for (int item = 0; item < MT * nchunks; ++item) {
-        const int mt = item / nchunks, c = (item - mt * nchunks) * 32;
-        const int r2 = mt * BM + quad * 32 + lane;
-        const int row = t0 - h2 + r2;
-        const bool ok = row >= 0 && row < len;            // xt outside the sequence is c2's ZERO padding
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * MT * C + mt * C + c), 32, v);
+      // ---- epi1: acc1 + b1 -> lrelu -> operand format -> xt tile.  Both warpgroups' c2 of the previous tile read the whole
+      // ---- xt tile (their taps overlap the other's rows), so the tile is only rewritten once both have finished it.
+      bar_sync(1, NCW * 32);
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(b1 + c) + q);
-          v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
-        }
+      for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float t = v[i];
-          if (BF16) t = __uint_as_float(pack_bf16(t, 0.f) << 16);      // the unfused path stores xt as bf16 before activating it
-          v[i] = ok ? lrelu_f(t, slope) : 0.f;
-        }
-        uint8_t* dst = a2_tile + ((size_t)(c / OCPG) * pl.rows2_pad + r2) * 16;
-        constexpr int NGO = 32 / OCPG;
-#pragma unroll
-        for (int q = 0; q < NGO; ++q) {
-          uint8_t* d = dst + (size_t)q * pl.rows2_pad * 16;
+        for (int i = 0; i < NA; i += 2) {
+          const int c = frag_col(i, lane);
+          if (c >= C) continue;
+          const int r2 = mt * BM + wg * 64 + frag_row(i, lane, wl);
+          const int row = t0 - h2 + r2;
+          const bool ok = row >= 0 && row < len;            // xt outside the sequence is c2's ZERO padding
+          const float2 b1 = __ldg(reinterpret_cast<const float2*>(G.b1 + c));
+          float v0 = acc[mt][i] + b1.x, v1 = acc[mt][i + 1] + b1.y;
+          if (BF16) {      // the unfused path stores xt as bf16 before activating it
+            v0 = __uint_as_float(pack_bf16(v0, 0.f) << 16);
+            v1 = __uint_as_float(pack_bf16(v1, 0.f) << 16);
+          }
+          v0 = ok ? lrelu_f(v0, slope) : 0.f;
+          v1 = ok ? lrelu_f(v1, slope) : 0.f;
+          uint8_t* d = a2_tile + ((size_t)(c / OCPG) * pl.rows2_pad + r2) * 16 + (c % OCPG) * (OP16 ? 2 : 4);
           if (OP16) {
-            uint32_t hi[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) hi[e] = pack_bf16(v[8 * q + 2 * e], v[8 * q + 2 * e + 1]);
-            *reinterpret_cast<uint4*>(d) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            if (X3B) {
-              uint32_t lo[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                lo[e] = pack_bf16(v[8 * q + 2 * e] - __uint_as_float(hi[e] << 16), v[8 * q + 2 * e + 1] - __uint_as_float(hi[e] & 0xffff0000u));
-              *reinterpret_cast<uint4*>(d + pl.a2_plane_bytes) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            }
+            const uint32_t hi = pack_bf16(v0, v1);
+            *reinterpret_cast<uint32_t*>(d) = hi;
+            if (X3B) *reinterpret_cast<uint32_t*>(d + pl.a2_plane_bytes) = pack_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xffff0000u));
           } else {
-            const float4 h = make_float4(to_tf32(v[4 * q]), to_tf32(v[4 * q + 1]), to_tf32(v[4 * q + 2]), to_tf32(v[4 * q + 3]));
-            *reinterpret_cast<float4*>(d) = h;
-            if (SPLIT3) {
-              const float4 l = make_float4(to_tf32(v[4 * q] - h.x), to_tf32(v[4 * q + 1] - h.y), to_tf32(v[4 * q + 2] - h.z), to_tf32(v[4 * q + 3] - h.w));
-              *reinterpret_cast<float4*>(d + pl.a2_plane_bytes) = l;
-            }
+            const float2 h = make_float2(to_tf32(v0), to_tf32(v1));
+            *reinterpret_cast<float2*>(d) = h;
+            if (SPLIT3) *reinterpret_cast<float2*>(d + pl.a2_plane_bytes) = make_float2(to_tf32(v0 - h.x), to_tf32(v1 - h.y));
           }
         }
       }
-      fence_proxy_async();
-      mbar_arrive(a2_full);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc1_empty(buf));
+      fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core
+      bar_sync(1, NCW * 32);        // the whole xt tile is written
+      // ---- c2 over the xt tile
+      {
+        int prev_sb = -1;
+        for (int cb = 0; cb < n_cb; ++cb) {
+          const int nk = min(KB, C - cb * KB) / (2 * OCPG);
+          const uint64_t a0 = desc_advance(a2_desc0, (uint32_t)(cb * KBGW) * a2_lbo);
+          for (int j = 0; j < K; ++j, ++b_cnt) {
+            const int sb = b_cnt % pl.b_stages;
+            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+            const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
+            const uint64_t aj = desc_advance(a0, (uint32_t)j * 16u);
+            wgmma_fence();
+            for (int k = 0; k < nk; ++k) {
+              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
+              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
+              const uint64_t a_k = desc_advance(aj, (uint32_t)k * 2u * a2_lbo);
+              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
+#pragma unroll
+              for (int mt = 0; mt < MT; ++mt) {
+                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
+                mma_step<MODE, NA>(C, acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a2_plane_bytes), b_hi, b_lo, first);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev_sb >= 0) release(prev_sb, -1);
+            prev_sb = sb;
+          }
+        }
+        wgmma_wait<0>();
+        release(prev_sb, -1);
+      }
+      // ---- epi2: acc2 + b2 + x (+ accumulate) -> out
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int i = 0; i < NA; i += 2) {
+          const int c = frag_col(i, lane);
+          const int rl = mt * BM + wg * 64 + frag_row(i, lane, wl);      // row inside the tile
+          const int row = t0 + rl;
+          if (c >= C || rl >= R || row >= len) continue;
+          const size_t e = (((size_t)b * gC + c / CPG) * p.L + row) * CPG + (c % CPG);
+          const float2 b2 = __ldg(reinterpret_cast<const float2*>(G.b2 + c));
+          float v0 = acc[mt][i] + b2.x, v1 = acc[mt][i + 1] + b2.y;
+          if (BF16) {
+            const uint32_t r = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.x) + e);   // the residual: L2 hit
+            v0 += __uint_as_float(r << 16); v1 += __uint_as_float(r & 0xffff0000u);
+            if (p.acc != EV_ACC_STORE) {
+              const uint32_t q = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.out) + e);
+              v0 += __uint_as_float(q << 16); v1 += __uint_as_float(q & 0xffff0000u);
+              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
+            }
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(G.out) + e) = pack_bf16(v0, v1);
+          } else {
+            const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.x) + e);
+            v0 += r.x; v1 += r.y;
+            if (p.acc != EV_ACC_STORE) {
+              const float2 q = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.out) + e);
+              v0 += q.x; v1 += q.y;
+              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
+            }
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(G.out) + e) = make_float2(v0, v1);
+          }
+        }
+      }
     }
   } else if (warp < W_ALOAD) {
     // ============================ transform warps: in-place pass over the landed x stage =======================
@@ -401,8 +390,8 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       }
     }
     __syncwarp();
-  } else if (warp == W_BLOAD) {
-    // ============================ weight loader: the MMA issuer's order  C1(0) | C1(i+1), C2(i) ====================
+  } else {
+    // ============================ weight loader: the consumers' order  w1(i), w2(i), w1(i+1), ... ====================
     if (lane == 0) {
       const int win = C / OCPG;
       int b_cnt = 0;
@@ -421,126 +410,13 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
           }
         }
       };
-      int tile = next_active(blockIdx.x);
-      if (tile < pl.total_tiles) stream(gs.g[group_of(tile)].w1, gs.g[group_of(tile)].K);
-      while (tile < pl.total_tiles) {
-        const int nxt = next_active(tile + gridDim.x);
-        if (nxt < pl.total_tiles) stream(gs.g[group_of(nxt)].w1, gs.g[group_of(nxt)].K);
-        stream(gs.g[group_of(tile)].w2, gs.g[group_of(tile)].K);
-        tile = nxt;
+      for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
+        const GpPairGroup& G = gs.g[group_of(tile)];
+        stream(G.w1, G.K);
+        stream(G.w2, G.K);
       }
     }
     __syncwarp();
-  } else {
-    // ============================ MMA issuer (all lanes in the control flow, one elected lane issues) =======================
-    const uint32_t x_lbo = (uint32_t)pl.rows1_pad * 16u, a2_lbo = (uint32_t)pl.rows2_pad * 16u, b_lbo = (uint32_t)C * 16u;
-    const uint32_t fmt = OP16 ? 1u : 2u;
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(C >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-    const uint64_t x_desc0 = make_desc(0u, X3B ? 2u * x_lbo : x_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
-    const uint64_t a2_desc0 = make_desc(smem_u32(a2_tile), a2_lbo, 128u);
-    const uint32_t x_k = (X3B ? 4u : 2u) * x_lbo, x_lo_off = X3B ? x_lbo : (uint32_t)pl.x_plane_bytes;
-    int a_cnt = 0, b_cnt = 0;
-    auto mma3 = [&](uint32_t d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t first) {
-      if (SPLIT3) {
-        umma_tf32(d, a_lo, b_hi, idesc, first); umma_tf32(d, a_hi, b_lo, idesc, 1u); umma_tf32(d, a_hi, b_hi, idesc, 1u);
-      } else if (X3B) {
-        umma_bf16(d, a_lo, b_hi, idesc, first); umma_bf16(d, a_hi, b_lo, idesc, 1u); umma_bf16(d, a_hi, b_hi, idesc, 1u);
-      } else if (BF16) {
-        umma_bf16(d, a_hi, b_hi, idesc, first);
-      } else {
-        umma_tf32(d, a_hi, b_hi, idesc, first);
-      }
-    };
-    auto conv1 = [&](int cnt, int tile) {          // acc1[cnt & 1] = c1 over the staged x tile of the cnt-th active tile
-      const int K = gs.g[group_of(tile)].K, dil = gs.g[group_of(tile)].dil;
-      const int buf = cnt & 1;
-      mbar_wait(acc1_empty(buf), ((cnt >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_base = tmem_base + (uint32_t)(buf * MT * C);
-      for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-        const int sa = a_cnt % pl.a_stages;
-        const int nk = min(KB, C - cb * KB) / (2 * OCPG);
-        mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
-        const uint64_t x0 = desc_advance(x_desc0, smem_u32(x_tiles + sa * pl.x_stage_bytes));
-        for (int j = 0; j < K; ++j, ++b_cnt) {
-          const int sb = b_cnt % pl.b_stages;
-          mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
-          tc_fence_after();
-          const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-          const uint64_t xj = desc_advance(x0, (uint32_t)(j * dil) * 16u);
-          if (elect_one()) {
-            for (int k = 0; k < nk; ++k) {
-              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-              const uint64_t a_k = desc_advance(xj, (uint32_t)k * x_k);
-              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
-#pragma unroll
-              for (int mt = 0; mt < MT; ++mt) {
-                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma3(d_base + (uint32_t)(mt * C), a_hi, desc_advance(a_hi, x_lo_off), b_hi, b_lo, first);
-              }
-            }
-            umma_commit(b_empty(sb));
-            if (j == K - 1) {
-              umma_commit(a_empty(sa));
-              if (cb == n_cb - 1) umma_commit(acc1_full(buf));
-            }
-          }
-          __syncwarp();
-        }
-      }
-    };
-    auto conv2 = [&](int cnt, int tile) {          // acc2[cnt & 1] = c2 over the xt tile epi1 wrote for the cnt-th active tile
-      const int K = gs.g[group_of(tile)].K;
-      const int buf = cnt & 1;
-      mbar_wait(a2_full, cnt & 1);
-      mbar_wait(acc2_empty(buf), ((cnt >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_base = tmem_base + (uint32_t)((2 + buf) * MT * C);
-      for (int cb = 0; cb < n_cb; ++cb) {
-        const int nk = min(KB, C - cb * KB) / (2 * OCPG);
-        const uint64_t a0 = desc_advance(a2_desc0, (uint32_t)(cb * KBGW) * a2_lbo);
-        for (int j = 0; j < K; ++j, ++b_cnt) {
-          const int sb = b_cnt % pl.b_stages;
-          mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
-          tc_fence_after();
-          const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-          const uint64_t aj = desc_advance(a0, (uint32_t)j * 16u);
-          if (elect_one()) {
-            for (int k = 0; k < nk; ++k) {
-              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-              const uint64_t a_k = desc_advance(aj, (uint32_t)k * 2u * a2_lbo);
-              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
-#pragma unroll
-              for (int mt = 0; mt < MT; ++mt) {
-                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma3(d_base + (uint32_t)(mt * C), a_hi, desc_advance(a_hi, (uint32_t)pl.a2_plane_bytes), b_hi, b_lo, first);
-              }
-            }
-            umma_commit(b_empty(sb));
-            if (j == K - 1 && cb == n_cb - 1) { umma_commit(a2_empty); umma_commit(acc2_full(buf)); }
-          }
-          __syncwarp();
-        }
-      }
-    };
-    int tile = next_active(blockIdx.x), cnt = 0;
-    if (tile < pl.total_tiles) conv1(0, tile);
-    while (tile < pl.total_tiles) {
-      const int nxt = next_active(tile + gridDim.x);
-      if (nxt < pl.total_tiles) conv1(cnt + 1, nxt);     // runs under epi1 / c2 / epi2 of the current tile
-      conv2(cnt, tile);
-      tile = nxt;
-      ++cnt;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(pl.tmem_cols));
   }
 }
 
@@ -585,7 +461,7 @@ bool gp_pair_supported(const GpPairParams& p, int mode) {
 int debug_gp_pair_plan(const GpPairParams& p, int mode, int* v) {
   gpp::PPlan pl;
   if (!plan_pair(p, mode, &pl)) { set_error("resblock_gp: shape not supported (C=%d K=%d dil=%d mode=%d)", p.C, p.K, p.dil, mode); return EV_EINVAL; }
-  v[0] = pl.mt; v[1] = pl.kbg; v[2] = pl.a_stages; v[3] = pl.b_stages; v[4] = gpp::NTW; v[5] = pl.tmem_cols; v[6] = pl.smem_total;
+  v[0] = pl.mt; v[1] = pl.kbg; v[2] = pl.a_stages; v[3] = pl.b_stages; v[4] = gpp::NTW; v[5] = pl.acc_cols; v[6] = pl.smem_total;
   v[7] = pl.total_tiles; v[8] = pl.R; v[9] = pl.rows1_pad; v[10] = pl.rows2_pad;
   return EV_OK;
 }
@@ -694,7 +570,7 @@ int debug_gp_pair_group_plan(const GpPairParams* ps, int n, int mode, int* v) { 
   GpPairGroups gs{};
   gpp::PPlan pl;
   if (!plan_pair_group(ps, n, mode, &gs, &pl)) { set_error("resblock_gp group: the %d layers do not share a launch shape", n); return EV_EINVAL; }
-  v[0] = pl.mt; v[1] = pl.kbg; v[2] = pl.total_tiles; v[3] = pl.rows1_pad; v[4] = pl.rows2_pad; v[5] = pl.smem_total; v[6] = pl.tmem_cols;
+  v[0] = pl.mt; v[1] = pl.kbg; v[2] = pl.total_tiles; v[3] = pl.rows1_pad; v[4] = pl.rows2_pad; v[5] = pl.smem_total; v[6] = pl.acc_cols;
   for (int i = 0; i < 3; ++i) {
     v[7 + 3 * i] = i < gs.ng ? gs.g[i].K : 0;
     v[8 + 3 * i] = i < gs.ng ? gs.g[i].tiles_m : 0;

@@ -2,7 +2,7 @@
 // BertModel + pooler, run on the CPU twice per utterance by every caller (inference_am_vocoder_joint.py:25-38,106-107).
 // This file holds its two small kernels (embedding sum + LayerNorm, the [CLS] GEMV with tanh), the context, weight
 // resolution, launch sequencing and the ev_style_* C ABI.  The GEMMs run in conv1d_tc.cu (K = 1 convolutions, 3xTF32 on
-// tcgen05 by default), attention / LayerNorm in am_kernels.cu -- the kernels the acoustic model already uses.
+// tensor cores by default), attention / LayerNorm in am_kernels.cu -- the kernels the acoustic model already uses.
 //
 // BertModel.forward restated (post-LN blocks; cited from the published architecture, the library is not vendored):
 //   x = LN(word[id] + type[tt] + pos[t])
@@ -223,8 +223,8 @@ int ev_style_create(ev_style_ctx** out, int device, const ev_style_config* cfg) 
   cudaDeviceProp prop;
   cudaError_t e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) { set_error("ev_style_create: cudaGetDeviceProperties(%d): %s", device, cudaGetErrorString(e)); return EV_ECUDA; }
-  if (prop.major != 10) {
-    set_error("ev_style_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_error("ev_style_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     return EV_EARCH;
   }
   const ev_style_config& g = *cfg;

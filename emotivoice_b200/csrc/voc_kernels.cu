@@ -1,4 +1,4 @@
-// HiFi-GAN generator kernels that are not implicit GEMMs (sm_100a, fp32): the layout change at
+// HiFi-GAN generator kernels that are not implicit GEMMs (sm_90a, fp32): the layout change at
 // the Generator.forward boundary, the final conv_post + tanh, and the callers' PCM16 conversion.
 #include "ev_common.cuh"
 

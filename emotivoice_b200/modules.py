@@ -12,7 +12,7 @@ openaiapi.py:78-82) run unchanged: ``JETSGenerator(conf).to(device)``,
 ``.load_state_dict(torch.load(path)['generator'])``, ``.eval()``, call under ``no_grad``.
 
 The modules hold ``nn.Parameter`` trees only (for state-dict compatibility); every FLOP
-of ``forward`` runs in libemotivoice_b200.so (hand-written sm_100a kernels) through the C
+of ``forward`` runs in libemotivoice_b200.so (hand-written sm_90a kernels) through the C
 ABI in include/emotivoice_b200.h.  PyTorch provides device memory and the stream.  There
 is no CPU path: calling ``forward`` on CPU tensors raises.
 """
@@ -88,7 +88,7 @@ class _Engine:
         self.lib = _abi.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("emotivoice_b200 runs on CUDA (sm_100a) only; got device %s. "
+            raise RuntimeError("emotivoice_b200 runs on CUDA (sm_90a) only; got device %s. "
                                "There is no CPU fallback." % (self.device,))
         self.index_dev = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self.cfg = _abi.make_config(conf)
@@ -242,7 +242,7 @@ class _EngineOwner(nn.Module):
 
     @property
     def precision(self):
-        """"fp32" (default): fp32-accurate 3xTF32 on the tcgen05 tensor cores (~1e-6 relative error).
+        """"fp32" (default): fp32-accurate 3xTF32 on the tensor cores (~1e-6 relative error).
         "tf32": decoder + vocoder with one tf32 MMA per K step (what the reference's eager PyTorch does for
         convolutions on a GPU); the duration-critical prefix stays fp32-accurate, so durations are
         identical in all modes.  "fp32_ffma": plain fp32 FFMA kernels, no tensor cores."""

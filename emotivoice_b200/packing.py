@@ -57,7 +57,7 @@ def to_tc_layout(w_kio):
     """(K, Cin, Cout) -> (2, Cout/BNp, K, Cin/4, BNp, 4) with BNp = min(Cout, 128): the tensor-core
     kernel's weight layout.  Blocked by N tile, then granule-major: 16-byte K-granules with the tile's
     C_out rows 16 B apart, so one pipeline stage (tap, channel block) of one N tile is ONE contiguous run
-    that a single bulk copy lands in shared memory exactly in the no-swizzle K-major UMMA layout.
+    that a single bulk copy lands in shared memory exactly in the no-swizzle K-major wgmma operand layout.
     Plane 0 = tf32(w) ("hi"), plane 1 = tf32(w - hi) ("lo", used by the 3xTF32 fp32-emulation mode only)."""
     if w_kio.dim() == 2:
         w_kio = w_kio.unsqueeze(0)

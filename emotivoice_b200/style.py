@@ -63,7 +63,7 @@ class _StyleEngine:
         self.lib = _abi.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("emotivoice_b200 runs on CUDA (sm_100a) only; got device %s. There is no CPU fallback." % (self.device,))
+            raise RuntimeError("emotivoice_b200 runs on CUDA (sm_90a) only; got device %s. There is no CPU fallback." % (self.device,))
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
         _, self.n_head_out = packing.style_head_slices(sc)
         self.cfg = _abi.EvStyleConfig(sc.vocab_size, sc.max_position_embeddings, sc.type_vocab_size, sc.hidden_size,
@@ -121,7 +121,7 @@ class StyleEncoder(_EngineOwner):
 
     @property
     def precision(self):
-        """"fp32" (default): fp32-accurate 3xTF32 on the tcgen05 tensor cores; "tf32": one tf32 MMA per K step."""
+        """"fp32" (default): fp32-accurate 3xTF32 on the tensor cores; "tf32": one tf32 MMA per K step."""
         return self._ev_precision
 
     @precision.setter

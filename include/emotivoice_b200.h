@@ -1,5 +1,5 @@
 /*
- * emotivoice_b200.h -- C ABI of libemotivoice_b200.so (sm_100a).
+ * emotivoice_b200.h -- C ABI of libemotivoice_b200.so (sm_90a, H100).
  *
  * The reference (netease-youdao/EmotiVoice) has no FFI / plugin registry: its
  * boundary for this path is the Python torch.nn.Module API of
@@ -47,7 +47,7 @@ enum {
   EV_ECUDA = -3,       /* CUDA runtime error (message has the cudaError string) */
   EV_EWORKSPACE = -4,  /* workspace too small */
   EV_EPELEN = -5,      /* positional table shorter than the sequence: rebind a longer one */
-  EV_EARCH = -6        /* device is not sm_100 */
+  EV_EARCH = -6        /* device is not sm_90 */
 };
 
 /* activation / epilogue selectors of ev_op_conv1d */
@@ -103,12 +103,12 @@ EV_API int ev_bind_weights(ev_ctx* ctx, const float* blob, size_t n_floats,
 EV_API int ev_bind_pe(ev_ctx* ctx, const float* pe, int pe_len);
 
 /* Arithmetic of the GEMM-shaped layers (linear / conv / transposed conv):
- *   EV_PREC_FP32 (default): fp32-accurate on the tcgen05 tensor cores by 3xTF32 splitting (x = hi + lo,
- *     three tf32 MMAs per K step, fp32 accumulation in TMEM); error ~1e-6 relative, like an fp32 FFMA chain.
+ *   EV_PREC_FP32 (default): fp32-accurate on the tensor cores by 3xTF32 splitting (x = hi + lo,
+ *     three tf32 MMAs per K step, fp32 accumulation); error ~1e-6 relative, like an fp32 FFMA chain.
  *   EV_PREC_TF32: decoder + vocoder with ONE tf32 MMA per K step (operands rounded to nearest tf32) -- the
  *     arithmetic the reference's eager PyTorch uses for convolutions on a GPU (cudnn.allow_tf32 default);
  *     the duration-critical prefix (encoder, conditioning, predictors) stays 3xTF32.
- *   EV_PREC_BF16: decoder + vocoder with bf16 operands (tcgen05 kind::f16, fp32 accumulation; activations stay fp32
+ *   EV_PREC_BF16: decoder + vocoder with bf16 operands (wgmma bf16, fp32 accumulation; activations stay fp32
  *     in HBM and are rounded by the staging warps); prefix 3xTF32 like EV_PREC_TF32.  BASELINE.json configs[2].
  *   EV_PREC_FP32_FFMA: plain fp32 FFMA kernels everywhere (no tensor cores; the round-1 baseline path).
  * Attention, LayerNorm, softmax, upsampling and the heads are fp32 in every mode. */
@@ -180,7 +180,7 @@ EV_API int ev_op_conv1d(const float* x, const float* w, const float* bias, size_
                         const float* res, float* out, int B, int L, int Cin, int Cout, int K, int dil,
                         const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act,
                         int acc, float div, void* stream);
-/* Same contract on the tensor cores (tcgen05.mma kind::tf32, accumulator in TMEM); w_tc is in the
+/* Same contract on the tensor cores (wgmma tf32 / bf16, fp32 accumulators in registers); w_tc is in the
  * tensor-core layout (2 planes hi|lo, Cout/BNp N tiles, K, Cin/4, BNp = min(Cout,128), 4; packing.to_tc_layout);
  * split3 = 0: 1xTF32, 1: 3xTF32 fp32 emulation, 2: bf16 operands (w_tc then in the bf16 layout of
  * packing.to_tc16_layout; Cin % 16 == 0).  Requires Cin % 8 == 0, Cout % 16 == 0 and Cout <= 128 or Cout % 128 == 0.  splitk_ws (optional, splitk_floats floats of scratch) lets a
@@ -190,8 +190,8 @@ EV_API int ev_op_conv1d_tc(const float* x, const float* w_tc, int split3, const 
                            const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act,
                            int acc, float div, float* splitk_ws, size_t splitk_floats, void* stream);
 /* Host-only introspection (no GPU needed): the tile / pipeline plan ev_op_conv1d_tc would use for a shape.
- * out11 = {BN, MT, KBG, a_stages, b_stages, producer groups, ksplit, tmem columns, smem bytes, tiles, rows_pad}.
- * The CPU tests check the invariants the kernel relies on (ring depth >= producer groups, TMEM/smem limits,
+ * out11 = {BN, MT, KBG, a_stages, b_stages, producer groups, ksplit, accumulator columns (MT x BN), smem bytes, tiles, rows_pad}.
+ * The CPU tests check the invariants the kernel relies on (ring depth >= producer groups, register/smem limits,
  * summation-order parameters independent of batch and length). */
 EV_API int ev_debug_tc_plan(int B, int L, int Cin, int Cout, int K, int dil, int split3, int ksplit, int* out11);
 /* HiFi-GAN convolution on GRANULE-PLANAR activations (csrc/conv1d_gp.cu; what ev_vocoder runs in every tensor-core mode).
@@ -244,8 +244,8 @@ EV_API int ev_op_layernorm(const float* x, const float* w, const float* b, float
 /* Multi-head self-attention core (encoder.py:84-109) on a packed (B,L,3H) q|k|v buffer. */
 EV_API int ev_op_attention(const float* qkv, const int32_t* key_lens, float* ctx_out, int B, int L, int H,
                            int n_heads, void* stream);
-/* The same attention on the tensor cores (csrc/attention_tc.cu): QK^T and PV as tcgen05.mma with the softmax between two TMEM
- * reads; d_k = 48 only.  tc_mode 1 = 3xTF32 fp32 emulation (what the engine uses wherever a layer runs fp32-accurate),
+/* The same attention on the tensor cores (csrc/attention_tc.cu): QK^T and PV as wgmma with the softmax on the register
+ * accumulators; d_k = 48 only.  tc_mode 1 = 3xTF32 fp32 emulation (what the engine uses wherever a layer runs fp32-accurate),
  * 0 = one tf32 MMA per K step. */
 EV_API int ev_op_attention_tc(const float* qkv, const int32_t* key_lens, float* ctx_out, int B, int L, int H, int n_heads,
                               int tc_mode, void* stream);
@@ -277,7 +277,7 @@ EV_API void ev_style_destroy(ev_style_ctx* ctx);
  * the ones emotivoice_b200.packing.pack_style_state_dict emits ("sty.*"). */
 EV_API int ev_style_bind_weights(ev_style_ctx* ctx, const float* blob, size_t blob_floats, const ev_weight_entry* index,
                                  int n_entries);
-/* EV_PREC_FP32 (3xTF32 on tcgen05, default) or EV_PREC_TF32. */
+/* EV_PREC_FP32 (3xTF32 on the tensor cores, default) or EV_PREC_TF32. */
 EV_API int ev_style_set_precision(ev_style_ctx* ctx, int precision);
 EV_API size_t ev_style_workspace_bytes(const ev_style_ctx* ctx, int B, int N);
 /* StyleEncoder.forward (simbert.py:48-72): ids / type_ids (B,N) int64, lens (B,) int64 = number of leading tokens with

@@ -14,6 +14,9 @@ import numpy as np
 import torch
 
 MAX_WAV_VALUE = 32768.0      # models/hifigan/get_vocoder.py (imported by inference_am_vocoder_joint.py:20)
+# CPU threads of the runs that produce and check the caller fixtures: torch's CPU convolutions split their sums by thread, so
+# the last bit of an int16 sample can depend on the count (1 LSB in a few samples between 8 and 16 threads)
+FIXTURE_THREADS = 8
 
 
 def synthetic_style_embedding(text, seed=1234, dim=768):

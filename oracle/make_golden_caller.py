@@ -32,7 +32,7 @@ def main():
     conf = refshim.load_reference_config(len(token2id), len(speaker2id))
     from emotivoice_b200.config import default_config
     sd = synth.make_state_dict(default_config(len(token2id), len(speaker2id)))
-    torch.set_num_threads(max(1, os.cpu_count() or 1))
+    torch.set_num_threads(caller_loop.FIXTURE_THREADS)
     JETS = refshim.import_reference_jets()
     res = caller_loop.run_caller_loop(JETS, conf, sd, lines, token2id, speaker2id, torch.device("cpu"))
     gold = os.path.join(ROOT, "tests", "golden")

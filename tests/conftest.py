@@ -14,15 +14,15 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):
     """`gpu` tests need a CUDA device AND the in-tree library: on a host without one they are skipped, not errors, so a
-    bare `pytest` is green on the CPU box (the driver runs `-m "not gpu"` here and `-m gpu` on the B200)."""
+    bare `pytest` is green on a machine without a GPU."""
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (sm_100a); there is no CPU path")
+    skip = pytest.mark.skip(reason="needs a CUDA device (sm_90a); there is no CPU path")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

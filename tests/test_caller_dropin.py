@@ -55,7 +55,12 @@ def test_oracle_behind_the_caller_loop_reproduces_the_reference_files_exactly():
     sd = synth.make_state_dict(conf)
     short = [n for n in pcm["line_no"].tolist() if "pcm_%d" % n in pcm.files]
     lines = [meta["lines"][n - 1] for n in short]
-    res = caller_loop.run_caller_loop(OracleJETS, conf, sd, lines, meta["token2id"], meta["speaker2id"], torch.device("cpu"))
+    threads = torch.get_num_threads()
+    torch.set_num_threads(caller_loop.FIXTURE_THREADS)     # the CPU convolutions' summation split depends on the thread count
+    try:
+        res = caller_loop.run_caller_loop(OracleJETS, conf, sd, lines, meta["token2id"], meta["speaker2id"], torch.device("cpu"))
+    finally:
+        torch.set_num_threads(threads)
     assert len(res) == len(short)
     for (_, audio), n in zip(res, short):
         assert audio.dtype == np.int16 and np.array_equal(audio, pcm["pcm_%d" % n])

@@ -2,7 +2,7 @@
 against (a) the committed fixtures generated from the unmodified reference and (b) the
 oracle, plus size-independent properties at larger sizes.
 
-The default precision mode "fp32" is 3xTF32 on the tcgen05 tensor cores (fp32-accurate); the
+The default precision mode "fp32" is 3xTF32 on the tensor cores (fp32-accurate); the
 plain FFMA path ("fp32_ffma") is held to the same bound.
 Tolerances (north_star: "within a stated fp32 mel/waveform tolerance"):
   durations: identical;  mel: max|err| <= 1e-4 * max|mel|;  wav: rms(err) <= 1e-4 * rms(wav).

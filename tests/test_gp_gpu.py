@@ -1,4 +1,4 @@
-"""Granule-planar HiFi-GAN convolution kernel (csrc/conv1d_gp.cu) on the B200.
+"""Granule-planar HiFi-GAN convolution kernel (csrc/conv1d_gp.cu) on the H100.
 
 * operator level (tools/gp_check.py, run as a child under a timeout so a pipeline deadlock cannot take pytest with it):
   BITWISE equality with the round-1 time-major tensor-core kernel in the tf32 and 3xTF32 modes (same reduction order, same
@@ -96,7 +96,7 @@ def test_vocoder_on_the_gp_path_is_bitwise_the_time_major_path(model, dev, tmp_p
 
 @pytest.mark.parametrize("name", ["b1_t12", "b1_t50", "b1_t100"])
 def test_bf16_storage_mode_against_the_reference_fixture(model, dev, name):
-    """ "bf16": bf16 operands AND bf16 activations in HBM through the vocoder (fp32 accumulation in TMEM; the duration prefix
+    """ "bf16": bf16 operands AND bf16 activations in HBM through the vocoder (fp32 accumulation; the duration prefix
     stays 3xTF32, so durations are identical).  Tolerance (SURVEY.md s8d cfg3): mel <= 2e-2 of max|mel|, wav rms <= 2e-2 of rms."""
     g = load_golden(name)
     try:

@@ -177,7 +177,7 @@ def test_attention(lib, dev, B, L, masked):
 @pytest.mark.parametrize("tc_mode,tol", [(1, 2e-5), (0, 3e-3)], ids=["3xtf32", "tf32"])
 @pytest.mark.parametrize("B,L,masked", [(1, 7, False), (1, 64, False), (1, 129, False), (2, 500, True), (3, 1300, True), (1, 2049, False), (4, 65, True)])
 def test_attention_tc(lib, dev, B, L, masked, tc_mode, tol):
-    """encoder.py:84-109 on the tensor cores (csrc/attention_tc.cu): QK^T / PV as tcgen05.mma, softmax between two TMEM reads.
+    """encoder.py:84-109 on the tensor cores (csrc/attention_tc.cu): QK^T / PV as wgmma, softmax on the register accumulators.
     3xTF32 is held to the fp32 FFMA kernel's tolerance class (2e-5 of max|ref|); one tf32 MMA per step to 3e-3."""
     H, heads, dk = 384, 8, 48
     g = torch.Generator().manual_seed(L + 17 * B)
@@ -216,7 +216,7 @@ def test_attention_tc(lib, dev, B, L, masked, tc_mode, tol):
 def test_attention_tc_lazy_rescale_path(lib, dev, tc_mode, tol):                               # in the exponent (inherent to tf32 operands)
     """The online softmax only rescales O / l when a key tile's row maximum exceeds the running one by more than 8.  Random
     scores never do, so this case makes them: the keys grow by a factor per 64-key tile (every tile after the first triggers
-    the TMEM load / multiply / store of the accumulator), for some rows only (the warp-collective decision must leave the
+    the multiply of the accumulator registers), for some rows only (the warp-collective decision must leave the
     other rows exact), with a ragged second item."""
     H, heads, dk, B, L = 384, 8, 48, 2, 400
     g = torch.Generator().manual_seed(77)

@@ -1,7 +1,7 @@
-"""tcgen05 implicit-GEMM convolution (conv1d_tc.cu) and the precision modes of the engine.
+"""Tensor-core implicit-GEMM convolution (conv1d_tc.cu) and the precision modes of the engine.
 
 Per-operator tolerances against a torch fp32 CPU reference:
-  1xTF32 (operands rounded to nearest tf32, 10-bit mantissa, fp32 accumulation in TMEM): 3e-3 * max|ref|
+  1xTF32 (operands rounded to nearest tf32, 10-bit mantissa, fp32 accumulation): 3e-3 * max|ref|
   3xTF32 (fp32 emulation: hi/lo split, three MMAs per K step):                          5e-5 * max|ref|
     (measured 2e-6 .. 2.1e-5, the largest at K = 3*1536; the fp32 FFMA kernel is held to 2e-5).
 End to end in "tf32" mode: mel <= 5e-3 * max|mel|, wav rms <= 2e-2 * rms(wav); durations identical in

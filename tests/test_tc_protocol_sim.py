@@ -1,12 +1,14 @@
-"""Discrete-event model of the mbarrier protocols of the two tcgen05 kernels (csrc/conv1d_tc.cu, csrc/conv1d_gp.cu).
+"""Discrete-event model of the mbarrier protocols of the Hopper tensor-core kernels (csrc/conv1d_tc.cu, csrc/conv1d_gp.cu,
+csrc/resblock_gp.cu).
 
 Both deadlocks of round 1 were protocol bugs that a GPU can only show as a hang (producer groups running two ring phases
-ahead of a parity wait; epilogue warps releasing an accumulator they never waited for).  This model replays the kernels' role
-loops -- producers (in groups), weight loader, MMA issuer, epilogue warps -- as coroutines over barriers with the hardware's
-semantics (arrival count, phase bit, `try_wait.parity(P)` passes iff the current phase parity != P; `tcgen05.commit` arrives
-when every MMA issued before it has completed; MMAs read their operands as late as their completion) under many random
-schedules, and checks: no deadlock, every slot holds the expected contents when it is read, no slot is overwritten before its
-last reader is done.  The role loops are transcribed from the kernels; the planner (ring depths, groups) is the real one.
+ahead of a parity wait; a consumer releasing a buffer it never waited for).  This model replays the kernels' role loops --
+producers (in groups) or bulk-copy loader + transform warps, weight loader, the eight consumer warps -- as coroutines over
+barriers with the hardware's semantics (arrival count, phase bit, `try_wait.parity(P)` passes iff the current phase parity
+!= P; a wgmma reads its shared-memory operands until `wgmma.wait_group` has seen it complete, which the consumers do one
+step after issuing it) under many random schedules, and checks: no deadlock, every slot holds the expected contents when it
+is read, no slot is overwritten before its last reader is done.  The role loops are transcribed from the kernels; the
+planner (ring depths, groups) is the real one.
 """
 import ctypes
 import random
@@ -15,7 +17,7 @@ import pytest
 
 from emotivoice_b200 import _abi
 
-NEPI_WARPS = 8
+NCONS_WARPS = 8
 NPWARPS = 6
 
 
@@ -36,35 +38,22 @@ class Bar:
 
 class Sim:
     """Cooperative scheduler.  Roles are generators yielding ('wait', bar, parity) | ('arrive', bar) | ('write', slot, tag)
-    | ('read', slot, tag) | ('mma_read', slot, tag) | ('commit', bar).  MMA reads are deferred to the next commit's
-    completion, and commits complete in order at a random later time: the most adversarial timing the hardware allows."""
+    | ('read', slot, tag); a random runnable role advances each step."""
 
     def __init__(self, seed):
         self.rng = random.Random(seed)
         self.slots = {}
         self.roles = []
-        self.inflight = []           # [(reads, bars)] groups of MMAs closed by a commit, oldest first
-        self.open_reads = []
 
     def add(self, name, gen):
         self.roles.append([name, gen, None])
 
-    def _complete_oldest(self):
-        reads, bars = self.inflight.pop(0)
-        for slot, tag in reads:
-            assert self.slots.get(slot) == tag, "MMA read %s: holds %r, expected %r" % (slot, self.slots.get(slot), tag)
-        for b in bars:
-            b.arrive()
-
     def run(self, max_steps=2_000_000):
         live = list(self.roles)
         for _ in range(max_steps):
-            if not live and not self.inflight:
+            if not live:
                 return
             runnable = [r for r in live if r[2] is None or r[2][0].passes(r[2][1])]
-            if self.inflight and (not runnable or self.rng.random() < 0.3):
-                self._complete_oldest()
-                continue
             if not runnable:
                 raise AssertionError("deadlock: %r" % ([(r[0], r[2][1], r[2][0].phase) for r in live],))
             role = self.rng.choice(runnable)
@@ -84,30 +73,46 @@ class Sim:
                 self.slots[ev[1]] = ev[2]
             elif kind == "read":
                 assert self.slots.get(ev[1]) == ev[2], "%s read %s: holds %r, expected %r" % (name, ev[1], self.slots.get(ev[1]), ev[2])
-            elif kind == "mma_read":
-                self.open_reads.append((ev[1], ev[2]))
-            elif kind == "commit":
-                if self.inflight and not self.open_reads:
-                    self.inflight[-1][1].append(ev[1])      # back-to-back commits track the same MMAs
-                else:
-                    self.inflight.append((self.open_reads, [ev[1]]))
-                    self.open_reads = []
         raise AssertionError("simulation did not finish")
+
+
+def mma_steps(steps, b_empty, early_release=False):
+    """A consumer warp's main loop over `steps` = [(wait_list, reads, releases)]: wait for the step's operands, issue its MMAs, then
+    (wgmma.wait_group 1) the PREVIOUS step's MMAs have completed -- their operand reads happen up to here -- and its stages are handed
+    back.  early_release: the bug the kernels must not have, releasing a step's stages at issue, before its MMAs have read them."""
+    prev = None
+    for waits, reads, releases in steps:
+        for bar, parity in waits:
+            yield ("wait", bar, parity)
+        if early_release:
+            for bar in releases:
+                yield ("arrive", bar)
+        if prev is not None:
+            for slot, tag in prev[0]:
+                yield ("read", slot, tag)
+            if not early_release:
+                for bar in prev[1]:
+                    yield ("arrive", bar)
+        prev = (reads, releases)
+    if prev is not None:                                       # wgmma.wait_group 0
+        for slot, tag in prev[0]:
+            yield ("read", slot, tag)
+        if not early_release:
+            for bar in prev[1]:
+                yield ("arrive", bar)
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # conv1d_tc.cu
 # ------------------------------------------------------------------------------------------------------------------
-def sim_conv(seed, tiles, n_cb, K, a_stages, b_stages, ngroups, epi_idle_warps=0, idle_warps_skip_wait=False):
+def sim_conv(seed, tiles, n_cb, K, a_stages, b_stages, ngroups, early_release=False):
     """tiles: list of booleans (True = active tile, False = padding tile that every role skips)."""
     sim = Sim(seed)
     wpg = NPWARPS // ngroups
     a_full = [Bar(wpg) for _ in range(a_stages)]            # one arrival per producer warp here (the kernel: per thread)
-    a_empty = [Bar(1) for _ in range(a_stages)]
+    a_empty = [Bar(NCONS_WARPS) for _ in range(a_stages)]
     b_full = [Bar(1) for _ in range(b_stages)]
-    b_empty = [Bar(1) for _ in range(b_stages)]
-    acc_full = [Bar(1), Bar(1)]
-    acc_empty = [Bar(NEPI_WARPS), Bar(NEPI_WARPS)]
+    b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
 
     def producer(grp, w):
         a_cnt = 0
@@ -136,56 +141,36 @@ def sim_conv(seed, tiles, n_cb, K, a_stages, b_stages, ngroups, epi_idle_warps=0
                     yield ("arrive", b_full[sb])           # expect_tx + complete_tx of the bulk copy
                     b_cnt += 1
 
-    def mma():
-        a_cnt = b_cnt = tile_cnt = 0
+    def consumer():
+        a_cnt = b_cnt = 0
         for ti, active in enumerate(tiles):
             if not active:
                 continue
-            buf = tile_cnt & 1
-            yield ("wait", acc_empty[buf], ((tile_cnt >> 1) & 1) ^ 1)
+            steps = []
             for cb in range(n_cb):
                 sa = a_cnt % a_stages
-                yield ("wait", a_full[sa], (a_cnt // a_stages) & 1)
                 for j in range(K):
                     sb = b_cnt % b_stages
-                    yield ("wait", b_full[sb], (b_cnt // b_stages) & 1)
-                    yield ("mma_read", ("A", sa), (ti, cb))
-                    yield ("mma_read", ("B", sb), (ti, cb, j))
-                    yield ("commit", b_empty[sb])
+                    waits = ([(a_full[sa], (a_cnt // a_stages) & 1)] if j == 0 else []) + [(b_full[sb], (b_cnt // b_stages) & 1)]
+                    steps.append((waits, [(("A", sa), (ti, cb)), (("B", sb), (ti, cb, j))],
+                                  [b_empty[sb]] + ([a_empty[sa]] if j == K - 1 else [])))
                     b_cnt += 1
-                yield ("commit", a_empty[sa])
                 a_cnt += 1
-            yield ("write", ("ACC", buf), ti)                # (written as the MMAs complete; conservatively at issue)
-            yield ("commit", acc_full[buf])
-            tile_cnt += 1
-
-    def epilogue(w):
-        tile_cnt = 0
-        for ti, active in enumerate(tiles):
-            if not active:
-                continue
-            buf = tile_cnt & 1
-            if not (idle_warps_skip_wait and w < epi_idle_warps):
-                yield ("wait", acc_full[buf], (tile_cnt >> 1) & 1)  # idle warps (no columns) wait too: the round-1 fix
-            if w >= epi_idle_warps:
-                yield ("read", ("ACC", buf), ti)
-            yield ("arrive", acc_empty[buf])
-            tile_cnt += 1
+            yield from mma_steps(steps, b_empty, early_release)
 
     for g in range(ngroups):
         for w in range(wpg):
             sim.add("producer%d.%d" % (g, w), producer(g, w))
     sim.add("loader", loader())
-    sim.add("mma", mma())
-    for w in range(NEPI_WARPS):
-        sim.add("epilogue%d" % w, epilogue(w))
+    for w in range(NCONS_WARPS):
+        sim.add("consumer%d" % w, consumer())
     sim.run()
 
 
 def _tc_plan(lib, B, L, Cin, Cout, K, dil, mode, ksplit=0):
     v = (ctypes.c_int * 11)()
     assert lib.ev_debug_tc_plan(B, L, Cin, Cout, K, dil, mode, ksplit, v) == 0
-    return dict(zip("BN MT KBG a_stages b_stages groups ksplit tmem smem tiles rows_pad".split(), list(v)))
+    return dict(zip("BN MT KBG a_stages b_stages groups ksplit acc smem tiles rows_pad".split(), list(v)))
 
 
 @pytest.fixture(scope="module")
@@ -206,17 +191,18 @@ def test_conv_protocol_with_the_real_plans(lib, shape, mode):
     for seed in range(6):
         rng = random.Random(seed)
         tiles = [rng.random() > 0.2 for _ in range(rng.randint(1, 5))]       # tiles of ONE persistent CTA, some of them padding
-        sim_conv(seed, tiles, n_cb, K, pl["a_stages"], pl["b_stages"], pl["groups"], epi_idle_warps=4 if Cout <= 32 else 0)
+        sim_conv(seed, tiles, n_cb, K, pl["a_stages"], pl["b_stages"], pl["groups"])
 
 
 def test_conv_protocol_model_catches_the_round1_bugs():
-    """The model is only worth something if it fails on the two protocols that hung the GPU in round 1."""
+    """The model is only worth something if it fails on the protocol that hung the GPU in round 1 and on a consumer that hands a
+    stage back before its MMAs have read it."""
     with pytest.raises(AssertionError):                       # 6 producer groups on a 2-deep ring: parity cannot tell phases apart
         for seed in range(20):
             sim_conv(seed, [True, True, True], n_cb=12, K=3, a_stages=2, b_stages=4, ngroups=6)
-    with pytest.raises(AssertionError):                       # column-less epilogue warps handing back an accumulator they never waited for
+    with pytest.raises(AssertionError):                       # stages released at issue, before wgmma.wait_group
         for seed in range(50):
-            sim_conv(seed, [True] * 6, n_cb=2, K=3, a_stages=2, b_stages=4, ngroups=2, epi_idle_warps=4, idle_warps_skip_wait=True)
+            sim_conv(seed, [True] * 6, n_cb=2, K=3, a_stages=2, b_stages=2, ngroups=2, early_release=True)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -225,19 +211,16 @@ def test_conv_protocol_model_catches_the_round1_bugs():
 NTW = 4
 
 
-def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, n_work_items=2, skip_idle_wait=False):
-    """tiles: list of booleans (True = active tile, False = padding tile that every role skips).  n_work_items: epilogue
-    work items (MT * BN/32) per lane quadrant; warp `half` of a quadrant takes items half, half+2, ...: with one item the
-    second warp of each quadrant has nothing to read but must still follow the accumulator phases."""
+def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, early_release=False):
+    """tiles: list of booleans (True = active tile, False = padding tile that every role skips); K: taps, or taps per tile (a
+    grouped launch)."""
     sim = Sim(seed)
     taps = (lambda ti: K[ti]) if isinstance(K, (list, tuple)) else (lambda ti: K)     # grouped launch: the taps differ from tile to tile
     a_full = [Bar(1) for _ in range(a_stages)]
     a_ready = [Bar(NTW) for _ in range(a_stages)]           # one arrival per transform warp here (the kernel: per thread)
-    a_empty = [Bar(1) for _ in range(a_stages)]
+    a_empty = [Bar(NCONS_WARPS) for _ in range(a_stages)]
     b_full = [Bar(1) for _ in range(b_stages)]
-    b_empty = [Bar(1) for _ in range(b_stages)]
-    acc_full = [Bar(1), Bar(1)]
-    acc_empty = [Bar(NEPI_WARPS), Bar(NEPI_WARPS)]
+    b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
 
     def aloader():
         a_cnt = 0
@@ -278,58 +261,36 @@ def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, n_work_items=2, skip_idle_w
                     yield ("arrive", b_full[sb])
                     b_cnt += 1
 
-    def mma():
-        a_cnt = b_cnt = tile_cnt = 0
+    def consumer():
+        a_cnt = b_cnt = 0
         for ti, active in enumerate(tiles):
             if not active:
                 continue
-            buf = tile_cnt & 1
-            yield ("wait", acc_empty[buf], ((tile_cnt >> 1) & 1) ^ 1)
+            steps = []
             for cb in range(n_cb):
                 sa = a_cnt % a_stages
-                yield ("wait", a_ready[sa], (a_cnt // a_stages) & 1)
                 for j in range(taps(ti)):
                     sb = b_cnt % b_stages
-                    yield ("wait", b_full[sb], (b_cnt // b_stages) & 1)
-                    yield ("mma_read", ("A", sa), ("op", ti, cb))
-                    yield ("mma_read", ("B", sb), (ti, cb, j))
-                    yield ("commit", b_empty[sb])
+                    waits = ([(a_ready[sa], (a_cnt // a_stages) & 1)] if j == 0 else []) + [(b_full[sb], (b_cnt // b_stages) & 1)]
+                    steps.append((waits, [(("A", sa), ("op", ti, cb)), (("B", sb), (ti, cb, j))],
+                                  [b_empty[sb]] + ([a_empty[sa]] if j == taps(ti) - 1 else [])))
                     b_cnt += 1
-                yield ("commit", a_empty[sa])
                 a_cnt += 1
-            yield ("write", ("ACC", buf), ti)
-            yield ("commit", acc_full[buf])
-            tile_cnt += 1
-
-    def epilogue(w):
-        half = w >> 2
-        has_work = half < n_work_items
-        tile_cnt = 0
-        for ti, active in enumerate(tiles):
-            if not active:
-                continue
-            buf = tile_cnt & 1
-            if has_work or not skip_idle_wait:
-                yield ("wait", acc_full[buf], (tile_cnt >> 1) & 1)
-            if has_work:
-                yield ("read", ("ACC", buf), ti)
-            yield ("arrive", acc_empty[buf])
-            tile_cnt += 1
+            yield from mma_steps(steps, b_empty, early_release)
 
     sim.add("aloader", aloader())
     for w in range(NTW):
         sim.add("xform%d" % w, xform(w))
     sim.add("bloader", bloader())
-    sim.add("mma", mma())
-    for w in range(NEPI_WARPS):
-        sim.add("epilogue%d" % w, epilogue(w))
+    for w in range(NCONS_WARPS):
+        sim.add("consumer%d" % w, consumer())
     sim.run()
 
 
 def _gp_plan(lib, B, L, Cin, Cout, K, dil, rate, mode):
     v = (ctypes.c_int * 11)()
     assert lib.ev_debug_gp_plan(B, L, Cin, Cout, K, dil, rate, mode, v) == 0, lib.ev_last_error()
-    return dict(zip("BN MT KBG a_stages b_stages ntw planes tmem smem tiles rows_pad".split(), list(v)))
+    return dict(zip("BN MT KBG a_stages b_stages ntw planes acc smem tiles rows_pad".split(), list(v)))
 
 
 GP_SHAPES = [(1, 537, 80, 512, 7, 1, 1), (1, 537, 512, 2048, 3, 1, 8), (1, 4296, 256, 256, 11, 5, 1), (1, 34368, 128, 128, 11, 1, 1),
@@ -344,18 +305,17 @@ def test_gp_plans_respect_the_hardware_limits_and_the_protocol(lib, shape, mode)
     pl = _gp_plan(lib, B, L, Cin, Cout, K, dil, rate, mode)
     cpg = 8 if mode == 2 else 4
     assert pl["smem"] <= 227 * 1024 and 2 <= pl["a_stages"] <= 8 and 1 <= pl["b_stages"] <= 8
-    assert pl["tmem"] in (32, 64, 128, 256, 512) and 2 * pl["MT"] * pl["BN"] <= pl["tmem"]
+    assert pl["acc"] == pl["MT"] * pl["BN"] <= 128        # register accumulators: MT x BN columns x 64 rows per consumer warpgroup
     assert pl["BN"] % 32 == 0 and Cout % pl["BN"] == 0 and pl["planes"] == (2 if mode == 1 else 1)
     rows = 128 * pl["MT"] + (K - 1) * dil
     assert pl["rows_pad"] >= rows and pl["rows_pad"] % 8 == 0
     # one stage's transaction count must fit the mbarrier tx-count field (2^20 - 1 bytes)
     assert pl["KBG"] * pl["rows_pad"] * 16 < (1 << 20) and pl["planes"] * pl["KBG"] * pl["BN"] * 16 < (1 << 20)
     n_cb = -(-Cin // (cpg * pl["KBG"]))
-    items = pl["MT"] * (pl["BN"] // 32)
     for seed in range(5):
         rng = random.Random(seed)
         tiles = [rng.random() > 0.2 for _ in range(rng.randint(1, 5))]
-        sim_gp(seed, tiles, min(n_cb, 6), K, pl["a_stages"], pl["b_stages"], n_work_items=items)
+        sim_gp(seed, tiles, min(n_cb, 6), K, pl["a_stages"], pl["b_stages"])
 
 
 def test_gp_summation_order_parameters_do_not_depend_on_batch_or_length(lib):
@@ -372,7 +332,7 @@ def _gp_group_plan(lib, Ks, dils, B, L, Cin, Cout, mode):
     v = (ctypes.c_int * 11)()
     IA = ctypes.c_int * n
     assert lib.ev_debug_gp_group_plan(n, IA(*Ks), IA(*dils), B, L, Cin, Cout, mode, v) == 0, lib.ev_last_error()
-    return dict(zip("BN MT KBG a_stages b_stages ntw planes tmem smem tiles rows_pad".split(), list(v)))
+    return dict(zip("BN MT KBG a_stages b_stages ntw planes acc smem tiles rows_pad".split(), list(v)))
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2, 3])
@@ -386,7 +346,7 @@ def test_gp_grouped_launch_plans(lib, shape, mode):
     g = _gp_group_plan(lib, Ks, dils, B, L, C, C, mode)
     solo = [_gp_plan(lib, B, L, C, C, K, d, 1, mode) for K, d in zip(Ks, dils)]
     assert {p["KBG"] for p in solo} == {g["KBG"]}
-    assert g["smem"] <= 227 * 1024 and 2 * g["MT"] * g["BN"] <= g["tmem"] <= 512
+    assert g["smem"] <= 227 * 1024 and g["acc"] == g["MT"] * g["BN"] <= 128
     assert g["rows_pad"] >= 128 * g["MT"] + (11 - 1) * 5 and g["rows_pad"] % 8 == 0
     tiles_one = B * -(-L // (128 * g["MT"])) * (C // g["BN"])
     assert g["tiles"] == 3 * tiles_one
@@ -394,7 +354,7 @@ def test_gp_grouped_launch_plans(lib, shape, mode):
     for seed in range(3):
         rng = random.Random(seed)
         n = rng.randint(2, 6)
-        sim_gp(seed, [True] * n, min(n_cb, 4), [rng.choice(Ks) for _ in range(n)], g["a_stages"], g["b_stages"], n_work_items=g["MT"] * (g["BN"] // 32))
+        sim_gp(seed, [True] * n, min(n_cb, 4), [rng.choice(Ks) for _ in range(n)], g["a_stages"], g["b_stages"])
 
 
 @pytest.mark.parametrize("mode", [0, 2, 3])
@@ -406,11 +366,11 @@ def test_gp_grouped_launch_plans_over_utterance_lengths(lib, C, mul, mode):
         g = _gp_group_plan(lib, (3, 7, 11), (1, 3, 5), 1, L, C, C, mode)
         assert g["KBG"] == _gp_plan(lib, 1, L, C, C, 11, 5, 1, mode)["KBG"] == _gp_plan(lib, 1, L, C, C, 3, 1, 1, mode)["KBG"]
         assert g["tiles"] == 3 * -(-L // (128 * g["MT"])) * (C // g["BN"]) and g["MT"] in (1, 2, 4)
-        assert g["smem"] <= 227 * 1024 and 2 * g["MT"] * g["BN"] <= g["tmem"] <= 512 and g["rows_pad"] >= 128 * g["MT"] + 50
+        assert g["smem"] <= 227 * 1024 and g["acc"] == g["MT"] * g["BN"] <= 128 and g["rows_pad"] >= 128 * g["MT"] + 50
 
 
 def test_gp_grouped_launch_plan_fills_the_machine_at_batch_1(lib):
-    """HiFi-GAN stage 1 at batch 1 in the fp32 mode: 3 x 68 one-accumulator tiles (204 > 148 SMs) instead of 3 x 34 two-accumulator
+    """HiFi-GAN stage 1 at batch 1 in the fp32 mode: 3 x 68 one-accumulator tiles (204 > 132 SMs) instead of 3 x 34 two-accumulator
     ones -- the plan is picked by simulating the round-robin deal, where the k = 11 member's double tile would be the critical path."""
     g = _gp_group_plan(lib, (3, 7, 11), (1, 3, 5), 1, 4296, 256, 256, 3)
     assert g["MT"] == 1 and g["tiles"] == 204
@@ -425,7 +385,7 @@ def test_gp_grouped_launch_protocol():
         n = rng.randint(2, 7)
         tiles = [rng.random() > 0.15 for _ in range(n)]
         taps = [rng.choice((3, 7, 11)) for _ in range(n)]
-        sim_gp(seed, tiles, rng.randint(1, 4), taps, rng.randint(2, 4), rng.randint(2, 8), n_work_items=rng.choice((1, 2, 4)))
+        sim_gp(seed, tiles, rng.randint(1, 4), taps, rng.randint(2, 4), rng.randint(2, 8))
 
 
 @pytest.mark.parametrize("mode", [0, 2, 3])
@@ -450,7 +410,7 @@ def test_resblock_gp_grouped_launch_plans_over_utterance_lengths(lib, C, mul, mo
             assert rc != 0          # a member that would not be fused on its own is never grouped
             continue
         assert rc == 0, lib.ev_last_error()
-        mt, kbg, total, rows1_pad, rows2_pad, smem, tmem = list(v)[:7]
+        mt, kbg, total, rows1_pad, rows2_pad, smem, acc = list(v)[:7]
         members = [tuple(v[7 + 3 * i: 10 + 3 * i]) for i in range(3)]
         seen_mt.add(mt)
         assert mt in (2, 4) and {x[1] for x in solo} == {kbg}
@@ -462,13 +422,13 @@ def test_resblock_gp_grouped_launch_plans_over_utterance_lengths(lib, C, mul, mo
             t0 += tiles_m
         assert total == t0
         assert rows1_pad >= 128 * mt + 10 * 5 and rows2_pad >= 128 * mt + 10 and rows1_pad % 8 == 0 and rows2_pad % 8 == 0
-        assert smem <= 227 * 1024 and 4 * mt * C <= tmem <= 512
+        assert smem <= 227 * 1024 and acc == mt * C <= 128
     assert seen_mt
 
 
 def test_resblock_gp_grouped_launch_protocol():
     """Grouped fused-ResBlock launch: consecutive tiles of a CTA may belong to layers with different taps; the weight loader streams
-    w1 of the NEXT tile's layer, then w2 of the current one, exactly as the MMA issuer consumes them."""
+    w1 then w2 of each tile's own layer, exactly as the consumers read them."""
     for seed in range(30):
         rng = random.Random(seed)
         n = rng.randint(1, 6)
@@ -476,35 +436,31 @@ def test_resblock_gp_grouped_launch_protocol():
 
 
 def test_gp_protocol_model_is_sensitive():
-    """The model must fail when an epilogue warp without work items releases an accumulator set it never waited for
-    (the round-1 hang), which is why the kernel's idle warps still wait on acc_full."""
+    """The model must fail when the consumers hand a stage back before wgmma.wait_group has seen the MMAs that read it complete
+    (the conv1d_gp and fused-ResBlock consumers release one step behind the issue for that reason)."""
     with pytest.raises(AssertionError):
         for seed in range(40):
-            sim_gp(seed, [True] * 5, n_cb=1, K=1, a_stages=2, b_stages=2, n_work_items=1, skip_idle_wait=True)
+            sim_gp(seed, [True] * 5, n_cb=2, K=3, a_stages=2, b_stages=2, early_release=True)
+    with pytest.raises(AssertionError):
+        for seed in range(40):
+            sim_pair(seed, 3, 2, 3, 2, 2, early_release=True)
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# resblock_gp.cu: C1(0) | C1(i+1), C2(i); epi1 writes the xt tile between them; separate epilogue warp groups
+# resblock_gp.cu: per tile c1 -> epi1 (xt tile in shared memory) -> c2 -> epi2, all in the consumer warps
 # ------------------------------------------------------------------------------------------------------------------
-def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages):
+def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages, early_release=False):
+    """Per tile, every consumer warp runs c1 over the x ring, epi1 into the shared xt tile between two named barriers of the eight
+    consumer warps (the first: both warpgroups' c2 of the previous tile have read the tile; the second: it is complete), then c2
+    over the xt tile; the weight loader streams w1 then w2 of every tile."""
     sim = Sim(seed)
     taps = (lambda ti: K[ti]) if isinstance(K, (list, tuple)) else (lambda ti: K)     # grouped launch: the taps differ from tile to tile
     a_full = [Bar(1) for _ in range(a_stages)]
     a_ready = [Bar(NTW) for _ in range(a_stages)]
-    a_empty = [Bar(1) for _ in range(a_stages)]
+    a_empty = [Bar(NCONS_WARPS) for _ in range(a_stages)]
     b_full = [Bar(1) for _ in range(b_stages)]
-    b_empty = [Bar(1) for _ in range(b_stages)]
-    acc1_full, acc1_empty = [Bar(1), Bar(1)], [Bar(4), Bar(4)]
-    acc2_full, acc2_empty = [Bar(1), Bar(1)], [Bar(4), Bar(4)]
-    a2_full, a2_empty = Bar(4), Bar(1)                  # one arrival per epi1 warp here (the kernel: per thread)
-
-    def order():                                         # the MMA issuer's / weight loader's schedule
-        if n_tiles:
-            yield (1, 0)
-        for i in range(n_tiles):
-            if i + 1 < n_tiles:
-                yield (1, i + 1)
-            yield (2, i)
+    b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
+    named = Bar(NCONS_WARPS)                                # bar.sync 1, 256
 
     def aloader():
         a_cnt = 0
@@ -530,76 +486,55 @@ def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages):
 
     def bloader():
         b_cnt = 0
-        for which, ti in order():
+        for ti in range(n_tiles):
+            for which in (1, 2):
+                for cb in range(n_cb):
+                    for j in range(taps(ti)):
+                        sb = b_cnt % b_stages
+                        yield ("wait", b_empty[sb], ((b_cnt // b_stages) & 1) ^ 1)
+                        yield ("write", ("B", sb), (which, ti, cb, j))
+                        yield ("arrive", b_full[sb])
+                        b_cnt += 1
+
+    def consumer(w):
+        a_cnt = b_cnt = uses = 0
+
+        def bar_sync():
+            nonlocal uses
+            yield ("arrive", named)
+            yield ("wait", named, uses & 1)
+            uses += 1
+
+        for ti in range(n_tiles):
+            steps = []
+            for cb in range(n_cb):
+                sa = a_cnt % a_stages
+                for j in range(taps(ti)):
+                    sb = b_cnt % b_stages
+                    waits = ([(a_ready[sa], (a_cnt // a_stages) & 1)] if j == 0 else []) + [(b_full[sb], (b_cnt // b_stages) & 1)]
+                    steps.append((waits, [(("X", sa), ("op", ti, cb)), (("B", sb), (1, ti, cb, j))],
+                                  [b_empty[sb]] + ([a_empty[sa]] if j == taps(ti) - 1 else [])))
+                    b_cnt += 1
+                a_cnt += 1
+            yield from mma_steps(steps, b_empty, early_release)
+            yield from bar_sync()
+            yield ("write", ("A2", w), ti)                   # this warp's rows of the xt tile
+            yield from bar_sync()
+            steps = []
             for cb in range(n_cb):
                 for j in range(taps(ti)):
                     sb = b_cnt % b_stages
-                    yield ("wait", b_empty[sb], ((b_cnt // b_stages) & 1) ^ 1)
-                    yield ("write", ("B", sb), (which, ti, cb, j))
-                    yield ("arrive", b_full[sb])
+                    reads = [(("A2", v), ti) for v in range(NCONS_WARPS)] + [(("B", sb), (2, ti, cb, j))]
+                    steps.append(([(b_full[sb], (b_cnt // b_stages) & 1)], reads, [b_empty[sb]]))
                     b_cnt += 1
-
-    def mma():
-        a_cnt = b_cnt = 0
-        for which, ti in order():
-            buf = ti & 1
-            if which == 1:
-                yield ("wait", acc1_empty[buf], ((ti >> 1) & 1) ^ 1)
-                for cb in range(n_cb):
-                    sa = a_cnt % a_stages
-                    yield ("wait", a_ready[sa], (a_cnt // a_stages) & 1)
-                    for j in range(taps(ti)):
-                        sb = b_cnt % b_stages
-                        yield ("wait", b_full[sb], (b_cnt // b_stages) & 1)
-                        yield ("mma_read", ("X", sa), ("op", ti, cb))
-                        yield ("mma_read", ("B", sb), (1, ti, cb, j))
-                        yield ("commit", b_empty[sb])
-                        b_cnt += 1
-                    yield ("commit", a_empty[sa])
-                    a_cnt += 1
-                yield ("write", ("ACC1", buf), ti)
-                yield ("commit", acc1_full[buf])
-            else:
-                yield ("wait", a2_full, ti & 1)
-                yield ("wait", acc2_empty[buf], ((ti >> 1) & 1) ^ 1)
-                for cb in range(n_cb):
-                    for j in range(taps(ti)):
-                        sb = b_cnt % b_stages
-                        yield ("wait", b_full[sb], (b_cnt // b_stages) & 1)
-                        yield ("mma_read", ("A2",), ti)
-                        yield ("mma_read", ("B", sb), (2, ti, cb, j))
-                        yield ("commit", b_empty[sb])
-                        b_cnt += 1
-                yield ("write", ("ACC2", buf), ti)
-                yield ("commit", a2_empty)
-                yield ("commit", acc2_full[buf])
-
-    def epi1(w):
-        for ti in range(n_tiles):
-            buf = ti & 1
-            yield ("wait", acc1_full[buf], (ti >> 1) & 1)
-            yield ("wait", a2_empty, (ti & 1) ^ 1)
-            yield ("read", ("ACC1", buf), ti)
-            if w == 0:
-                yield ("write", ("A2",), ti)
-            yield ("arrive", a2_full)
-            yield ("arrive", acc1_empty[buf])
-
-    def epi2(w):
-        for ti in range(n_tiles):
-            buf = ti & 1
-            yield ("wait", acc2_full[buf], (ti >> 1) & 1)
-            yield ("read", ("ACC2", buf), ti)
-            yield ("arrive", acc2_empty[buf])
+            yield from mma_steps(steps, b_empty, early_release)
 
     sim.add("aloader", aloader())
     for w in range(NTW):
         sim.add("xform%d" % w, xform(w))
     sim.add("bloader", bloader())
-    sim.add("mma", mma())
-    for w in range(4):
-        sim.add("epi1_%d" % w, epi1(w))
-        sim.add("epi2_%d" % w, epi2(w))
+    for w in range(NCONS_WARPS):
+        sim.add("consumer%d" % w, consumer(w))
     sim.run()
 
 
@@ -608,8 +543,8 @@ def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages):
 def test_resblock_gp_protocol_with_the_real_plans(lib, C, K, dil, mode):
     v = (ctypes.c_int * 11)()
     assert lib.ev_debug_resblock_gp_plan(1, 137472, C, K, dil, mode, v) == 0, lib.ev_last_error()
-    pl = dict(zip("MT KBG a_stages b_stages ntw tmem smem tiles R rows1_pad rows2_pad".split(), list(v)))
-    assert pl["smem"] <= 227 * 1024 and 4 * pl["MT"] * C <= pl["tmem"] <= 512 and pl["a_stages"] >= 2 and pl["b_stages"] >= 2
+    pl = dict(zip("MT KBG a_stages b_stages ntw acc smem tiles R rows1_pad rows2_pad".split(), list(v)))
+    assert pl["smem"] <= 227 * 1024 and pl["acc"] == pl["MT"] * C <= 128 and pl["a_stages"] >= 2 and pl["b_stages"] >= 2
     assert pl["R"] == 128 * pl["MT"] - (K - 1) and pl["rows1_pad"] >= 128 * pl["MT"] + (K - 1) * dil and pl["rows2_pad"] >= 128 * pl["MT"] + K - 1
     cpg = 8 if mode == 2 else 4
     n_cb = -(-C // (cpg * pl["KBG"]))

@@ -1,6 +1,6 @@
 """GPU tests written after the last hardware run of round 1 (the round's GPU budget was spent): the bf16 precision
 mode, per operator and end to end, and the micro-batching queue on the real engine.  The file name sorts last on
-purpose: the driver runs `pytest -m gpu -x`, and a failure in a test that has never seen a B200 must not hide the
+purpose: under `pytest -m gpu -x` a failure in a test that has never run on a GPU must not hide the
 suite that has.  The bf16 forward itself was measured once (tools/quick_fwd.py bf16: durations identical, wav 8.8e-4);
 the tolerances are <= 4x the CPU emulation of the mode (profiles/r01_precision_emulation_cpu.json).  Fold these back
 into test_tc_gpu.py / test_e2e_gpu.py once they have run green on hardware."""
@@ -254,7 +254,7 @@ print("ALTERNATE_OK" if ok else "ALTERNATE_MISMATCH", flush=True)
 def test_back_to_back_batches_of_different_lengths():
     """Programmatic dependent launch lets a kernel start while its predecessors still run; the int32 lengths are written by the first
     kernel of a forward.  A role that read them before griddepcontrol.wait would decode tiles from the PREVIOUS batch's lengths: wrong
-    results or -- roles disagreeing on the tile sequence -- a deadlock (that happened once: tcgen05 roles that skipped the wait).
+    results or -- roles disagreeing on the tile sequence -- a deadlock (that happened once: tensor-core kernel roles that skipped the wait).
     Alternating batches of very different lengths without host synchronisation must reproduce their first results bit for bit."""
     import subprocess
     import sys
@@ -264,7 +264,7 @@ def test_back_to_back_batches_of_different_lengths():
 
 
 def test_alignment_module_and_segments_match_reference_fixture(lib, dev):
-    """The rest of SURVEY.md s8f rank 4: AlignmentModule.forward (five 3xTF32 convolutions on tcgen05 + the distance /
+    """The rest of SURVEY.md s8f rank 4: AlignmentModule.forward (five 3xTF32 convolutions on the tensor cores + the distance /
     log-softmax kernel + the host-built prior) against the unmodified reference module's output (1e-4 on finite entries, the
     -inf pattern identical), and get_random_segments / get_segments bit-exact (same torch RNG calls as the reference)."""
     from emotivoice_b200 import align, synth

@@ -1,4 +1,4 @@
-"""Secondary comparison (BASELINE.md s3 item 4): the reference's algorithm in EAGER PyTorch on the same B200
+"""Secondary comparison (BASELINE.md s3 item 4): the reference's algorithm in EAGER PyTorch on the same H100
 (cuDNN / cuBLAS library kernels; ~520 launches and 3 host syncs per utterance) next to the engine.
 The oracle restatement issues exactly the torch ops the reference issues (it is bit-identical to it on CPU),
 so running it on cuda:0 is the reference's own GPU path.  Test infrastructure, not product code."""

@@ -1,5 +1,5 @@
 """Time the two attention kernels on one shape (for ncu / A-B):  python tools/profile_attn.py B L [tc_mode] [reps]
-Prints per-launch microseconds of the tcgen05 kernel (attention_tc.cu) and the fp32 FFMA flash kernel (am_kernels.cu)."""
+Prints per-launch microseconds of the tensor-core kernel (attention_tc.cu) and the fp32 FFMA flash kernel (am_kernels.cu)."""
 import json
 import os
 import sys
