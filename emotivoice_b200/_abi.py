@@ -71,6 +71,7 @@ SIGNATURES = {
     "ev_op_conv1d_gp_group": (_i, [_i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _f, _vp]),
     "ev_op_resblock_gp_group": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "ev_debug_resblock_gp_group_plan": (_i, [_i, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), _i, _i, _i, _i, ctypes.POINTER(ctypes.c_int)]),
+    "ev_op_gp_sum_div": (_i, [_vp, _vp, _vp, _vp, _sz, _f, _vp]),
     "ev_debug_gp_group_plan": (_i, [_i, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_int)]),
     "ev_debug_gp_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_int)]),
     "ev_op_to_gp": (_i, [_vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _i, _i, _i, _i, _vp]),

@@ -1048,6 +1048,12 @@ int ev_op_conv1d_gp_group(int n, const void* const* x, const float* const* w, in
   return launch_conv1d_gp_group(ps, n, mode, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int ev_op_gp_sum_div(const float* a, const float* b, const float* c, float* out, size_t n_floats, float div, void* stream) {
+  EV_CHECK_ARG(a && b && out, "ev_op_gp_sum_div: null argument");
+  EV_TRY(use_device_of(a));
+  return launch_gp_sum_div(a, b, c, out, n_floats, div, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int ev_debug_gp_group_plan(int n, const int* K, const int* dil, int B, int L, int Cin, int Cout, int mode, int* out11) {
   EV_CHECK_ARG(out11 && K && dil && n >= 1 && n <= 3, "ev_debug_gp_group_plan: bad arguments");
   static float dummy_in, dummy_w, dummy_out[3];

@@ -211,6 +211,10 @@ EV_API int ev_op_conv1d_gp(const void* x, const float* w, int mode, const float*
 EV_API int ev_op_conv1d_gp_group(int n, const void* const* x, const float* const* w, int mode, const float* const* bias,
                                  const void* const* res, void* const* out, const int* K, const int* dil, int B, int L, int Cin,
                                  int Cout, const int32_t* lens, int lens_mul, int in_act, float in_slope, void* stream);
+/* out = ((b + a) [+ c]) / div elementwise over n_floats fp32 values (c may be null): the pass that forms a HiFi-GAN stage's
+ * `xs / n` after its ResBlocks' last layers ran as one grouped launch (fp32 storage modes); bitwise equal to the ACC_ADD /
+ * ACC_ADD_DIV epilogues it replaces.  n_floats % 4 == 0. */
+EV_API int ev_op_gp_sum_div(const float* a, const float* b, const float* c, float* out, size_t n_floats, float div, void* stream);
 /* Host-only: the plan of a grouped launch, out11 as ev_debug_gp_plan (tiles = all members'). */
 EV_API int ev_debug_gp_group_plan(int n, const int* K, const int* dil, int B, int L, int Cin, int Cout, int mode, int* out11);
 /* One ResBlock1 layer (hifigan/models.py:50-57) as ONE kernel on granule-planar activations (csrc/resblock_gp.cu):
