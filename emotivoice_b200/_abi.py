@@ -58,6 +58,7 @@ SIGNATURES = {
     "ev_phase1_workspace_bytes": (_sz, [_vp, _i, _i]),
     "ev_phase2_workspace_bytes": (_sz, [_vp, _i, _i]),
     "ev_am_phase1": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ev_am_phase1_prosody": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_am_phase2": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_vocoder": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_wav_to_pcm16": (_i, [_vp, _vp, _sz, _vp]),
@@ -81,6 +82,7 @@ SIGNATURES = {
     "ev_op_attention": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ev_op_attention_tc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ev_op_gauss_upsample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ev_op_duration_scan": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "ev_op_mas": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_op_average_by_duration": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "ev_op_align_logp": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),

@@ -445,21 +445,34 @@ int launch_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T
 // ---------------------------------------------------------------------------------------------
 // x += pitch_embed(p) + energy_embed(e): two Conv1d(1 -> C, k=K, pad=(K-1)/2) on the predicted
 // scalar tracks (model_open_source.py:131-134).  wp/we are tap-major (K, C).
+// prosody (B,5) or null: per-item {alpha, p_scale, p_shift, e_scale, e_shift}; the tracks enter the
+// convolutions as p*p_scale + p_shift and e*e_scale + e_shift (unfused, so 1 and 0 give p back).  With
+// prosody and lens (batch-invariant contract) the window ends at lens[b] like the item's own B=1 call,
+// where the conv's zero padding follows the last token; the shifted pads would otherwise leak in.
 // ---------------------------------------------------------------------------------------------
 template <bool PDL>
 __global__ void var_embed_add_kernel(float* __restrict__ x, const float* __restrict__ pitch,
                                      const float* __restrict__ energy, const float* __restrict__ wp,
                                      const float* __restrict__ bp, const float* __restrict__ we,
-                                     const float* __restrict__ be, int T, int C, int K) {
+                                     const float* __restrict__ be, const float* __restrict__ prosody,
+                                     const int32_t* __restrict__ lens, int T, int C, int K) {
   pdl_entry<PDL>();
   const int row = blockIdx.x;   // b*T + t
   const int b = row / T, t = row % T;
   __shared__ float ps[16], es[16];
   if (threadIdx.x < K) {
+    const int tl = (prosody && lens) ? min(T, lens[b]) : T;
     const int tt = t + threadIdx.x - (K - 1) / 2;
-    const bool ok = tt >= 0 && tt < T;
-    ps[threadIdx.x] = ok ? pitch[(size_t)b * T + tt] : 0.f;
-    es[threadIdx.x] = ok ? energy[(size_t)b * T + tt] : 0.f;
+    const bool ok = tt >= 0 && tt < tl;
+    float p = ok ? pitch[(size_t)b * T + tt] : 0.f;
+    float e = ok ? energy[(size_t)b * T + tt] : 0.f;
+    if (prosody && ok) {
+      const float* pr = prosody + (size_t)b * 5;
+      p = __fadd_rn(__fmul_rn(p, pr[1]), pr[2]);
+      e = __fadd_rn(__fmul_rn(e, pr[3]), pr[4]);
+    }
+    ps[threadIdx.x] = p;
+    es[threadIdx.x] = e;
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -473,29 +486,41 @@ __global__ void var_embed_add_kernel(float* __restrict__ x, const float* __restr
   }
 }
 int launch_var_embed_add(float* x, const float* pitch, const float* energy, const float* wp, const float* bp,
-                         const float* we, const float* be, int B, int T, int C, int K, cudaStream_t st) {
+                         const float* we, const float* be, const float* prosody, const int32_t* lens, int B, int T, int C,
+                         int K, cudaStream_t st) {
   EV_CHECK_ARG(K <= 16, "var_embed: K=%d > 16", K);
-  launch_k(var_embed_add_kernel<true>, var_embed_add_kernel<false>, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, T, C, K);
+  launch_k(var_embed_add_kernel<true>, var_embed_add_kernel<false>, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, prosody,
+           lens, T, C, K);
   EV_CUDA_LAUNCH_CHECK("var_embed_add_kernel");
   return EV_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
-// Duration bookkeeping of GaussianUpsampling.forward (alignment.py:183-199): ds = float(d);
-// the "all durations are zero" guard (:187-191, applied over the WHOLE batch, pads included);
-// c = cumsum(ds) - ds/2; mel_lens[b] = sum_t ds; mel_lens[B] = max_b.  One CTA (B*T is tiny).
-// Integer-valued fp32 sums are exact below 2^24 frames.
+// Duration bookkeeping of GaussianUpsampling.forward (alignment.py:183-199): ds = float(d) * alpha
+// (alpha[b * alpha_stride] per item, 1 when alpha is null); the "all durations are zero" guard
+// (:187-191, applied after the scaling and over the WHOLE batch, pads included; it writes 1, not
+// alpha); c = cumsum(ds) - ds/2; mel_lens[b] = trunc(fl32(sum_t ds)); mel_lens[B] = max_b.
+// The scan runs in fp64 and rounds each output to fp32, which is what ATen's CPU cumsum does.  Each
+// ds is an fp32 value whose ulp is at least alpha * 2^-23 and the sums stay below 2^24, so every fp64
+// partial sum is exact and the order of the parallel scan cannot change a bit.  The frame count rounds
+// the exact sum once; the reference's cascade fp32 sum can land one frame off when the exact sum lies
+// within a few fp32 ulps of an integer.
+// status (may be null) gets bit 8 when an output would have no frames: any item under the
+// batch-invariant contract (its own B=1 call fails in the decoder), or the whole batch otherwise.
+// One CTA (B*T is tiny).
 // ---------------------------------------------------------------------------------------------
 template <bool PDL>
 __global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __restrict__ dur,
-                                                             const int32_t* __restrict__ lens, int invariant, int B, int T,
-                                                             float* __restrict__ centers, float* __restrict__ ds_f,
-                                                             int32_t* __restrict__ mel_lens) {
+                                                             const int32_t* __restrict__ lens,
+                                                             const float* __restrict__ alpha, int alpha_stride,
+                                                             int invariant, int B, int T, float* __restrict__ centers,
+                                                             float* __restrict__ ds_f, int32_t* __restrict__ mel_lens,
+                                                             int32_t* __restrict__ status) {
   pdl_entry<PDL>();
   __shared__ unsigned long long s_total;
-  __shared__ int s_max;
+  __shared__ int s_max, s_min;
   const int tid = threadIdx.x, nw = blockDim.x >> 5, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) { s_total = 0ull; s_max = 0; }
+  if (tid == 0) { s_total = 0ull; s_max = 0; s_min = 0x7fffffff; }
   __syncthreads();
   unsigned long long part = 0;
   for (int i = tid; i < B * T; i += blockDim.x) part += (unsigned long long)dur[i];
@@ -516,34 +541,41 @@ __global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __re
       for (int o = 16; o > 0; o >>= 1) own += __shfl_xor_sync(0xffffffffu, own, o);
       all_zero = (own == 0ull);
     }
-    float run = 0.f;
+    const float a = alpha ? alpha[(size_t)b * alpha_stride] : 1.0f;
+    double run = 0.0;
     for (int t0 = 0; t0 < T; t0 += 32) {
       const int t = t0 + lane;
       float d = 0.f;
-      if (t < T) d = all_zero ? (t < tl ? 1.0f : 0.f) : (float)dur[(size_t)b * T + t];
-      float incl = d;
+      if (t < T) d = all_zero ? (t < tl ? 1.0f : 0.f) : __fmul_rn((float)dur[(size_t)b * T + t], a);
+      double incl = d;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
-        const float n = __shfl_up_sync(0xffffffffu, incl, o);
+        const double n = __shfl_up_sync(0xffffffffu, incl, o);
         if (lane >= o) incl += n;
       }
       if (t < T) {
-        centers[(size_t)b * T + t] = (run + incl) - d / 2;
+        centers[(size_t)b * T + t] = __fsub_rn(__double2float_rn(run + incl), d * 0.5f);
         ds_f[(size_t)b * T + t] = d;
       }
       run += __shfl_sync(0xffffffffu, incl, 31);
     }
     if (lane == 0) {
-      mel_lens[b] = (int)run;
-      atomicMax(&s_max, (int)run);
+      const int n = (int)__double2float_rn(run);
+      mel_lens[b] = n;
+      atomicMax(&s_max, n);
+      atomicMin(&s_min, n);
     }
   }
   __syncthreads();
-  if (tid == 0) mel_lens[B] = s_max;
+  if (tid == 0) {
+    mel_lens[B] = s_max;
+    if (status && (invariant ? s_min == 0 : s_max == 0)) atomicOr(status, 8);
+  }
 }
-int launch_duration_scan(const int64_t* dur, const int32_t* lens, int invariant, int B, int T, float* centers,
-                         float* ds_f, int32_t* mel_lens, cudaStream_t st) {
-  launch_k(duration_scan_kernel<true>, duration_scan_kernel<false>, 1, 1024, 0, st, dur, lens, invariant, B, T, centers, ds_f, mel_lens);
+int launch_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int alpha_stride, int invariant, int B,
+                         int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, cudaStream_t st) {
+  launch_k(duration_scan_kernel<true>, duration_scan_kernel<false>, 1, 1024, 0, st, dur, lens, alpha, alpha_stride, invariant, B, T,
+           centers, ds_f, mel_lens, status);
   EV_CUDA_LAUNCH_CHECK("duration_scan_kernel");
   return EV_OK;
 }

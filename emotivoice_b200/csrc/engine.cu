@@ -776,6 +776,14 @@ int ev_am_phase1(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64, const 
                  const float* content, int B, int T, int invariant, int64_t* dur_out, float* pitch_out,
                  float* energy_out, int32_t* lens32_out, int32_t* mel_lens_out, void* workspace, size_t workspace_bytes,
                  void* stream) {
+  return ev_am_phase1_prosody(ctx, ling, lens64, spk, style, content, B, T, invariant, nullptr, dur_out, pitch_out, energy_out,
+                              lens32_out, mel_lens_out, workspace, workspace_bytes, stream);
+}
+
+int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64, const int64_t* spk, const float* style,
+                         const float* content, int B, int T, int invariant, const float* prosody, int64_t* dur_out,
+                         float* pitch_out, float* energy_out, int32_t* lens32_out, int32_t* mel_lens_out, void* workspace,
+                         size_t workspace_bytes, void* stream) {
   EV_CHECK_ARG(ctx && ctx->bound && ctx->has_am, "ev_am_phase1: acoustic-model weights not bound");
   EV_CHECK_ARG(ling && lens64 && spk && style && content && dur_out && pitch_out && energy_out && lens32_out &&
                    mel_lens_out && workspace,
@@ -818,11 +826,11 @@ int ev_am_phase1(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64, const 
   EV_TRY(run_predictor(ctx, ctx->pitch, pin, b.p1[0], b.p2[0], B, T, lens, conv_lens, 0, pitch_out, nullptr, prefix_mode, st));
   EV_TRY(run_predictor(ctx, ctx->energy, pin, b.p1[1], b.p2[1], B, T, lens, conv_lens, 0, energy_out, nullptr, prefix_mode, st));
   EV_TRY(run_predictor(ctx, ctx->dur, pin, b.p1[2], b.p2[2], B, T, lens, conv_lens, 1, nullptr, dur_out, prefix_mode, st));
-  // x = x + pitch_embed + energy_embed (model_open_source.py:131-134)
-  EV_TRY(launch_var_embed_add(b.hs, pitch_out, energy_out, ctx->pemb_w, ctx->pemb_b, ctx->eemb_w, ctx->eemb_b, B, T, H,
-                              g.embed_kernel, st));
-  // duration bookkeeping for the length regulator (alignment.py:183-199)
-  EV_TRY(launch_duration_scan(dur_out, lens, invariant, B, T, b.centers, b.ds_f, mel_lens_out, st));
+  // x = x + pitch_embed + energy_embed (model_open_source.py:131-134), the tracks shifted / scaled per item when prosody is given
+  EV_TRY(launch_var_embed_add(b.hs, pitch_out, energy_out, ctx->pemb_w, ctx->pemb_b, ctx->eemb_w, ctx->eemb_b, prosody, conv_lens,
+                              B, T, H, g.embed_kernel, st));
+  // duration bookkeeping for the length regulator (alignment.py:183-199), durations scaled by alpha = prosody[b*5]
+  EV_TRY(launch_duration_scan(dur_out, lens, prosody, 5, invariant, B, T, b.centers, b.ds_f, mel_lens_out, mel_lens_out + B + 1, st));
   return EV_OK;
 }
 
@@ -1194,8 +1202,18 @@ int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* len
   EV_TRY(use_device_of(hs));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // centers_tmp holds 2*B*T floats: centres then float durations
-  EV_TRY(launch_duration_scan(dur, lens, invariant, B, T, centers_tmp, centers_tmp + (size_t)B * T, mel_lens_tmp, st));
+  EV_TRY(launch_duration_scan(dur, lens, nullptr, 0, invariant, B, T, centers_tmp, centers_tmp + (size_t)B * T, mel_lens_tmp, nullptr,
+                              st));
   return launch_gauss_upsample(hs, centers_tmp, lens, mel_lens_tmp, B, T, H, F, invariant, pe, alpha, out, st);
+}
+
+int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int invariant, int B, int T, float* centers,
+                        float* ds, int32_t* mel_lens, void* stream) {
+  EV_CHECK_ARG(dur && centers && ds && mel_lens, "ev_op_duration_scan: null argument");
+  EV_CHECK_ARG(B > 0 && T > 0, "ev_op_duration_scan: B=%d T=%d", B, T);
+  EV_TRY(use_device_of(dur));
+  return launch_duration_scan(dur, lens, alpha, 1, invariant, B, T, centers, ds, mel_lens, nullptr,
+                              reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -53,10 +53,31 @@ def encode(req, token2id, speaker2id):
     return ids, int(speaker2id[req.speaker])
 
 
+NEUTRAL_CONTROLS = (1.0, 0.0, 1.0)      # (duration_scale, pitch_shift, energy_scale)
+
+
+def speech_controls(speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+    """A serving API's ``speed`` (openaiapi.py:159) and the pitch / energy controls -> the per-item
+    ``(duration_scale, pitch_shift, energy_scale)`` of ``JETSGenerator.forward``: duration_scale = 1 / speed, computed in
+    double.  Raises ValueError for a non-finite or non-positive speed / energy_scale or a non-finite pitch_shift."""
+    speed, pitch_shift, energy_scale = float(speed), float(pitch_shift), float(energy_scale)
+    if not (np.isfinite(speed) and speed > 0):
+        raise ValueError("speed must be finite and > 0, got %r" % speed)
+    if not np.isfinite(pitch_shift):
+        raise ValueError("pitch_shift must be finite, got %r" % pitch_shift)
+    if not (np.isfinite(energy_scale) and energy_scale > 0):
+        raise ValueError("energy_scale must be finite and > 0, got %r" % energy_scale)
+    return (1.0 / speed, pitch_shift, energy_scale)
+
+
 def collate(items, device="cpu", pad_id=0):
     """items: list of (ids, speaker_id, style_vec, content_vec) -> the keyword arguments of
     ``JETSGenerator.forward`` (inference_am_vocoder_joint.py:113-128), padded with id 0 (the collate
-    convention of the reference's dataset, prompt_dataset.py:183)."""
+    convention of the reference's dataset, prompt_dataset.py:183).
+
+    An item may carry a fifth field, its ``(duration_scale, pitch_shift, energy_scale)`` (see ``speech_controls``).
+    When some item's controls are not neutral the result also holds the three per-item lists; otherwise it holds the
+    five inputs only, so neutral traffic makes exactly the uncontrolled call."""
     B, T = len(items), max(len(it[0]) for it in items)
     ling = np.full((B, T), pad_id, dtype=np.int64)
     for b, it in enumerate(items):
@@ -70,13 +91,19 @@ def collate(items, device="cpu", pad_id=0):
             return torch.stack([torch.as_tensor(r, dtype=torch.float32).to(device) for r in rows])
         return to(np.stack([np.asarray(r, dtype=np.float32) for r in rows]))
 
-    return dict(
+    out = dict(
         inputs_ling=to(ling),
         input_lengths=to(np.asarray([len(it[0]) for it in items], dtype=np.int64)),
         inputs_speaker=to(np.asarray([it[1] for it in items], dtype=np.int64)),
         inputs_style_embedding=vecs(2),
         inputs_content_embedding=vecs(3),
     )
+    controls = [tuple(it[4]) if len(it) > 4 else NEUTRAL_CONTROLS for it in items]
+    if any(c != NEUTRAL_CONTROLS for c in controls):
+        out["duration_scale"] = [c[0] for c in controls]
+        out["pitch_shift"] = [c[1] for c in controls]
+        out["energy_scale"] = [c[2] for c in controls]
+    return out
 
 
 class MicroBatcher:
@@ -86,7 +113,8 @@ class MicroBatcher:
     ``(ids, speaker_id, style_vec, content_vec)``.  ``submit`` returns a Future whose result is the item's
     float32 waveform trimmed to its own length (``mel_lengths[b] * hop``).  A worker thread collects up to
     ``max_batch`` requests, waiting at most ``max_wait_s`` after the first one, and runs ONE forward.
-    Errors of a batch are delivered to every future of that batch.
+    Errors of a batch are delivered to every future of that batch.  Requests with different prosody controls
+    (``speed``, ``pitch_shift``, ``energy_scale``) share one forward: the controls are per item.
     """
 
     def __init__(self, forward, device="cpu", max_batch=32, max_wait_s=0.005, hop=256):
@@ -99,12 +127,15 @@ class MicroBatcher:
         self._thread = threading.Thread(target=self._loop, name="ev-microbatcher", daemon=True)
         self._thread.start()
 
-    def submit(self, ids, speaker_id, style_vec, content_vec):
+    def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+        """``speed`` > 1 speaks faster (duration_scale = 1 / speed); ``pitch_shift`` in semitones; ``energy_scale``
+        multiplies frame energy.  Invalid controls raise ValueError here, so they cannot fail a batch of other requests."""
+        controls = speech_controls(speed, pitch_shift, energy_scale)
         fut = Future()
         with self._lock:
             if self._closed:
                 raise RuntimeError("MicroBatcher is closed")
-            self._queue.append(((np.asarray(ids, dtype=np.int64), int(speaker_id), style_vec, content_vec), fut))
+            self._queue.append(((np.asarray(ids, dtype=np.int64), int(speaker_id), style_vec, content_vec, controls), fut))
             self._lock.notify()
         return fut
 

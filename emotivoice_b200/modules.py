@@ -38,6 +38,60 @@ _HOST_WAIT_BLOCK = os.environ.get("EV_HOST_WAIT", "") == "block"
 _TLS = threading.local()          # per-thread pinned read-back buffer + event
 
 
+# Statistics of the pitch / energy targets the predictors were trained on (config.pitch_stats / energy_stats of the reference,
+# config/joint/config.py:108,111; prompt_dataset.py:130-142 normalises as (x - mean) / std).  Used when the config has none.
+PITCH_STATS = (225.089, 53.78)
+ENERGY_STATS = (30.610, 21.78)
+
+
+def _per_item(name, v, B, neutral):
+    """None / float / length-B sequence / CPU tensor -> float64 numpy (B,).  Raises ValueError before anything is enqueued."""
+    if v is None:
+        return np.full(B, neutral, dtype=np.float64)
+    if isinstance(v, torch.Tensor):
+        if v.device.type != "cpu":
+            raise ValueError("%s must be a float, a sequence or a CPU tensor (reading a %s tensor would synchronise the device)"
+                             % (name, v.device.type))
+        v = v.detach().double().numpy()
+    try:
+        a = np.asarray(v, dtype=np.float64)
+    except (TypeError, ValueError):
+        raise ValueError("%s must be a float, a length-%d sequence or a CPU tensor" % (name, B)) from None
+    if a.ndim == 0:
+        return np.full(B, float(a), dtype=np.float64)
+    if a.shape != (B,):
+        raise ValueError("%s has shape %s, expected a float or length %d" % (name, a.shape, B))
+    return a
+
+
+def prosody_table(B, duration_scale=None, pitch_shift=None, energy_scale=None, config=None):
+    """Host side of the prosody controls: -> None when every item is neutral, else a (B,5) float32 CPU tensor, row b =
+    {alpha, p_scale, p_shift, e_scale, e_shift}.  alpha = fl32(duration_scale) (GaussianUpsampling's alpha, alignment.py:183);
+    with r = 2^(semitones/12): p_scale = fl32(r), p_shift = fl32(mean (r-1) / std) in the normalised units of the pitch
+    predictor, so that the shifted track is the normalised pitch of r * f0; energy likewise with r = energy_scale."""
+    a = _per_item("duration_scale", duration_scale, B, 1.0)
+    s = _per_item("pitch_shift", pitch_shift, B, 0.0)
+    e = _per_item("energy_scale", energy_scale, B, 1.0)
+    if not (np.all(np.isfinite(a)) and np.all(a > 0)):
+        raise ValueError("duration_scale must be finite and > 0, got %s" % a.tolist())
+    if not np.all(np.isfinite(s)):
+        raise ValueError("pitch_shift must be finite, got %s" % s.tolist())
+    if not (np.all(np.isfinite(e)) and np.all(e > 0)):
+        raise ValueError("energy_scale must be finite and > 0, got %s" % e.tolist())
+    if np.all(a == 1.0) and np.all(s == 0.0) and np.all(e == 1.0):
+        return None
+    mp, sp = getattr(config, "pitch_stats", None) or PITCH_STATS
+    me, se = getattr(config, "energy_stats", None) or ENERGY_STATS
+    with np.errstate(over="ignore", invalid="ignore"):
+        rp = np.exp2(s / 12.0)
+        tab = np.stack([a, rp, float(mp) * (rp - 1.0) / float(sp), e, float(me) * (e - 1.0) / float(se)], axis=1)
+        tab32 = tab.astype(np.float32)
+    if not (np.all(np.isfinite(tab32)) and np.all(tab32[:, 0] > 0) and np.all(tab32[:, 3] > 0)):
+        raise ValueError("prosody controls outside the fp32 range: duration_scale %s, pitch_shift %s, energy_scale %s"
+                         % (a.tolist(), s.tolist(), e.tolist()))
+    return torch.from_numpy(tab32)
+
+
 def _bucket(nbytes):
     """Workspace sizes are rounded up to a geometric series (x1.125 steps, 2 MiB granularity): utterances of similar length
     then request IDENTICAL sizes, so torch's caching allocator serves them from its pool instead of calling cudaMalloc
@@ -177,10 +231,14 @@ class _Engine:
             pass
         return tl.pin[:n].clone()
 
-    def acoustic(self, ling, lens, spk, style, content, invariant):
+    def acoustic(self, ling, lens, spk, style, content, invariant, prosody=None):
+        """``prosody``: None (neutral: the plain ev_am_phase1 call) or the (B,5) CPU table of ``prosody_table``."""
         lib, dev = self.lib, self.device
         B, T = ling.shape
         self.ensure_pe(T)
+        if prosody is not None:       # uploaded with the inputs; the pinned source lives until the read-back below
+            prosody_host = prosody.pin_memory()
+            prosody = prosody_host.to(dev, non_blocking=True)
         dur = torch.empty((B, T), dtype=torch.int64, device=dev)
         pitch = torch.empty((B, T), dtype=torch.float32, device=dev)
         energy = torch.empty((B, T), dtype=torch.float32, device=dev)
@@ -190,9 +248,15 @@ class _Engine:
         st = self._stream()
         lens32_ptr = meta.data_ptr()
         mel_lens_ptr = meta.data_ptr() + 4 * B
-        _abi.check(lib.ev_am_phase1(self.handle, ling.data_ptr(), lens.data_ptr(), spk.data_ptr(), style.data_ptr(),
-                                    content.data_ptr(), B, T, int(invariant), dur.data_ptr(), pitch.data_ptr(),
-                                    energy.data_ptr(), lens32_ptr, mel_lens_ptr, ws1.data_ptr(), n1, st))
+        if prosody is None:
+            _abi.check(lib.ev_am_phase1(self.handle, ling.data_ptr(), lens.data_ptr(), spk.data_ptr(), style.data_ptr(),
+                                        content.data_ptr(), B, T, int(invariant), dur.data_ptr(), pitch.data_ptr(),
+                                        energy.data_ptr(), lens32_ptr, mel_lens_ptr, ws1.data_ptr(), n1, st))
+        else:
+            _abi.check(lib.ev_am_phase1_prosody(self.handle, ling.data_ptr(), lens.data_ptr(), spk.data_ptr(), style.data_ptr(),
+                                                content.data_ptr(), B, T, int(invariant), prosody.data_ptr(), dur.data_ptr(),
+                                                pitch.data_ptr(), energy.data_ptr(), lens32_ptr, mel_lens_ptr, ws1.data_ptr(), n1,
+                                                st))
         # the path's single host sync: the output length is data dependent (alignment.py:194-195).  Asynchronous copy into pinned
         # memory + a polled event instead of a blocking .cpu(): a blocking wait of a few milliseconds puts the thread to sleep, and its
         # wake-up latency (measured: 5-15 ms now and then on a busy host) would sit in the middle of the forward with the GPU idle.
@@ -203,7 +267,11 @@ class _Engine:
                 raise IndexError("inputs_ling holds token ids outside [0, %d)" % int(self.cfg.n_vocab))
             if status & 2:
                 raise IndexError("inputs_speaker holds ids outside [0, %d)" % int(self.cfg.n_speaker))
-            raise RuntimeError("input_lengths must lie in [1, %d] (the padded width of inputs_ling)" % T)
+            if status & 4:
+                raise RuntimeError("input_lengths must lie in [1, %d] (the padded width of inputs_ling)" % T)
+            # the reference's decoder fails on a zero-length input (Conv1d raises); nothing of phase 2 has been enqueued
+            raise RuntimeError("duration_scale leaves an utterance with no frames (mel lengths %s); use a larger duration_scale"
+                               % mel_lens_host[:B].tolist())
         F = int(mel_lens_host[B])
         self.ensure_pe(F)
         ws2 = self._ws("p2", lib.ev_phase2_workspace_bytes(self.handle, B, F))
@@ -375,16 +443,19 @@ class PromptTTS(_EngineOwner):
 
     @torch.no_grad()
     def forward(self, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
-                mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0):
+                mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0,
+                duration_scale=None, pitch_shift=None, energy_scale=None):
+        """``duration_scale`` / ``pitch_shift`` / ``energy_scale``: prosody controls, see ``JETSGenerator.forward``."""
         if mel_targets is not None:
             raise NotImplementedError("training-mode forward (teacher forcing) is out of scope for this engine")
+        prosody = prosody_table(inputs_ling.shape[0], duration_scale, pitch_shift, energy_scale, self.config)
         eng = self._engine()
         with eng.call_lock:
             return _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                               inputs_content_embedding, not self.compat_padded_batch)[0]
+                               inputs_content_embedding, not self.compat_padded_batch, prosody)[0]
 
 
-def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant):
+def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant, prosody=None):
     dev = eng.device
     ling = _prep(inputs_ling, torch.int64, dev)
     lens = _prep(input_lengths, torch.int64, dev)
@@ -398,7 +469,7 @@ def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content,
     if tuple(style.shape) != want or tuple(content.shape) != want:
         raise RuntimeError("inputs_style_embedding %s / inputs_content_embedding %s must both be %s"
                            % (tuple(style.shape), tuple(content.shape), want))
-    r = eng.acoustic(ling, lens, spk, style, content, invariant)
+    r = eng.acoustic(ling, lens, spk, style, content, invariant, prosody)
     out = {
         "mel_targets": None,
         "dec_outputs": r["mel"],
@@ -427,6 +498,20 @@ class JETSGenerator(_EngineOwner):
     SURVEY.md s4 item 4).  By default every item of a batch is computed exactly like the
     reference's B=1 call for that item (what every reference caller runs); set the attribute
     to True to reproduce the literal padded-batch forward instead.  For B=1 both agree.
+
+    Prosody controls (keyword arguments of ``forward``; each None, one float for every item, or a length-B
+    sequence / CPU tensor with one value per item):
+
+    * ``duration_scale`` (1.0): multiplies the predicted durations before the length regulator -- the ``alpha`` of
+      the reference's GaussianUpsampling (alignment.py:180-183).  Above 1 is slower speech; a server's ``speed``
+      is ``duration_scale = 1 / speed``.
+    * ``pitch_shift`` (0.0): semitones; the predicted pitch enters ``pitch_embed`` as the normalised pitch of
+      2^(s/12) * f0, with the statistics of ``config.pitch_stats`` (default 225.089, 53.78).
+    * ``energy_scale`` (1.0): multiplies frame energy the same way (``config.energy_stats``, default 30.610, 21.78).
+
+    The returned predictions stay the model's raw ones; ``mel_lengths`` counts the scaled frames.  Neutral values
+    give bitwise the uncontrolled output.  ``alpha=`` is accepted and ignored, as in the reference's inference
+    branch.  An utterance scaled to zero frames raises RuntimeError (the reference's decoder raises too).
     """
 
     def __init__(self, config):
@@ -446,13 +531,15 @@ class JETSGenerator(_EngineOwner):
     @torch.no_grad()
     def forward(self, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
                 mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0,
-                cut_flag=True):
+                cut_flag=True, duration_scale=None, pitch_shift=None, energy_scale=None):
         if mel_targets is not None:
             raise NotImplementedError("training-mode forward (teacher forcing / random segments) is out of scope")
+        prosody = prosody_table(inputs_ling.shape[0], duration_scale, pitch_shift, energy_scale, self.config)
         eng = self._engine()
         invariant = not self.compat_padded_batch
         with eng.call_lock:
-            return self._forward_locked(eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding)
+            return self._forward_locked(eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
+                                        inputs_content_embedding, prosody)
 
     def reserve(self, batch=1, phonemes=256, frames=2048):
         """Serving set-up: pre-size the engine's workspace arena (current CUDA stream) for requests up to this shape, so that no
@@ -460,9 +547,10 @@ class JETSGenerator(_EngineOwner):
         stall per new maximum)."""
         self._engine().reserve(batch, phonemes, frames)
 
-    def _forward_locked(self, eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding):
+    def _forward_locked(self, eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
+                        prosody=None):
         outputs, r = _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                                 inputs_content_embedding, invariant)
+                                 inputs_content_embedding, invariant, prosody)
         B = r["mel"].shape[0]
         mel_lens_ptr = (r["meta"].data_ptr() + 4 * B) if invariant else None
         # jets.py:62-66: z = dec_outputs.transpose(1, 2); wav = generator(z).  dec_outputs is already the

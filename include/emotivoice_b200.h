@@ -131,13 +131,32 @@ EV_API size_t ev_phase2_workspace_bytes(const ev_ctx* ctx, int B, int F);
  *   mel_lens_out (B+2) i32: per-item frame counts, max over items in slot B, and in slot B+1 an input
  *     status word the host checks at the same read-back (the reference raises IndexError from nn.Embedding
  *     for these; the kernels clamp so nothing is read out of bounds): bit 0 = a token id outside
- *     [0, n_vocab), bit 1 = a speaker id outside [0, n_speaker), bit 2 = a length outside [1, T].
+ *     [0, n_vocab), bit 1 = a speaker id outside [0, n_speaker), bit 2 = a length outside [1, T],
+ *     bit 3 = an output with no frames (set only by ev_am_phase1_prosody with duration scales below 1:
+ *     under the batch-invariant contract any item, otherwise the whole batch; the reference's decoder raises
+ *     RuntimeError on a zero-length input).  Do not run phase 2 when it is set.
  *   invariant != 0: batch-invariant contract (each item == the reference's B=1 call);
  *   invariant == 0: literal padded-batch forward of the reference. */
 EV_API int ev_am_phase1(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, const int64_t* spk,
                         const float* style, const float* content, int B, int T, int invariant,
                         int64_t* dur_out, float* pitch_out, float* energy_out, int32_t* lens32_out,
                         int32_t* mel_lens_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ev_am_phase1 with per-item prosody controls.  prosody (B,5) f32 on the device, or NULL (== ev_am_phase1):
+ * row b = {alpha, p_scale, p_shift, e_scale, e_shift}.
+ *   alpha scales the predicted durations before the length regulator, ds = fl32(d * alpha), exactly the
+ *     alpha of GaussianUpsampling.forward (alignment.py:180-183); the all-zero guard then writes 1, not alpha.
+ *     The cumsum runs in fp64 (exact for these inputs) and rounds to fp32 like ATen's CPU cumsum;
+ *     mel_lens[b] = trunc(fl32(exact sum)).  The reference's fp32 cascade sum can differ by one frame when the
+ *     exact sum lies within a few fp32 ulps of an integer.
+ *   pitch / energy enter pitch_embed / energy_embed (model_open_source.py:131-134) as p*p_scale + p_shift and
+ *     e*e_scale + e_shift (two fp32 roundings each; 1 and 0 give the unscaled track back bit for bit).
+ *   dur_out, pitch_out and energy_out stay the model's raw predictions. */
+EV_API int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, const int64_t* spk,
+                                const float* style, const float* content, int B, int T, int invariant,
+                                const float* prosody, int64_t* dur_out, float* pitch_out, float* energy_out,
+                                int32_t* lens32_out, int32_t* mel_lens_out, void* workspace, size_t workspace_bytes,
+                                void* stream);
 
 /* Replaces: GaussianUpsampling.forward matmul (alignment.py:201-211), the decoder
  * (model_open_source.py:146) and to_mel (:147).  Must follow ev_am_phase1 on the same stream;
@@ -255,6 +274,11 @@ EV_API int ev_op_attention_tc(const float* qkv, const int32_t* key_lens, float* 
                               int tc_mode, void* stream);
 /* Gaussian upsampling (alignment.py:180-211) incl. cumsum; out (B,F,H); adds alpha*pe[f] when pe != NULL.
  * centers_tmp: 2*B*T floats of scratch; mel_lens_tmp: B+1 int32 (frame counts, max in slot B). */
+/* The duration bookkeeping of ev_am_phase1_prosody alone: dur (B,T) i64; lens (B) i32 or NULL; alpha (B) f32 or
+ * NULL (1); centers, ds (B,T) f32 = cumsum(ds) - ds/2 and ds = fl32(d * alpha) after the all-zero guard;
+ * mel_lens (B+1) i32: trunc(fl32(sum ds)) per item, max in slot B. */
+EV_API int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int invariant, int B, int T,
+                               float* centers, float* ds, int32_t* mel_lens, void* stream);
 EV_API int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* lens, int B, int T, int H,
                                 int F, int invariant, const float* pe, const float* alpha, float* centers_tmp,
                                 int32_t* mel_lens_tmp, float* out, void* stream);
