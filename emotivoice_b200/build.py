@@ -85,6 +85,7 @@ def _build_locked(force, verbose):
         if verbose:
             print(" ".join(cmd), flush=True)
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
+    serialised = []
     for src, p in procs:
         out, _ = p.communicate()
         if p.returncode != 0:
@@ -92,6 +93,14 @@ def _build_locked(force, verbose):
             raise RuntimeError("nvcc failed on %s" % src)
         if verbose and out.strip():
             print(out.decode())
+        if b"C7520" in out:
+            if not verbose:
+                sys.stderr.write(out.decode())
+            serialised.append(os.path.basename(src))
+    if serialised:
+        # such a binary computes the same results, but every MMA waits for the previous one to finish: refuse to build it
+        raise RuntimeError("ptxas serialised wgmma instructions (warning C7520, reason above) in %s; a wgmma on a path ptxas cannot "
+                           "prove warp-uniform is one cause" % ", ".join(serialised))
     cmd = [nvcc_path(), "-shared", "-o", LIB_PATH] + objs + ["-cudart", "static",
                                                            "-gencode", "arch=compute_90a,code=sm_90a"]
     if verbose:

@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules (16 channels) per MMA K step");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
-  const int warp = tid >> 5;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int lane = tid & 31;
   const int BN = pl.BN;
 

@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
   constexpr int NCW = NCONS / 32;         // consumer warps: every one of them releases each stage
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
-  const int warp = tid >> 5;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int lane = tid & 31;
   const int BN = pl.BN;
 

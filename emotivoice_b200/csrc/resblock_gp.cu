@@ -95,7 +95,8 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
   constexpr int NA = ACC_REGS / MT;
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules per MMA K step");
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int C = p.C;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
