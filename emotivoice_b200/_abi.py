@@ -65,6 +65,7 @@ SIGNATURES = {
     "ev_launch_count": (_u64, []),
     "ev_op_conv1d": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp]),
     "ev_op_conv1d_tc": (_i, [_vp, _vp, _i, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp, _sz, _vp]),
+    "ev_op_conv1d_tc_ks": (_i, [_vp, _vp, _i, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _i, _vp, _sz, _vp]),
     "ev_set_precision": (_i, [_vp, _i]),
     "ev_op_conv1d_gp": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _f, _vp]),
     "ev_op_resblock_gp": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _vp]),

@@ -1004,9 +1004,18 @@ int ev_op_conv1d_tc(const float* x, const float* w_tc, int split3, const float* 
                     float* out, int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul,
                     int in_act, float in_slope, int out_act, int acc, float div, float* splitk_ws, size_t splitk_floats,
                     void* stream) {
+  return ev_op_conv1d_tc_ks(x, w_tc, split3, bias, bias_bstride, res, out, B, L, Cin, Cout, K, dil, lens, lens_mul, in_act, in_slope,
+                            out_act, acc, div, splitk_ws ? 4 : 0, splitk_ws, splitk_floats, stream);
+}
+
+int ev_op_conv1d_tc_ks(const float* x, const float* w_tc, int split3, const float* bias, size_t bias_bstride, const float* res,
+                       float* out, int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul,
+                       int in_act, float in_slope, int out_act, int acc, float div, int ksplit, float* splitk_ws,
+                       size_t splitk_floats, void* stream) {
   EV_CHECK_ARG(x && w_tc && out, "ev_op_conv1d_tc: null argument");
+  EV_CHECK_ARG(ksplit <= 1 || splitk_ws, "ev_op_conv1d_tc: ksplit=%d needs split-K scratch", ksplit);
   EV_TRY(use_device_of(x));
-  EV_TRY(set_split_ws(splitk_ws, splitk_floats, splitk_ws ? 4 : 0));
+  EV_TRY(set_split_ws(splitk_ws, splitk_floats, splitk_ws ? ksplit : 0));
   EV_CHECK_ARG(Cin % 8 == 0 && Cout % 16 == 0 && (Cout <= 128 || Cout % 128 == 0),
                "ev_op_conv1d_tc: needs Cin %% 8 == 0, Cout %% 16 == 0 and Cout <= 128 or a multiple of 128 (Cin=%d Cout=%d)", Cin, Cout);
   EV_CHECK_ARG(split3 < 2 || Cin % 16 == 0, "ev_op_conv1d_tc: the bf16 / bf16x3 modes need Cin %% 16 == 0 (Cin=%d)", Cin);

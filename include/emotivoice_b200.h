@@ -202,12 +202,21 @@ EV_API int ev_op_conv1d(const float* x, const float* w, const float* bias, size_
 /* Same contract on the tensor cores (wgmma tf32 / bf16, fp32 accumulators in registers); w_tc is in the
  * tensor-core layout (2 planes hi|lo, Cout/BNp N tiles, K, Cin/4, BNp = min(Cout,128), 4; packing.to_tc_layout);
  * split3 = 0: 1xTF32, 1: 3xTF32 fp32 emulation, 2: bf16 operands (w_tc then in the bf16 layout of
- * packing.to_tc16_layout; Cin % 16 == 0).  Requires Cin % 8 == 0, Cout % 16 == 0 and Cout <= 128 or Cout % 128 == 0.  splitk_ws (optional, splitk_floats floats of scratch) lets a
- * launch with few output tiles and a long reduction be split along K (deterministic two-pass). */
+ * packing.to_tc16_layout; Cin % 16 == 0), 3: bf16x3 fp32 emulation (w_tc then holds the two bf16 planes of
+ * packing.to_tc16x2_layout; Cin % 16 == 0).  Requires Cin % 8 == 0, Cout % 16 == 0 and Cout <= 128 or Cout % 128 == 0.
+ * splitk_ws (optional, splitk_floats floats of scratch) lets a launch with few output tiles and a long reduction be split
+ * along K into 4 slices (deterministic two-pass). */
 EV_API int ev_op_conv1d_tc(const float* x, const float* w_tc, int split3, const float* bias, size_t bias_bstride,
                            const float* res, float* out, int B, int L, int Cin, int Cout, int K, int dil,
                            const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act,
                            int acc, float div, float* splitk_ws, size_t splitk_floats, void* stream);
+/* ev_op_conv1d_tc with an explicit K-split factor: ksplit <= 1 runs one pass; ksplit = S > 1 (needs splitk_ws) shares each
+ * output tile's reduction among S CTAs -- clamped to the number of C_in blocks, exactly as the engine's layers request it --
+ * and sums the slices in a second, fixed-order pass.  ev_op_conv1d_tc is this call with ksplit = 4 (0 without scratch). */
+EV_API int ev_op_conv1d_tc_ks(const float* x, const float* w_tc, int split3, const float* bias, size_t bias_bstride,
+                              const float* res, float* out, int B, int L, int Cin, int Cout, int K, int dil,
+                              const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act,
+                              int acc, float div, int ksplit, float* splitk_ws, size_t splitk_floats, void* stream);
 /* Host-only introspection (no GPU needed): the tile / pipeline plan ev_op_conv1d_tc would use for a shape.
  * out11 = {BN, MT, KBG, a_stages, b_stages, producer groups, ksplit, accumulator columns (MT x BN), smem bytes, tiles, rows_pad}.
  * The CPU tests check the invariants the kernel relies on (ring depth >= producer groups, register/smem limits,
