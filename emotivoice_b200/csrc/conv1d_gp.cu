@@ -218,50 +218,77 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
           prev_sa = j == K - 1 ? sa : -1;
         }
       }
+
+      // epilogue: register pair i, i+1 = channels n, n+1 of one row (one granule).  Pair i = 4 q + 2 h of accumulator mt lies in
+      // column group q (8 columns: the same bias for every mt and h) and row row0 + mt * BM + 8 h.  The pairs are walked in chunks
+      // of EQ column groups, 4 pairs (8 at MT = 4: one column group; larger chunks spill at MT = 1, 2).  A chunk issues all its
+      // loads (bias, residual, `out` in the accumulate modes) before its arithmetic and stores, and the first chunk's loads run
+      // under the tile's last MMAs.  In place (out == res, or out read by the accumulate modes) this stays correct: every output
+      // element is loaded and stored by exactly one thread, once per launch, and that thread loads it before it stores it.
+      constexpr int EQ = MT == 1 ? 2 : 1;
+      const bool has_res = G.res != nullptr;
+      const int row0 = t0 + wg * 64 + frag_row(0, lane, wl);   // GEMM rows = input-resolution time steps
+      float2 ebias[EQ];
+      pair_t<BF16> eres[EQ][MT][2], eout[EQ][MT][2];
+      auto column = [&](int q, int& n) {
+        n = n0 + frag_col(4 * q, lane);
+        const int phase = n / coutR, co = n - phase * coutR;
+        return (((size_t)b * gout + co / CPG) * Lout + phase) * CPG + (co % CPG);     // element index at row 0
+      };
+      auto epi_load = [&](int ch) {         // chunk ch = column groups [ch * EQ, ch * EQ + EQ)
+#pragma unroll
+        for (int q = 0; q < EQ; ++q) {
+          int n;
+          const size_t ec = column(ch * EQ + q, n);
+          if (n - n0 >= BN) continue;
+          if (G.bias) ebias[q] = __ldg(reinterpret_cast<const float2*>(G.bias + n));
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + mt * BM + 8 * h;
+              if (row >= len) continue;
+              const size_t e = ec + (size_t)row * p.rate * CPG;
+              if (has_res) eres[q][mt][h] = load_pair<BF16>(G.res, e);
+              if (accm != EV_ACC_STORE) eout[q][mt][h] = load_pair<BF16>(G.out, e);
+            }
+        }
+      };
+      auto epi_store = [&](int ch) {
+#pragma unroll
+        for (int q = 0; q < EQ; ++q) {
+          int n;
+          const size_t ec = column(ch * EQ + q, n);
+          if (n - n0 >= BN) continue;
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + mt * BM + 8 * h;
+              if (row >= len) continue;
+              const int i = 4 * (ch * EQ + q) + 2 * h;
+              float v0 = acc[mt][i], v1 = acc[mt][i + 1];
+              if (G.bias) { v0 += ebias[q].x; v1 += ebias[q].y; }
+              if (has_res) {
+                const float2 r = unpack_pair(eres[q][mt][h]);
+                v0 += r.x; v1 += r.y;
+              }
+              if (accm != EV_ACC_STORE) {
+                const float2 o = unpack_pair(eout[q][mt][h]);
+                v0 += o.x; v1 += o.y;
+                if (accm == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
+              }
+              store_pair<BF16>(G.out, ec + (size_t)row * p.rate * CPG, v0, v1);
+            }
+        }
+      };
+      epi_load(0);
       wgmma_wait<0>();
       release(prev_sb, prev_sa);
-
-      // epilogue: register pair i, i+1 = channels n, n+1 of one row (one granule)
-      const bool has_res = G.res != nullptr;
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-        for (int i = 0; i < NA; i += 2) {
-          const int c = frag_col(i, lane);
-          const int row = t0 + mt * BM + wg * 64 + frag_row(i, lane, wl);    // this GEMM row (input-resolution time step)
-          if (c >= BN || row >= len) continue;
-          const int n = n0 + c;
-          const int phase = n / coutR, co = n - phase * coutR;
-          const size_t e = (((size_t)b * gout + co / CPG) * Lout + (size_t)row * p.rate + phase) * CPG + (co % CPG);   // element index
-          float v0 = acc[mt][i], v1 = acc[mt][i + 1];
-          if (G.bias) {
-            const float2 b2 = __ldg(reinterpret_cast<const float2*>(G.bias + n));
-            v0 += b2.x; v1 += b2.y;
-          }
-          if (BF16) {
-            if (has_res) {
-              const uint32_t r = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.res) + e);
-              v0 += __uint_as_float(r << 16); v1 += __uint_as_float(r & 0xffff0000u);
-            }
-            if (accm != EV_ACC_STORE) {
-              const uint32_t q = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.out) + e);
-              v0 += __uint_as_float(q << 16); v1 += __uint_as_float(q & 0xffff0000u);
-              if (accm == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
-            }
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(G.out) + e) = pack_bf16(v0, v1);
-          } else {
-            if (has_res) {
-              const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.res) + e);
-              v0 += r.x; v1 += r.y;
-            }
-            if (accm != EV_ACC_STORE) {
-              const float2 q = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.out) + e);
-              v0 += q.x; v1 += q.y;
-              if (accm == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
-            }
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(G.out) + e) = make_float2(v0, v1);
-          }
-        }
+      for (int ch = 0; ch < NA / 4 / EQ; ++ch) {
+        if (ch > 0) epi_load(ch);
+        epi_store(ch);
       }
     }
   } else if (warp < W_ALOAD) {

@@ -164,6 +164,17 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       const GpPairGroup& G = gs.g[gi];
       const int K = G.K, dil = G.dil, R = G.R;
       const int h2 = (K - 1) / 2;
+      // epi1 in parts of B1Q column groups (pair i = 4 q + 2 h of every accumulator lies in column group q: 8 columns, one b1): a
+      // part's b1 loads are all issued ahead of its shared-memory stores, the first part's under c1's last MMAs
+      constexpr int B1Q = 2;
+      float2 bias1[B1Q];
+      auto load_b1 = [&](int part) {
+#pragma unroll
+        for (int q = 0; q < B1Q; ++q) {
+          const int c = frag_col(4 * (part * B1Q + q), lane);
+          if (c < C) bias1[q] = __ldg(reinterpret_cast<const float2*>(G.b1 + c));
+        }
+      };
       // ---- c1 over the staged x tile
       {
         int prev_sb = -1, prev_sa = -1;
@@ -196,6 +207,7 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
             prev_sa = j == K - 1 ? sa : -1;
           }
         }
+        load_b1(0);
         wgmma_wait<0>();
         release(prev_sb, prev_sa);
       }
@@ -203,36 +215,91 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       // ---- xt tile (their taps overlap the other's rows), so the tile is only rewritten once both have finished it.
       bar_sync(1, NCW * 32);
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
+      for (int part = 0; part < NA / 4 / B1Q; ++part) {
+        if (part > 0) load_b1(part);
 #pragma unroll
-        for (int i = 0; i < NA; i += 2) {
-          const int c = frag_col(i, lane);
-          if (c >= C) continue;
-          const int r2 = mt * BM + wg * 64 + frag_row(i, lane, wl);
-          const int row = t0 - h2 + r2;
-          const bool ok = row >= 0 && row < len;            // xt outside the sequence is c2's ZERO padding
-          const float2 b1 = __ldg(reinterpret_cast<const float2*>(G.b1 + c));
-          float v0 = acc[mt][i] + b1.x, v1 = acc[mt][i + 1] + b1.y;
-          if (BF16) {      // the unfused path stores xt as bf16 before activating it
-            v0 = __uint_as_float(pack_bf16(v0, 0.f) << 16);
-            v1 = __uint_as_float(pack_bf16(v1, 0.f) << 16);
-          }
-          v0 = ok ? lrelu_f(v0, slope) : 0.f;
-          v1 = ok ? lrelu_f(v1, slope) : 0.f;
-          uint8_t* d = a2_tile + ((size_t)(c / OCPG) * pl.rows2_pad + r2) * 16 + (c % OCPG) * (OP16 ? 2 : 4);
-          if (OP16) {
-            const uint32_t hi = pack_bf16(v0, v1);
-            *reinterpret_cast<uint32_t*>(d) = hi;
-            if (X3B) *reinterpret_cast<uint32_t*>(d + pl.a2_plane_bytes) = pack_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xffff0000u));
-          } else {
-            const float2 h = make_float2(to_tf32(v0), to_tf32(v1));
-            *reinterpret_cast<float2*>(d) = h;
-            if (SPLIT3) *reinterpret_cast<float2*>(d + pl.a2_plane_bytes) = make_float2(to_tf32(v0 - h.x), to_tf32(v1 - h.y));
-          }
-        }
+        for (int q = 0; q < B1Q; ++q)
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * (part * B1Q + q) + 2 * h;
+              const int c = frag_col(i, lane);
+              if (c >= C) continue;
+              const int r2 = mt * BM + wg * 64 + frag_row(i, lane, wl);
+              const int row = t0 - h2 + r2;
+              const bool ok = row >= 0 && row < len;            // xt outside the sequence is c2's ZERO padding
+              float v0 = acc[mt][i] + bias1[q].x, v1 = acc[mt][i + 1] + bias1[q].y;
+              if (BF16) {      // the unfused path stores xt as bf16 before activating it
+                v0 = __uint_as_float(pack_bf16(v0, 0.f) << 16);
+                v1 = __uint_as_float(pack_bf16(v1, 0.f) << 16);
+              }
+              v0 = ok ? lrelu_f(v0, slope) : 0.f;
+              v1 = ok ? lrelu_f(v1, slope) : 0.f;
+              uint8_t* d = a2_tile + ((size_t)(c / OCPG) * pl.rows2_pad + r2) * 16 + (c % OCPG) * (OP16 ? 2 : 4);
+              if (OP16) {
+                const uint32_t hi = pack_bf16(v0, v1);
+                *reinterpret_cast<uint32_t*>(d) = hi;
+                if (X3B) *reinterpret_cast<uint32_t*>(d + pl.a2_plane_bytes) = pack_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xffff0000u));
+              } else {
+                const float2 t = make_float2(to_tf32(v0), to_tf32(v1));
+                *reinterpret_cast<float2*>(d) = t;
+                if (SPLIT3) *reinterpret_cast<float2*>(d + pl.a2_plane_bytes) = make_float2(to_tf32(v0 - t.x), to_tf32(v1 - t.y));
+              }
+            }
       }
       fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core
       bar_sync(1, NCW * 32);        // the whole xt tile is written
+      // ---- epi2 (acc2 + b2 + x (+ accumulate) -> out): pair i = 4 q + 2 h of accumulator mt is column group q (8 columns, one b2)
+      // at tile row rl0 + mt * BM + 8 h.  One column group is one chunk of 2 MT pairs: it issues all its loads (b2, the residual x,
+      // `out` in the accumulate modes) before its stores, the first chunk's under c2's last MMAs (a larger chunk spills in the MT = 1
+      // tf32 / bf16 instantiations).  out != x (plan_pair), and in the accumulate modes every element of out is loaded and stored
+      // by exactly one thread, load first.
+      const int rl0 = wg * 64 + frag_row(0, lane, wl);
+      float2 ebias;
+      pair_t<BF16> eres[MT][2], eout[MT][2];
+      auto column = [&](int q, int& c) {
+        c = frag_col(4 * q, lane);
+        return ((size_t)b * gC + c / CPG) * p.L * CPG + (c % CPG);      // element index at row 0
+      };
+      auto epi_load = [&](int q) {
+        int c;
+        const size_t ec = column(q, c);
+        if (c >= C) return;
+        ebias = __ldg(reinterpret_cast<const float2*>(G.b2 + c));
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int rl = rl0 + mt * BM + 8 * h, row = t0 + rl;
+            if (rl >= R || row >= len) continue;
+            const size_t e = ec + (size_t)row * CPG;
+            eres[mt][h] = load_pair<BF16>(G.x, e);      // the residual: L2 hit
+            if (p.acc != EV_ACC_STORE) eout[mt][h] = load_pair<BF16>(G.out, e);
+          }
+      };
+      auto epi_store = [&](int q) {
+        int c;
+        const size_t ec = column(q, c);
+        if (c >= C) return;
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int rl = rl0 + mt * BM + 8 * h, row = t0 + rl;
+            if (rl >= R || row >= len) continue;
+            const int i = 4 * q + 2 * h;
+            float v0 = acc[mt][i] + ebias.x, v1 = acc[mt][i + 1] + ebias.y;
+            const float2 r = unpack_pair(eres[mt][h]);
+            v0 += r.x; v1 += r.y;
+            if (p.acc != EV_ACC_STORE) {
+              const float2 o = unpack_pair(eout[mt][h]);
+              v0 += o.x; v1 += o.y;
+              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
+            }
+            store_pair<BF16>(G.out, ec + (size_t)row * CPG, v0, v1);
+          }
+      };
       // ---- c2 over the xt tile
       {
         int prev_sb = -1;
@@ -262,41 +329,14 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
             prev_sb = sb;
           }
         }
+        epi_load(0);
         wgmma_wait<0>();
         release(prev_sb, -1);
       }
-      // ---- epi2: acc2 + b2 + x (+ accumulate) -> out
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-        for (int i = 0; i < NA; i += 2) {
-          const int c = frag_col(i, lane);
-          const int rl = mt * BM + wg * 64 + frag_row(i, lane, wl);      // row inside the tile
-          const int row = t0 + rl;
-          if (c >= C || rl >= R || row >= len) continue;
-          const size_t e = (((size_t)b * gC + c / CPG) * p.L + row) * CPG + (c % CPG);
-          const float2 b2 = __ldg(reinterpret_cast<const float2*>(G.b2 + c));
-          float v0 = acc[mt][i] + b2.x, v1 = acc[mt][i + 1] + b2.y;
-          if (BF16) {
-            const uint32_t r = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.x) + e);   // the residual: L2 hit
-            v0 += __uint_as_float(r << 16); v1 += __uint_as_float(r & 0xffff0000u);
-            if (p.acc != EV_ACC_STORE) {
-              const uint32_t q = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(G.out) + e);
-              v0 += __uint_as_float(q << 16); v1 += __uint_as_float(q & 0xffff0000u);
-              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
-            }
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(G.out) + e) = pack_bf16(v0, v1);
-          } else {
-            const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.x) + e);
-            v0 += r.x; v1 += r.y;
-            if (p.acc != EV_ACC_STORE) {
-              const float2 q = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(G.out) + e);
-              v0 += q.x; v1 += q.y;
-              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
-            }
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(G.out) + e) = make_float2(v0, v1);
-          }
-        }
+      for (int q = 0; q < NA / 4; ++q) {
+        if (q > 0) epi_load(q);
+        epi_store(q);
       }
     }
   } else if (warp < W_ALOAD) {

@@ -2,6 +2,7 @@
 // attention_tc.cu): mbarrier / bulk-copy wrappers, the no-swizzle K-major shared-memory descriptor, warpgroup MMA (wgmma)
 // with fp32 accumulators in registers, and the accumulator fragment layout.  Internal header.
 #pragma once
+#include <type_traits>
 #include "ev_common.cuh"
 
 namespace ev {
@@ -83,6 +84,25 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ int frag_row(int i, int lane, int wl) { return wl * 16 + (lane >> 2) + 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int i, int lane) { return (i >> 2) * 8 + (lane & 3) * 2 + (i & 1); }
+
+// The granule-planar epilogues (conv1d_gp.cu, resblock_gp.cu) read and write one accumulator register pair at a time: two adjacent
+// channels of one row, a float2 of an fp32 tensor or one bf16x2 word.  They walk the pairs in chunks and issue all of a chunk's
+// global loads before its first store: the output may alias the residual, so the compiler cannot hoist a load above an earlier
+// store by itself, and one pair at a time every pair would wait a full global-load latency.
+template <bool BF16>
+using pair_t = std::conditional_t<BF16, uint32_t, float2>;
+template <bool BF16>
+__device__ __forceinline__ pair_t<BF16> load_pair(const void* t, size_t e) {      // elements e, e+1
+  if constexpr (BF16) return *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(t) + e);
+  else return *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(t) + e);
+}
+__device__ __forceinline__ float2 unpack_pair(float2 v) { return v; }
+__device__ __forceinline__ float2 unpack_pair(uint32_t v) { return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u)); }
+template <bool BF16>
+__device__ __forceinline__ void store_pair(void* t, size_t e, float v0, float v1) {
+  if constexpr (BF16) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(t) + e) = pack_bf16(v0, v1);
+  else *reinterpret_cast<float2*>(reinterpret_cast<float*>(t) + e) = make_float2(v0, v1);
+}
 
 __device__ __forceinline__ void wgmma_tf32_n16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
