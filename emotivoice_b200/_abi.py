@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libemotivoice_b200.so")
 
 EV_OK = 0
+EV_ENOWEIGHT = -2
 EV_EPELEN = -5
 ACT_NONE, ACT_LRELU, ACT_RELU, ACT_GELU, ACT_TANH = 0, 1, 2, 3, 4
 ACC_STORE, ACC_ADD, ACC_ADD_DIV = 0, 1, 2

@@ -437,11 +437,6 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(ConvParams p, int S)
 
 }  // namespace tc
 
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return (e && *e) ? atoi(e) : dflt;
-}
-
 template <int MODE, int MT, int KBG, int PDLM>
 static int launch_tc_pdl(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
   static std::atomic<uint64_t> attr_devs{0};   // per instantiation; function attributes are per device
@@ -538,8 +533,7 @@ static int plan_conv1d_tc(const ConvParams& p, int mode, tc::Plan* out) {
   //    replicated A staging than it gains in parallelism).
   //  * rows per tile: as many 128-row accumulators as still leave about one tile per SM (every weight tile
   //    fetched from L2 then feeds MT MMAs), limited by the accumulator registers (MT x BN <= 128) and smem.
-  static const int bn_thresh = env_int("EV_TC_BN_TILES", 24);     // tuning knobs (tile shape only: results are unaffected)
-  static const int mt_thresh = env_int("EV_TC_MT_TILES", 120);
+  const int bn_thresh = 24, mt_thresh = 120;     // tuning constants (tile shape only: results are unaffected)
   const long long tiles128 = (long long)((p.L + tc::BM - 1) / tc::BM) * p.B;
   int BN = p.Cout <= 128 ? p.Cout : 128;          // == the packing tile of packing.to_tc_layout
   while (BN >= 64 && (BN / 2) % 16 == 0 && tiles128 * ((p.Cout + BN - 1) / BN) < bn_thresh) BN /= 2;

@@ -79,11 +79,14 @@ struct Tensor {
   uint64_t numel = 0;
 };
 
+// The weights of one GEMM-shaped layer: the plain fp32 copy (K, C_in, C_out) the FFMA kernels read, and the tensor-core copies
+// packing.add_tc_weights adds: '.tc' (two tf32 planes), '.tc16' (bf16), '.tc16x2' (two bf16 planes).  A copy the blob lacks is null.
+struct GemmW {
+  const float *w = nullptr, *tc = nullptr, *tc16 = nullptr, *tc16x2 = nullptr;
+};
 struct EncLayerW {
-  const float *ln1w, *ln1b, *wqkv, *bqkv, *wo, *bo, *ln2w, *ln2b, *w1, *b1, *w2, *b2;
-  const float *wqkv_tc = nullptr, *wo_tc = nullptr, *w1_tc = nullptr, *w2_tc = nullptr;   // tensor-core layout (optional)
-  const float *wqkv_h = nullptr, *wo_h = nullptr, *w1_h = nullptr, *w2_h = nullptr;       // bf16 tensor-core layout (optional)
-  const float *wqkv_x2 = nullptr, *wo_x2 = nullptr, *w1_x2 = nullptr, *w2_x2 = nullptr;   // two bf16 planes (bf16x3 emulation; decoder only)
+  const float *ln1w, *ln1b, *bqkv, *bo, *ln2w, *ln2b, *b1, *b2;
+  GemmW wqkv, wo, w1, w2;
 };
 struct StackW {
   const float* alpha;
@@ -91,21 +94,18 @@ struct StackW {
   const float *lnfw, *lnfb;
 };
 struct PredW {
-  std::vector<const float*> w, b, lnw, lnb, w_tc;
+  std::vector<GemmW> w;
+  std::vector<const float*> b, lnw, lnb;
   const float *linw, *linb;
 };
 struct ConvW {
-  const float *w, *b;
-  const float* w_tc = nullptr;
-  const float* w_h = nullptr;
-  const float* w_x2 = nullptr;     // two bf16 planes (hi, lo): the bf16x3 fp32 emulation of the granule-planar vocoder
+  GemmW w;
+  const float* b;
   int K, dil, cin, cout;
 };
 struct UpW {
-  const float *w, *b;
-  const float* w_tc = nullptr;
-  const float* w_h = nullptr;
-  const float* w_x2 = nullptr;
+  GemmW w;
+  const float* b;
   int K, cin, cout_packed, rate, cout;
 };
 
@@ -116,22 +116,19 @@ struct ev_ctx {
   int device = 0;
   bool bound = false;
   bool has_am = false, has_voc = false;
-  bool has_tc = false;      // every '.tc' tensor the tf32 path needs is present
   int precision = EV_PREC_FP32;
-  const float* mel_w_tc = nullptr;
-  const float* mel_w_h = nullptr;
-  const float* mel_w_x2 = nullptr;
-  const float* cond_wx_tc = nullptr;   // a blob may carry only one half (PromptTTS / Generator used alone)
   std::unordered_map<std::string, ev::Tensor> tensors;
   const float* pe = nullptr;
   int pe_len = 0;
   // resolved weights
   const float *emb_word = nullptr, *emb_spk = nullptr;
   ev::StackW enc, dec;
-  const float *cond_wx, *cond_wc, *cond_b;
+  ev::GemmW cond_wx;
+  const float *cond_wc, *cond_b;
   ev::PredW dur, pitch, energy;
   const float *pemb_w, *pemb_b, *eemb_w, *eemb_b;
-  const float *mel_w, *mel_b;
+  ev::GemmW mel_w;
+  const float* mel_b;
   ev::ConvW pre;
   std::vector<ev::UpW> ups;
   std::vector<ev::ConvW> rb_c1, rb_c2;   // [(stage*n_resk + j)*n_dil + l]
@@ -166,8 +163,7 @@ struct Phase2Bufs {
   size_t part_cap;
 };
 struct VocBufs {
-  float *X, *ACC, *part;
-  size_t part_cap;
+  float *X, *ACC;
   float *Tm, *R1, *R2;   // ResBlock chain scratch
   float *G0, *G1, *G2;   // small batches only: the three parallel ResBlocks of a stage advance together (grouped launches)
 };
@@ -209,8 +205,6 @@ static void carve_voc(const ev_ctx* c, Carver& cv, int B, int F, VocBufs* o) {
   const size_t n = (size_t)B * F * (size_t)c->max_stage_width;
   o->X = cv.take(n);
   o->ACC = cv.take(n);
-  o->part_cap = n / 2;                  // split-K partials of the first (widest-channel) stage: 2 slices of B*r0*F*C1
-  o->part = cv.take(o->part_cap);
   o->Tm = cv.take(n);
   o->R1 = cv.take(n);
   o->R2 = cv.take(n);
@@ -239,6 +233,15 @@ static const float* find_opt(ev_ctx* c, const std::string& name, uint64_t expect
   return it->second.p;
 }
 
+// the plain weight `name` of n elements, and whichever tensor-core copies of it the blob carries
+static int find_gemm(ev_ctx* c, const std::string& name, uint64_t n, GemmW* o) {
+  EV_TRY(find(c, name, n, &o->w));
+  o->tc = find_opt(c, name + ".tc", 2 * n);
+  o->tc16 = find_opt(c, name + ".tc16", n / 2);
+  o->tc16x2 = find_opt(c, name + ".tc16x2", n);
+  return EV_OK;
+}
+
 static int resolve_stack(ev_ctx* c, const char* pre, int n_layers, StackW* s) {
   const uint64_t H = c->cfg.hidden, K = c->cfg.ffn_kernel;
   std::string p(pre);
@@ -249,28 +252,16 @@ static int resolve_stack(ev_ctx* c, const char* pre, int n_layers, StackW* s) {
     EncLayerW& l = s->layers[i];
     EV_TRY(find(c, q + ".ln1.w", H, &l.ln1w));
     EV_TRY(find(c, q + ".ln1.b", H, &l.ln1b));
-    EV_TRY(find(c, q + ".wqkv", H * 3 * H, &l.wqkv));
+    EV_TRY(find_gemm(c, q + ".wqkv", H * 3 * H, &l.wqkv));
     EV_TRY(find(c, q + ".bqkv", 3 * H, &l.bqkv));
-    EV_TRY(find(c, q + ".wo", H * H, &l.wo));
+    EV_TRY(find_gemm(c, q + ".wo", H * H, &l.wo));
     EV_TRY(find(c, q + ".bo", H, &l.bo));
     EV_TRY(find(c, q + ".ln2.w", H, &l.ln2w));
     EV_TRY(find(c, q + ".ln2.b", H, &l.ln2b));
-    EV_TRY(find(c, q + ".w1", K * H * 4 * H, &l.w1));
+    EV_TRY(find_gemm(c, q + ".w1", K * H * 4 * H, &l.w1));
     EV_TRY(find(c, q + ".b1", 4 * H, &l.b1));
-    EV_TRY(find(c, q + ".w2", K * 4 * H * H, &l.w2));
+    EV_TRY(find_gemm(c, q + ".w2", K * 4 * H * H, &l.w2));
     EV_TRY(find(c, q + ".b2", H, &l.b2));
-    l.wqkv_tc = find_opt(c, q + ".wqkv.tc", 2 * H * 3 * H);
-    l.wo_tc = find_opt(c, q + ".wo.tc", 2 * H * H);
-    l.w1_tc = find_opt(c, q + ".w1.tc", 2 * K * H * 4 * H);
-    l.w2_tc = find_opt(c, q + ".w2.tc", 2 * K * 4 * H * H);
-    l.wqkv_h = find_opt(c, q + ".wqkv.tc16", H * 3 * H / 2);
-    l.wo_h = find_opt(c, q + ".wo.tc16", H * H / 2);
-    l.w1_h = find_opt(c, q + ".w1.tc16", K * H * 4 * H / 2);
-    l.w2_h = find_opt(c, q + ".w2.tc16", K * 4 * H * H / 2);
-    l.wqkv_x2 = find_opt(c, q + ".wqkv.tc16x2", H * 3 * H);
-    l.wo_x2 = find_opt(c, q + ".wo.tc16x2", H * H);
-    l.w1_x2 = find_opt(c, q + ".w1.tc16x2", K * H * 4 * H);
-    l.w2_x2 = find_opt(c, q + ".w2.tc16x2", K * 4 * H * H);
   }
   EV_TRY(find(c, p + ".lnf.w", H, &s->lnfw));
   EV_TRY(find(c, p + ".lnf.b", H, &s->lnfb));
@@ -280,11 +271,10 @@ static int resolve_stack(ev_ctx* c, const char* pre, int n_layers, StackW* s) {
 static int resolve_pred(ev_ctx* c, const char* pre, int n_layers, PredW* s) {
   const uint64_t H = c->cfg.hidden, K = c->cfg.pred_kernel;
   std::string p(pre);
-  s->w.resize(n_layers); s->b.resize(n_layers); s->lnw.resize(n_layers); s->lnb.resize(n_layers); s->w_tc.resize(n_layers);
+  s->w.resize(n_layers); s->b.resize(n_layers); s->lnw.resize(n_layers); s->lnb.resize(n_layers);
   for (int i = 0; i < n_layers; ++i) {
     std::string q = p + "." + std::to_string(i);
-    EV_TRY(find(c, q + ".w", K * H * H, &s->w[i]));
-    s->w_tc[i] = find_opt(c, q + ".w.tc", 2 * K * H * H);
+    EV_TRY(find_gemm(c, q + ".w", K * H * H, &s->w[i]));
     EV_TRY(find(c, q + ".b", H, &s->b[i]));
     EV_TRY(find(c, q + ".ln.w", H, &s->lnw[i]));
     EV_TRY(find(c, q + ".ln.b", H, &s->lnb[i]));
@@ -311,8 +301,7 @@ static int resolve_all(ev_ctx* c) {
   EV_TRY(find(c, "emb.spk", (uint64_t)g.n_speaker * H, &c->emb_spk));
   EV_TRY(resolve_stack(c, "enc", g.enc_layers, &c->enc));
   EV_TRY(resolve_stack(c, "dec", g.dec_layers, &c->dec));
-  EV_TRY(find(c, "cond.wx", H * H, &c->cond_wx));
-  c->cond_wx_tc = find_opt(c, "cond.wx.tc", 2 * H * H);
+  EV_TRY(find_gemm(c, "cond.wx", H * H, &c->cond_wx));
   EV_TRY(find(c, "cond.wc", (H + 2 * (uint64_t)g.bert_dim) * H, &c->cond_wc));
   EV_TRY(find(c, "cond.b", H, &c->cond_b));
   EV_TRY(resolve_pred(c, "dur", g.dur_layers, &c->dur));
@@ -322,22 +311,16 @@ static int resolve_all(ev_ctx* c) {
   EV_TRY(find(c, "pitch_emb.b", H, &c->pemb_b));
   EV_TRY(find(c, "energy_emb.w", (uint64_t)g.embed_kernel * H, &c->eemb_w));
   EV_TRY(find(c, "energy_emb.b", H, &c->eemb_b));
-  EV_TRY(find(c, "to_mel.w", H * g.n_mels, &c->mel_w));
+  EV_TRY(find_gemm(c, "to_mel.w", H * g.n_mels, &c->mel_w));
   EV_TRY(find(c, "to_mel.b", g.n_mels, &c->mel_b));
-  c->mel_w_tc = find_opt(c, "to_mel.w.tc", 2 * H * g.n_mels);
-  c->mel_w_h = find_opt(c, "to_mel.w.tc16", H * g.n_mels / 2);
-  c->mel_w_x2 = find_opt(c, "to_mel.w.tc16x2", H * g.n_mels);
   return EV_OK;
 }
 
 static int resolve_voc(ev_ctx* c) {
   const ev_config& g = c->cfg;
   c->pre.K = 7; c->pre.dil = 1; c->pre.cin = g.n_mels; c->pre.cout = g.voc_c0;
-  EV_TRY(find(c, "voc.pre.w", (uint64_t)7 * g.n_mels * g.voc_c0, &c->pre.w));
+  EV_TRY(find_gemm(c, "voc.pre.w", (uint64_t)7 * g.n_mels * g.voc_c0, &c->pre.w));
   EV_TRY(find(c, "voc.pre.b", g.voc_c0, &c->pre.b));
-  c->pre.w_tc = find_opt(c, "voc.pre.w.tc", (uint64_t)2 * 7 * g.n_mels * g.voc_c0);
-  c->pre.w_h = find_opt(c, "voc.pre.w.tc16", (uint64_t)7 * g.n_mels * g.voc_c0 / 2);
-  c->pre.w_x2 = find_opt(c, "voc.pre.w.tc16x2", (uint64_t)7 * g.n_mels * g.voc_c0);
   c->ups.resize(g.n_ups);
   c->rb_c1.clear(); c->rb_c2.clear();
   int ch = g.voc_c0, mul = 1;
@@ -355,10 +338,7 @@ static int resolve_voc(ev_ctx* c) {
       return EV_EINVAL;
     }
     u.K = (int)(it->second.numel / per_tap);
-    u.w = it->second.p;
-    u.w_tc = find_opt(c, q + ".w.tc", 2 * it->second.numel);
-    u.w_h = find_opt(c, q + ".w.tc16", it->second.numel / 2);
-    u.w_x2 = find_opt(c, q + ".w.tc16x2", it->second.numel);
+    EV_TRY(find_gemm(c, q + ".w", it->second.numel, &u.w));
     EV_TRY(find(c, q + ".b", u.cout_packed, &u.b));
     ch = u.cout; mul *= u.rate;
     if (mul * ch > c->max_stage_width) c->max_stage_width = mul * ch;
@@ -369,16 +349,10 @@ static int resolve_voc(ev_ctx* c) {
         ConvW c1, c2;
         c1.K = k; c1.dil = g.res_dils[j][l]; c1.cin = ch; c1.cout = ch;
         c2.K = k; c2.dil = 1; c2.cin = ch; c2.cout = ch;
-        EV_TRY(find(c, r + ".c1." + std::to_string(l) + ".w", (uint64_t)k * ch * ch, &c1.w));
+        EV_TRY(find_gemm(c, r + ".c1." + std::to_string(l) + ".w", (uint64_t)k * ch * ch, &c1.w));
         EV_TRY(find(c, r + ".c1." + std::to_string(l) + ".b", ch, &c1.b));
-        EV_TRY(find(c, r + ".c2." + std::to_string(l) + ".w", (uint64_t)k * ch * ch, &c2.w));
+        EV_TRY(find_gemm(c, r + ".c2." + std::to_string(l) + ".w", (uint64_t)k * ch * ch, &c2.w));
         EV_TRY(find(c, r + ".c2." + std::to_string(l) + ".b", ch, &c2.b));
-        c1.w_tc = find_opt(c, r + ".c1." + std::to_string(l) + ".w.tc", (uint64_t)2 * k * ch * ch);
-        c2.w_tc = find_opt(c, r + ".c2." + std::to_string(l) + ".w.tc", (uint64_t)2 * k * ch * ch);
-        c1.w_h = find_opt(c, r + ".c1." + std::to_string(l) + ".w.tc16", (uint64_t)k * ch * ch / 2);
-        c2.w_h = find_opt(c, r + ".c2." + std::to_string(l) + ".w.tc16", (uint64_t)k * ch * ch / 2);
-        c1.w_x2 = find_opt(c, r + ".c1." + std::to_string(l) + ".w.tc16x2", (uint64_t)k * ch * ch);
-        c2.w_x2 = find_opt(c, r + ".c2." + std::to_string(l) + ".w.tc16x2", (uint64_t)k * ch * ch);
         c->rb_c1.push_back(c1); c->rb_c2.push_back(c2);
       }
   }
@@ -389,80 +363,96 @@ static int resolve_voc(ev_ctx* c) {
   return EV_OK;
 }
 
-static int conv(const float* x, const float* w, const float* bias, long long bias_bs, const float* res, float* out,
-                int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul, int in_act,
-                float in_slope, int out_act, int acc, float div, cudaStream_t st) {
+static ConvParams conv_params(const float* x, const float* w, const float* bias, long long bias_bs, const float* res, float* out,
+                              int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul, int in_act,
+                              float in_slope, int out_act, int acc, float div) {
   ConvParams p;
   p.x = x; p.w = w; p.bias = bias; p.res = res; p.out = out; p.bias_bs = bias_bs;
   p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil;
   p.lens = lens; p.lens_mul = lens_mul; p.in_act = in_act; p.in_slope = in_slope;
   p.out_act = out_act; p.acc = acc; p.div = div;
-  return launch_conv1d(p, st);
+  return p;
+}
+// the fp32 FFMA kernel on time-major activations (conv1d_tm.cu)
+static int conv(const float* x, const float* w, const float* bias, long long bias_bs, const float* res, float* out,
+                int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul, int in_act,
+                float in_slope, int out_act, int acc, float div, cudaStream_t st) {
+  return launch_conv1d(conv_params(x, w, bias, bias_bs, res, out, B, L, Cin, Cout, K, dil, lens, lens_mul, in_act, in_slope, out_act,
+                                   acc, div), st);
 }
 
-// mode 0: fp32 FFMA kernel; 1: tensor cores, one tf32 MMA per K step; 3: tensor cores, 3xTF32 fp32 emulation;
-// 2: tensor cores, bf16 operands (needs w_h; layers without bf16 weights run 3xTF32).
-// Falls back to the FFMA kernel when the layer has no tensor-core weights or an unsupported shape.
-struct SplitWs {
-  float* p = nullptr;
-  size_t cap = 0;
-  int ksplit = 0;     // K-split factor for the convs launched next (set per layer, see conv1d_tc.cu)
-};
-static thread_local SplitWs g_split_ws;   // set by the phase entry points for the convs they launch
-
-static int set_split_ws(float* part, size_t cap, int ksplit) {
-  g_split_ws = SplitWs{};
-  g_split_ws.p = part; g_split_ws.cap = part ? cap : 0; g_split_ws.ksplit = ksplit;
-  return EV_OK;
-}
-
-// bf16x3 in the decoder (fp32 mode): EV_AM_FP32=tf32x3 keeps 3xTF32 there as well
-static inline bool am_bf16x3_enabled() {
-  static const int v = [] { const char* e = getenv("EV_AM_FP32"); return (e && e[0] == 't') ? 0 : 1; }();
-  return v == 1;
-}
-// w_x2: two bf16 planes; when given (decoder layers only) and the mode is the fp32-accurate one (3), the layer runs the bf16x3
-// emulation instead of 3xTF32.  The duration-critical prefix never passes it.
-static int conv_x(int mode, const float* w_tc, const float* w_h, const float* x, const float* w, const float* bias,
-                  long long bias_bs, const float* res, float* out, int B, int L, int Cin, int Cout, int K, int dil,
-                  const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act, int acc, float div,
-                  cudaStream_t st, const float* w_x2 = nullptr) {
-  const bool x3b = mode == 3 && w_x2 && (Cin % 16) == 0 && am_bf16x3_enabled();
-  if (mode == 2 && (!w_h || (Cin % 16))) mode = 3;
-  if (mode == 0 || (mode != 2 && !w_tc) || (Cin % 8) || (Cout % 16) || (Cout > 128 && Cout % 128))
-    return conv(x, w, bias, bias_bs, res, out, B, L, Cin, Cout, K, dil, lens, lens_mul, in_act, in_slope, out_act, acc, div, st);
-  ConvParams p;
-  p.x = x; p.w = x3b ? w_x2 : ((mode == 2) ? w_h : w_tc); p.bias = bias; p.res = res; p.out = out; p.bias_bs = bias_bs;
-  p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil;
-  p.lens = lens; p.lens_mul = lens_mul; p.in_act = in_act; p.in_slope = in_slope;
-  p.out_act = out_act; p.acc = acc; p.div = div;
-  p.splitk_ws = g_split_ws.p; p.splitk_cap = g_split_ws.cap; p.ksplit = g_split_ws.ksplit;
-  return launch_conv1d_tc(p, x3b ? 3 : (mode == 3 ? 1 : (mode == 2 ? 2 : 0)), st);
-}
-
-// HiFi-GAN convolution on granule-planar activations (conv1d_gp.cu).  mode as conv_x: 1 = tf32, 2 = bf16 (bf16 activations), 3 = 3xTF32.
-// In the fp32-accurate mode (3) the vocoder runs the "bf16x3" emulation when the blob carries the two-plane bf16 weights (half the
-// tensor-core and shared-memory cost of 3xTF32, ~1e-5 relative error; EV_VOC_FP32=tf32x3 keeps 3xTF32).
-static inline bool voc_bf16x3_enabled() {
-  static const int v = [] { const char* e = getenv("EV_VOC_FP32"); return (e && e[0] == 't') ? 0 : 1; }();
-  return v == 1;
-}
-static int gp_params(int mode, const float* w_tc, const float* w_h, const float* w_x2, const void* x, const float* bias, const void* res, void* out,
-                     int B, int L, int Cin, int Cout, int K, int dil, int rate, const int32_t* lens, int lens_mul, int in_act, float in_slope, int acc,
-                     float div, GpConvParams* o) {      // returns the kernel mode
-  GpConvParams& p = *o;
-  const bool x3b = mode == 3 && w_x2 && voc_bf16x3_enabled();
-  p.x = x; p.w = x3b ? w_x2 : ((mode == 2) ? w_h : w_tc); p.bias = bias; p.res = res; p.out = out;
+static GpConvParams gp_params(const float* w, const void* x, const float* bias, const void* res, void* out, int B, int L, int Cin,
+                              int Cout, int K, int dil, int rate, const int32_t* lens, int lens_mul, int in_act, float in_slope, int acc,
+                              float div) {
+  GpConvParams p;
+  p.x = x; p.w = w; p.bias = bias; p.res = res; p.out = out;
   p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil; p.rate = rate;
   p.lens = lens; p.lens_mul = lens_mul; p.in_act = in_act; p.in_slope = in_slope; p.acc = acc; p.div = div;
-  return x3b ? 3 : (mode == 3 ? 1 : (mode == 2 ? 2 : 0));
+  return p;
 }
-static int conv_gp(int mode, const float* w_tc, const float* w_h, const float* w_x2, const void* x, const float* bias, const void* res, void* out,
-                   int B, int L, int Cin, int Cout, int K, int dil, int rate, const int32_t* lens, int lens_mul, int in_act, float in_slope, int acc,
-                   float div, cudaStream_t st) {
-  GpConvParams p;
-  const int gm = gp_params(mode, w_tc, w_h, w_x2, x, bias, res, out, B, L, Cin, Cout, K, dil, rate, lens, lens_mul, in_act, in_slope, acc, div, &p);
-  return launch_conv1d_gp(p, gm, st);
+
+// Kernel MODEs of the tensor-core kernels (conv1d_tc.cu, conv1d_gp.cu, resblock_gp.cu): 0 = 1xTF32, 1 = 3xTF32, 2 = bf16 (bf16
+// activations in the vocoder), 3 = bf16x3.  kFfma: the fp32 FFMA kernels on the plain weights.
+enum { kFfma = -1 };
+static const char* const kModeCopy[4] = {".tc", ".tc", ".tc16", ".tc16x2"};   // the weight copy each MODE reads
+struct LayerRun {
+  const float* w;      // null when the blob lacks the copy
+  int mode;
+};
+
+// The one place a precision becomes arithmetic.  The duration-critical prefix (encoder, cond.wx, predictors) is fp32-accurate in every
+// precision: 3xTF32, or FFMA in "fp32_ffma".  The decoder, to_mel and the vocoder run bf16x3 / 1xTF32 / bf16 / FFMA in "fp32" /
+// "tf32" / "bf16" / "fp32_ffma".
+static LayerRun layer_run(const GemmW& l, int precision, bool prefix) {
+  if (precision == EV_PREC_FP32_FFMA) return {l.w, kFfma};
+  if (prefix) return {l.tc, 1};
+  if (precision == EV_PREC_TF32) return {l.tc, 0};
+  if (precision == EV_PREC_BF16) return {l.tc16, 2};
+  return {l.tc16x2, 3};
+}
+
+// EV_ENOWEIGHT unless every bound layer has the copy `precision` runs it on (blobs from packing.add_tc_weights carry all of them)
+static int check_weights(const ev_ctx* c, int precision, const char* who) {
+  int missing = -1;      // the MODE of the first layer without its copy
+  auto need = [&](const GemmW& l, bool prefix) {
+    const LayerRun r = layer_run(l, precision, prefix);
+    if (!r.w && missing < 0) missing = r.mode;
+  };
+  if (c->has_am) {
+    for (const EncLayerW& l : c->enc.layers) { need(l.wqkv, true); need(l.wo, true); need(l.w1, true); need(l.w2, true); }
+    need(c->cond_wx, true);
+    for (const PredW* p : {&c->dur, &c->pitch, &c->energy})
+      for (const GemmW& w : p->w) need(w, true);
+    for (const EncLayerW& l : c->dec.layers) { need(l.wqkv, false); need(l.wo, false); need(l.w1, false); need(l.w2, false); }
+    need(c->mel_w, false);
+  }
+  if (c->has_voc) {
+    need(c->pre.w, false);
+    for (const UpW& u : c->ups) need(u.w, false);
+    for (const ConvW& w : c->rb_c1) need(w.w, false);
+    for (const ConvW& w : c->rb_c2) need(w.w, false);
+  }
+  if (missing < 0) return EV_OK;
+  set_error("%s: precision %d needs the '%s' weight copies, which the bound blob lacks", who, precision, kModeCopy[missing]);
+  return EV_ENOWEIGHT;
+}
+
+// split-K scratch of a phase, carved from its workspace
+struct SplitWs {
+  float* p;
+  size_t cap;      // floats
+};
+
+// One GEMM-shaped layer of the acoustic model (a convolution over time; K = 1 is a linear layer) on the kernel layer_run picks.
+// ksplit: the layer's K-split factor on the tensor cores (conv1d_tc.cu), with the phase's scratch ws.
+static int conv_x(const ev_ctx* c, const GemmW& l, bool prefix, int ksplit, const SplitWs& ws, const float* x, const float* bias,
+                  long long bias_bs, const float* res, float* out, int B, int L, int Cin, int Cout, int K, const int32_t* lens,
+                  int out_act, cudaStream_t st) {
+  const LayerRun r = layer_run(l, c->precision, prefix);
+  ConvParams p = conv_params(x, r.w, bias, bias_bs, res, out, B, L, Cin, Cout, K, 1, lens, 1, EV_ACT_NONE, 0.f, out_act, EV_ACC_STORE, 1.f);
+  if (r.mode == kFfma) return launch_conv1d(p, st);
+  p.splitk_ws = ws.p; p.splitk_cap = ws.cap; p.ksplit = ksplit;
+  return launch_conv1d_tc(p, r.mode, st);
 }
 
 // One ResBlock layer through the fused kernel (resblock_gp.cu) where it takes the shape (C <= 128); EV_FUSE_RES=0 keeps two launches.
@@ -470,144 +460,134 @@ static inline bool fuse_res_enabled() {
   static const int v = [] { const char* e = getenv("EV_FUSE_RES"); return (e && e[0] == '0') ? 0 : 1; }();
   return v == 1;
 }
-static bool try_gp_pair(int mode, const ConvW& c1, const ConvW& c2, const void* src, void* dst, int B, int L, int C, const int32_t* lens, int lens_mul,
-                        int acc, float div, cudaStream_t st, int* rc, bool dry_run = false, GpPairParams* p_out = nullptr, int* gm_out = nullptr) {
-  if (!fuse_res_enabled() || c1.K != c2.K || c2.dil != 1) return false;
-  // Fused and unfused are bitwise equal, so the choice may depend on the batch: measured (profiles/r02_fused_vs_unfused.jsonl) the fused
-  // layer wins 1.1-1.8x on the HBM-bound shapes (k <= 7, or 32 channels) and wherever the launch count matters (batch 1), and loses
-  // ~25 % on 64 channels x 11 taps once the batch is large enough to be tensor / issue bound.
-  if (C >= 64 && c1.K > 7 && (long long)B * L > 4ll * 70000) return false;
-  const bool x3b = mode == 3 && c1.w_x2 && c2.w_x2 && voc_bf16x3_enabled();
-  const int gm = x3b ? 3 : (mode == 3 ? 1 : (mode == 2 ? 2 : 0));
-  GpPairParams p;
-  p.x = src; p.out = dst; p.b1 = c1.b; p.b2 = c2.b;
-  p.w1 = x3b ? c1.w_x2 : (mode == 2 ? c1.w_h : c1.w_tc);
-  p.w2 = x3b ? c2.w_x2 : (mode == 2 ? c2.w_h : c2.w_tc);
-  p.B = B; p.L = L; p.C = C; p.K = c1.K; p.dil = c1.dil; p.lens = lens; p.lens_mul = lens_mul; p.slope = 0.1f; p.acc = acc; p.div = div;
-  if (!p.w1 || !p.w2 || !gp_pair_supported(p, gm)) return false;
-  if (p_out) *p_out = p;
-  if (gm_out) *gm_out = gm;
-  if (!dry_run) *rc = launch_gp_pair(p, gm, st);
-  return true;
+// Fused and unfused are bitwise equal, so the choice may depend on the batch: measured (profiles/r02_fused_vs_unfused.jsonl) the fused
+// layer wins 1.1-1.8x on the HBM-bound shapes (k <= 7, or 32 channels) and wherever the launch count matters (batch 1), and loses
+// ~25 % on 64 channels x 11 taps once the batch is large enough to be tensor / issue bound.
+static bool fuse_layer(const GpPairParams& p, int mode) {
+  if (!fuse_res_enabled() || (p.C >= 64 && p.K > 7 && (long long)p.B * p.L > 4ll * 70000)) return false;
+  return gp_pair_supported(p, mode);
 }
 
-// One HiFi-GAN stage's ResBlocks (hifigan/models.py:120-126) with the three parallel blocks advancing together: the same-index
-// convolutions of the blocks (different taps / dilations / weights, one shape) are ONE launch.  Used while a single convolution has
-// fewer than two waves of tiles (batch 1: 68 / 135 tiles on 132 SMs); every tile is computed as in the ungrouped launches, so the
-// result is bitwise the same.  The last c2 of each block accumulates into xs in block order (three plain launches).
-// Returns false (nothing launched) when the stage does not qualify.
-static bool try_grouped_stage(ev_ctx* ctx, const VocBufs& v, int mode, size_t rb0, int B, int L, int C, const int32_t* lens, int mul, cudaStream_t st, int* rc) {
-  const ev_config& g = ctx->cfg;
-  const int J = g.n_resk, D = g.n_dil;
-  if (!v.G0 || J < 2 || J > 3 || D < 1) return false;
-  void* T[3] = {v.Tm, v.G0, v.G1};
-  void* Y[3] = {v.R1, v.R2, v.G2};
-  int frc = EV_OK;
-  // qualify: the stage's layers either all take the fused-pair kernel or none does, every step's members can share a launch, and
-  // one member alone is small
-  GpConvParams ps[3];
-  GpPairParams pp[3];
-  int gm = 0, n_pair = 0;
+// One (block j, layer l) step of a stage's ResBlocks, xt = c1(lrelu(x)); x = c2(lrelu(xt)) + x (hifigan/models.py:50-57): one fused
+// launch where the shape takes it, else two.
+struct ResStep {
+  bool fused;
+  GpPairParams pair;     // fused
+  GpConvParams c1, c2;   // unfused
+  void *in, *out;        // where the step reads x and where it leaves it
+};
+
+// A stage's buffers: X, its input, which no step writes; ACC, its output xs; and two buffers A[j], I[j] per block.  A grouped stage
+// gives every block its own; run one step after another, all blocks share R1 and Tm.
+struct StageBufs {
+  void *X, *ACC;
+  void *A[4], *I[4];
+};
+
+// Step (j, l) of a stage with layer input s (X at l = 0):
+//   * a fused layer writes s == A ? I : A (the fused kernel's output must not alias its input);
+//   * an unfused layer runs c1 into s == I ? A : I (never its own input), then c2 into s in place -- each residual element is read by
+//     the thread that overwrites it -- or into A when s is X;
+//   * to_acc: the last layer writes ACC instead, in block order xs = x_0, xs += x_j, xs = (xs + x_J-1) / J (:120-126).
+static ResStep res_step(const ev_ctx* ctx, const StageBufs& b, size_t rb0, int j, int l, void* s, bool to_acc, int B, int L, int C,
+                        const int32_t* lens, int mul) {
+  const int J = ctx->cfg.n_resk;
+  const ConvW& w1 = ctx->rb_c1[rb0 + (size_t)j * ctx->cfg.n_dil + l];
+  const ConvW& w2 = ctx->rb_c2[rb0 + (size_t)j * ctx->cfg.n_dil + l];
+  const LayerRun r1 = layer_run(w1.w, ctx->precision, false), r2 = layer_run(w2.w, ctx->precision, false);
+  const int acc = (!to_acc || j == 0) ? EV_ACC_STORE : (j == J - 1 ? EV_ACC_ADD_DIV : EV_ACC_ADD);
+  void *A = b.A[j], *I = b.I[j];
+  ResStep st{};
+  st.in = s;
+  st.pair = GpPairParams{s, r1.w, w1.b, r2.w, w2.b, to_acc ? b.ACC : (s == A ? I : A), B, L, C, w1.K, w1.dil, lens, mul, 0.1f, acc, (float)J};
+  st.fused = fuse_layer(st.pair, r1.mode);
+  if (st.fused) {
+    st.out = st.pair.out;
+    return st;
+  }
+  void* t = (s == I) ? A : I;
+  st.out = to_acc ? b.ACC : (s == b.X ? A : s);
+  st.c1 = gp_params(r1.w, s, w1.b, nullptr, t, B, L, C, C, w1.K, w1.dil, 1, lens, mul, EV_ACT_LRELU, 0.1f, EV_ACC_STORE, 1.f);
+  st.c2 = gp_params(r2.w, t, w2.b, s, st.out, B, L, C, C, w2.K, 1, 1, lens, mul, EV_ACT_LRELU, 0.1f, acc, (float)J);
+  return st;
+}
+
+// the members of one layer of a grouped stage, side by side as the grouped launches take them
+struct LayerGroup {
+  GpPairParams pair[3];
+  GpConvParams c1[3], c2[3];
+  LayerGroup(const ResStep* m, int J) {
+    for (int j = 0; j < J; ++j) { pair[j] = m[j].pair; c1[j] = m[j].c1; c2[j] = m[j].c2; }
+  }
+};
+
+// Grouping pays while one convolution has fewer than two waves of tiles (batch 1: 68 / 135 tiles on 132 SMs).  It needs the layers
+// all fused or none, and every layer's members able to share a launch.
+static bool groupable(ResStep (*s)[3], int J, int D, int mode) {
+  int n_fused = 0;
   for (int l = 0; l < D; ++l)
-    for (int j = 0; j < J; ++j)
-      n_pair += try_gp_pair(mode, ctx->rb_c1[rb0 + (size_t)j * D + l], ctx->rb_c2[rb0 + (size_t)j * D + l], v.X, Y[j], B, L, C, lens, mul, EV_ACC_STORE, 1.f, st,
-                            &frc, true) ? 1 : 0;
-  if (n_pair == J * D) {
-    // ---- fused layers: layer l of the three blocks is one launch (x -> Y, Y -> T, T -> Y, ...); the last layer accumulates into
-    // ---- xs block by block (three single launches) ----------------------------------------------------------------------------
-    for (int l = 0; l < D; ++l) {
-      for (int j = 0; j < J; ++j)
-        try_gp_pair(mode, ctx->rb_c1[rb0 + (size_t)j * D + l], ctx->rb_c2[rb0 + (size_t)j * D + l], v.X, Y[j], B, L, C, lens, mul, EV_ACC_STORE, 1.f, st, &frc, true,
-                    &pp[j], &gm);
-      if (!gp_pair_group_supported(pp, J, gm)) return false;
-    }
-    if (gp_pair_solo_tiles(pp[0], gm) >= 2 * sm_count()) return false;
-    *rc = EV_OK;
-    for (int l = 0; l < D && *rc == EV_OK; ++l) {
-      const bool last = (l == D - 1);
-      // fp32 storage: the last layer is grouped too, into the blocks' own tensors, and one elementwise pass forms ((y1 + y0) + y2) / n
-      // -- the additions of the accumulate modes in their order, identical bits.  (With bf16 storage xs is rounded after every
-      // accumulation, which that pass cannot reproduce: three single launches.)
-      const bool sum_pass = last && gm != 2 && D >= 2;
-      for (int j = 0; j < J; ++j) {
-        const void* src = l == 0 ? (const void*)v.X : ((l & 1) ? Y[j] : T[j]);
-        void* dst = (last && !sum_pass) ? (void*)v.ACC : ((l & 1) ? T[j] : Y[j]);
-        int acc = EV_ACC_STORE;
-        if (last && !sum_pass && j > 0) acc = (j == J - 1) ? EV_ACC_ADD_DIV : EV_ACC_ADD;
-        try_gp_pair(mode, ctx->rb_c1[rb0 + (size_t)j * D + l], ctx->rb_c2[rb0 + (size_t)j * D + l], src, dst, B, L, C, lens, mul, acc, (float)J, st, &frc, true,
-                    &pp[j], &gm);
-      }
-      if (!last || sum_pass) {
-        *rc = launch_gp_pair_group(pp, J, gm, st);
-        if (sum_pass && *rc == EV_OK)
-          *rc = launch_gp_sum_div((const float*)pp[0].out, (const float*)pp[1].out, J == 3 ? (const float*)pp[2].out : nullptr, v.ACC, (size_t)B * L * C, (float)J, st);
-      } else {
-        for (int j = 0; j < J && *rc == EV_OK; ++j) *rc = launch_gp_pair(pp[j], gm, st);
-      }
-    }
-    return true;
-  }
-  if (n_pair != 0) return false;
+    for (int j = 0; j < J; ++j) n_fused += s[l][j].fused ? 1 : 0;
+  if (n_fused != 0 && n_fused != J * D) return false;
   for (int l = 0; l < D; ++l) {
-    for (int j = 0; j < J; ++j) {
-      const ConvW& c1 = ctx->rb_c1[rb0 + (size_t)j * D + l];
-      gm = gp_params(mode, c1.w_tc, c1.w_h, c1.w_x2, v.X, c1.b, nullptr, T[j], B, L, C, C, c1.K, c1.dil, 1, lens, mul, EV_ACT_LRELU, 0.1f, EV_ACC_STORE, 1.f, &ps[j]);
-      if (!ps[j].w) return false;
-    }
-    if (!gp_group_supported(ps, J, gm)) return false;
-    for (int j = 0; j < J; ++j) {
-      const ConvW& c2 = ctx->rb_c2[rb0 + (size_t)j * D + l];
-      gp_params(mode, c2.w_tc, c2.w_h, c2.w_x2, T[j], c2.b, v.X, Y[j], B, L, C, C, c2.K, 1, 1, lens, mul, EV_ACT_LRELU, 0.1f, EV_ACC_STORE, 1.f, &ps[j]);
-      if (!ps[j].w) return false;
-    }
-    if (!gp_group_supported(ps, J, gm)) return false;
+    const LayerGroup m(s[l], J);
+    if (n_fused ? !gp_pair_group_supported(m.pair, J, mode) : !(gp_group_supported(m.c1, J, mode) && gp_group_supported(m.c2, J, mode)))
+      return false;
   }
-  if (gp_solo_tiles(ps[0], gm) >= 2 * sm_count()) return false;
-  *rc = EV_OK;
-  for (int l = 0; l < D && *rc == EV_OK; ++l) {
-    const bool last = (l == D - 1);
-    const bool sum_pass = last && gm != 2 && D >= 2;      // see the fused path above
-    for (int j = 0; j < J; ++j) {      // xt_j = c1_j(lrelu(x_j))
-      const ConvW& c1 = ctx->rb_c1[rb0 + (size_t)j * D + l];
-      gp_params(mode, c1.w_tc, c1.w_h, c1.w_x2, l == 0 ? (const void*)v.X : Y[j], c1.b, nullptr, T[j], B, L, C, C, c1.K, c1.dil, 1, lens, mul, EV_ACT_LRELU, 0.1f,
-                EV_ACC_STORE, 1.f, &ps[j]);
-    }
-    *rc = launch_conv1d_gp_group(ps, J, gm, st);
-    if (*rc != EV_OK) break;
-    for (int j = 0; j < J; ++j) {      // x_j = c2_j(lrelu(xt_j)) + x_j  (in place from the second layer on: a thread reads and writes its own elements)
-      const ConvW& c2 = ctx->rb_c2[rb0 + (size_t)j * D + l];
-      const void* res = l == 0 ? (const void*)v.X : Y[j];
-      int acc = EV_ACC_STORE;
-      if (last && j > 0) acc = (j == J - 1) ? EV_ACC_ADD_DIV : EV_ACC_ADD;       // xs += ...; x = xs / n
-      if (sum_pass) acc = EV_ACC_STORE;
-      gp_params(mode, c2.w_tc, c2.w_h, c2.w_x2, T[j], c2.b, res, (last && !sum_pass) ? (void*)v.ACC : Y[j], B, L, C, C, c2.K, 1, 1, lens, mul, EV_ACT_LRELU, 0.1f, acc,
-                (float)J, &ps[j]);
-    }
-    if (!last || sum_pass) {
-      *rc = launch_conv1d_gp_group(ps, J, gm, st);
-      if (sum_pass && *rc == EV_OK)
-        *rc = launch_gp_sum_div((const float*)Y[0], (const float*)Y[1], J == 3 ? (const float*)Y[2] : nullptr, v.ACC, (size_t)B * L * C, (float)J, st);
-    } else {
-      for (int j = 0; j < J && *rc == EV_OK; ++j) *rc = launch_conv1d_gp(ps[j], gm, st);
+  const ResStep& a = s[D - 1][0];
+  return (n_fused ? gp_pair_solo_tiles(a.pair, mode) : gp_solo_tiles(a.c2, mode)) < 2 * sm_count();
+}
+
+// One HiFi-GAN stage's ResBlocks (hifigan/models.py:120-126): ACC = sum_j ResBlock_j(X) / J.  Where the stage buffers exist (small
+// batches, carve_voc) and the stage is groupable, the J blocks advance together: the same-index convolutions of the blocks (different
+// taps / dilations / weights, one shape) are ONE launch.  Every tile is computed as in the ungrouped launches: bitwise the same.
+static int run_resblocks(const ev_ctx* ctx, const VocBufs& v, size_t rb0, int mode, int B, int L, int C, const int32_t* lens, int mul,
+                         cudaStream_t st) {
+  const int J = ctx->cfg.n_resk, D = ctx->cfg.n_dil;
+  if (v.G0 && J >= 2 && J <= 3) {
+    const StageBufs b = {v.X, v.ACC, {v.R1, v.R2, v.G2}, {v.Tm, v.G0, v.G1}};
+    ResStep s[4][3];
+    for (int l = 0; l < D; ++l)
+      for (int j = 0; j < J; ++j) s[l][j] = res_step(ctx, b, rb0, j, l, l ? s[l - 1][j].out : v.X, false, B, L, C, lens, mul);
+    if (groupable(s, J, D, mode)) {
+      // fp32 storage: the last layer is grouped too, into the blocks' own buffers, and one elementwise pass forms ((x1 + x0) + x2) / J
+      // -- the additions of the accumulate modes in their order, identical bits.  bf16 storage rounds xs after every accumulation,
+      // which that pass cannot reproduce: there the last layer accumulates into ACC block by block.
+      const bool sum_pass = mode != 2 && D >= 2;
+      for (int l = 0; l < D; ++l) {
+        const LayerGroup m(s[l], J);
+        const bool fused = s[l][0].fused;
+        if (l < D - 1 || sum_pass) {
+          EV_TRY(fused ? launch_gp_pair_group(m.pair, J, mode, st) : launch_conv1d_gp_group(m.c1, J, mode, st));
+          if (!fused) EV_TRY(launch_conv1d_gp_group(m.c2, J, mode, st));
+          continue;
+        }
+        if (!fused) EV_TRY(launch_conv1d_gp_group(m.c1, J, mode, st));     // c1 does not depend on where the layer's output goes
+        for (int j = 0; j < J; ++j) {
+          const ResStep a = res_step(ctx, b, rb0, j, l, s[l][j].in, true, B, L, C, lens, mul);
+          EV_TRY(fused ? launch_gp_pair(a.pair, mode, st) : launch_conv1d_gp(a.c2, mode, st));
+        }
+      }
+      if (!sum_pass) return EV_OK;
+      const ResStep* last = s[D - 1];
+      return launch_gp_sum_div((const float*)last[0].out, (const float*)last[1].out, J == 3 ? (const float*)last[2].out : nullptr, v.ACC,
+                               (size_t)B * L * C, (float)J, st);
     }
   }
-  return true;
-}
-
-// The vocoder runs on granule-planar activations whenever it runs on the tensor cores (every mode but "fp32_ffma");
-// EV_VOC_LAYOUT=tm keeps the round-1 time-major path (conv1d_tc.cu) for A/B measurements.
-static inline bool voc_gp_enabled() {
-  static const int v = [] { const char* e = getenv("EV_VOC_LAYOUT"); return (e && e[0] == 't') ? 0 : 1; }();
-  return v == 1;
-}
-
-static inline int body_mode(const ev_ctx* c) {
-  return c->precision == EV_PREC_FP32_FFMA ? 0 : (c->precision == EV_PREC_TF32 ? 1 : (c->precision == EV_PREC_BF16 ? 2 : 3));
-}
-
-static inline bool attn_tc_enabled() {
-  static const int v = [] { const char* e = getenv("EV_ATTN"); return (e && e[0] == 'f') ? 0 : 1; }();
-  return v == 1;
+  const StageBufs b = {v.X, v.ACC, {v.R1, v.R1, v.R1, v.R1}, {v.Tm, v.Tm, v.Tm, v.Tm}};
+  for (int j = 0; j < J; ++j) {
+    void* x = v.X;
+    for (int l = 0; l < D; ++l) {
+      const ResStep s = res_step(ctx, b, rb0, j, l, x, l == D - 1, B, L, C, lens, mul);
+      if (s.fused) {
+        EV_TRY(launch_gp_pair(s.pair, mode, st));
+      } else {
+        EV_TRY(launch_conv1d_gp(s.c1, mode, st));
+        EV_TRY(launch_conv1d_gp(s.c2, mode, st));
+      }
+      x = s.out;
+    }
+  }
+  return EV_OK;
 }
 
 // Encoder.forward (encoder.py:316-324) minus the positional prologue (done by the caller of this
@@ -621,34 +601,26 @@ static const StackSplits kEncSplits = {4, 8, 4, 16};
 static const StackSplits kDecSplits = {2, 4, 4, 8};
 
 static int run_stack(const ev_ctx* c, const StackW& s, float* x, float* y, float* qkv, float* ctxb, float* h,
-                     int B, int L, const int32_t* key_lens, const int32_t* conv_lens, bool first_ln_done, int mode,
-                     const StackSplits& sp, cudaStream_t st) {
+                     int B, int L, const int32_t* key_lens, const int32_t* conv_lens, bool first_ln_done, bool prefix,
+                     const StackSplits& sp, const SplitWs& ws, cudaStream_t st) {
   const int H = c->cfg.hidden, K = c->cfg.ffn_kernel, heads = c->cfg.n_heads;
   for (size_t i = 0; i < s.layers.size(); ++i) {
     const EncLayerW& l = s.layers[i];
     if (!(i == 0 && first_ln_done))
       EV_TRY(launch_layernorm(x, nullptr, nullptr, nullptr, nullptr, nullptr, l.ln1w, l.ln1b, y, B * L, L, H, st));
-    g_split_ws.ksplit = sp.qkv;
-    EV_TRY(conv_x(mode, l.wqkv_tc, l.wqkv_h, y, l.wqkv, l.bqkv, 0, nullptr, qkv, B, L, H, 3 * H, 1, 1, conv_lens, 1, EV_ACT_NONE, 0.f,
-                  EV_ACT_NONE, EV_ACC_STORE, 1.f, st, l.wqkv_x2));
-    // QK^T / softmax / PV: tensor cores (3xTF32 where the layer runs fp32-accurate, one tf32 MMA otherwise) for d_k = 48; the fp32 FFMA
-    // flash kernel in the "fp32_ffma" mode, for other head sizes, or with EV_ATTN=ffma (A/B measurements)
-    if (mode != 0 && H / heads == 48 && attn_tc_enabled())
-      EV_TRY(launch_attention_tc(qkv, key_lens, ctxb, B, L, H, heads, mode == 3 ? 1 : 0, st));
+    EV_TRY(conv_x(c, l.wqkv, prefix, sp.qkv, ws, y, l.bqkv, 0, nullptr, qkv, B, L, H, 3 * H, 1, conv_lens, EV_ACT_NONE, st));
+    // QK^T / softmax / PV on the tensor cores for d_k = 48: 3xTF32 beside fp32-accurate layers (MODE 1 / 3), one tf32 MMA otherwise;
+    // the fp32 FFMA flash kernel in the "fp32_ffma" mode and for other head sizes
+    const int mode = layer_run(l.wqkv, c->precision, prefix).mode;
+    if (mode != kFfma && H / heads == 48)
+      EV_TRY(launch_attention_tc(qkv, key_lens, ctxb, B, L, H, heads, (mode == 1 || mode == 3) ? 1 : 0, st));
     else
       EV_TRY(launch_attention(qkv, key_lens, ctxb, B, L, H, heads, st));
-    g_split_ws.ksplit = sp.wo;
-    EV_TRY(conv_x(mode, l.wo_tc, l.wo_h, ctxb, l.wo, l.bo, 0, x, x, B, L, H, H, 1, 1, conv_lens, 1, EV_ACT_NONE, 0.f, EV_ACT_NONE,
-                  EV_ACC_STORE, 1.f, st, l.wo_x2));
+    EV_TRY(conv_x(c, l.wo, prefix, sp.wo, ws, ctxb, l.bo, 0, x, x, B, L, H, H, 1, conv_lens, EV_ACT_NONE, st));
     EV_TRY(launch_layernorm(x, nullptr, nullptr, nullptr, nullptr, nullptr, l.ln2w, l.ln2b, y, B * L, L, H, st));
-    g_split_ws.ksplit = sp.ffn1;
-    EV_TRY(conv_x(mode, l.w1_tc, l.w1_h, y, l.w1, l.b1, 0, nullptr, h, B, L, H, 4 * H, K, 1, conv_lens, 1, EV_ACT_NONE, 0.f, EV_ACT_GELU,
-                  EV_ACC_STORE, 1.f, st, l.w1_x2));
-    g_split_ws.ksplit = sp.ffn2;
-    EV_TRY(conv_x(mode, l.w2_tc, l.w2_h, h, l.w2, l.b2, 0, x, x, B, L, 4 * H, H, K, 1, conv_lens, 1, EV_ACT_NONE, 0.f, EV_ACT_NONE,
-                  EV_ACC_STORE, 1.f, st, l.w2_x2));
+    EV_TRY(conv_x(c, l.w1, prefix, sp.ffn1, ws, y, l.b1, 0, nullptr, h, B, L, H, 4 * H, K, conv_lens, EV_ACT_GELU, st));
+    EV_TRY(conv_x(c, l.w2, prefix, sp.ffn2, ws, h, l.b2, 0, x, x, B, L, 4 * H, H, K, conv_lens, EV_ACT_NONE, st));
   }
-  g_split_ws.ksplit = 2;
   EV_TRY(launch_layernorm(x, nullptr, nullptr, nullptr, nullptr, nullptr, s.lnfw, s.lnfb, y, B * L, L, H, st));
   return EV_OK;
 }
@@ -656,13 +628,12 @@ static int run_stack(const ev_ctx* c, const StackW& s, float* x, float* y, float
 // [conv k -> ReLU -> channel LN] x n -> Linear(H -> 1) (variance.py:36-56, :101-124)
 static int run_predictor(const ev_ctx* c, const PredW& p, const float* in, float* t1, float* t2, int B, int T,
                          const int32_t* lens, const int32_t* conv_lens, int mode, float* out_f, int64_t* out_i,
-                         int cmode, cudaStream_t st) {
+                         const SplitWs& ws, cudaStream_t st) {
   const int H = c->cfg.hidden, K = c->cfg.pred_kernel;
-  g_split_ws.ksplit = 8;      // K = 3H on ~100 tokens and 3 N tiles: eight slices (see StackSplits)
   const float* cur = in;
   for (size_t i = 0; i < p.w.size(); ++i) {
-    EV_TRY(conv_x(cmode, p.w_tc[i], nullptr, cur, p.w[i], p.b[i], 0, nullptr, t1, B, T, H, H, K, 1, conv_lens, 1, EV_ACT_NONE, 0.f,
-                  EV_ACT_RELU, EV_ACC_STORE, 1.f, st));
+    // K = 3H on ~100 tokens and 3 N tiles: eight slices (see StackSplits)
+    EV_TRY(conv_x(c, p.w[i], true, 8, ws, cur, p.b[i], 0, nullptr, t1, B, T, H, H, K, conv_lens, EV_ACT_RELU, st));
     EV_TRY(launch_layernorm(t1, nullptr, nullptr, nullptr, nullptr, nullptr, p.lnw[i], p.lnb[i], t2, B * T, T, H, st));
     cur = t2;
   }
@@ -734,6 +705,7 @@ int ev_bind_weights(ev_ctx* ctx, const float* blob, size_t n_floats, const ev_we
     ctx->tensors[std::string(nm)] = t;
   }
   EV_TRY(resolve_all(ctx));
+  EV_TRY(check_weights(ctx, ctx->precision, "ev_bind_weights"));
   ctx->bound = true;
   return EV_OK;
 }
@@ -798,34 +770,30 @@ int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64
   carve_phase1(ctx, cv, B, T, &b);
   if (cv.off > workspace_bytes) { set_error("ev_am_phase1: workspace %zu < %zu bytes", workspace_bytes, cv.off); return EV_EWORKSPACE; }
   EV_TRY(use_device(ctx));
-  EV_TRY(set_split_ws(b.part, b.part_cap, 2));
+  const SplitWs ws{b.part, b.part_cap};
   // lengths -> int32, plus range checks of ids / speakers / lengths into the status word mel_lens_out[B + 1]
   EV_TRY(launch_validate_inputs(ling, lens64, spk, lens32_out, mel_lens_out + B + 1, B, T, g.n_vocab, g.n_speaker, st));
   const int32_t* lens = lens32_out;
   const int32_t* conv_lens = invariant ? lens : nullptr;
-  // the duration-critical prefix is fp32-accurate in every mode: 3xTF32 on the tensor cores, or FFMA
-  const int prefix_mode = (ctx->precision == EV_PREC_FP32_FFMA) ? 0 : 3;
 
   Range r_phase("ev:am_phase1");
   // encoder: x = word_emb[ids] + alpha*pe (model_open_source.py:107, encoder.py:257-261), fused with LN1 of layer 0
   EV_TRY(launch_layernorm(nullptr, ling, ctx->emb_word, ctx->pe, ctx->enc.alpha, b.x, ctx->enc.layers[0].ln1w,
                           ctx->enc.layers[0].ln1b, b.y, B * T, T, H, st, g.n_vocab));
-  EV_TRY(run_stack(ctx, ctx->enc, b.x, b.y, b.qkv, b.ctx, b.h, B, T, lens, conv_lens, true, prefix_mode, kEncSplits, st));
-  g_split_ws.ksplit = 4;
+  EV_TRY(run_stack(ctx, ctx->enc, b.x, b.y, b.qkv, b.ctx, b.h, B, T, lens, conv_lens, true, true, kEncSplits, ws, st));
   // conditioning (model_open_source.py:109-111): per-utterance bias + W_x x
   EV_TRY(launch_cond_gather(spk, ctx->emb_spk, style, content, b.cond_in, B, H, g.bert_dim, g.n_speaker, st));
   EV_TRY(launch_cond_gemv(b.cond_in, ctx->cond_wc, ctx->cond_b, b.cond_bias, B, H + 2 * g.bert_dim, H, st));
-  EV_TRY(conv_x(prefix_mode, ctx->cond_wx_tc, nullptr, b.y, ctx->cond_wx, b.cond_bias, H, nullptr, b.hs, B, T, H, H, 1, 1, conv_lens, 1,
-                EV_ACT_NONE, 0.f, EV_ACT_NONE, EV_ACC_STORE, 1.f, st));
+  EV_TRY(conv_x(ctx, ctx->cond_wx, true, 4, ws, b.y, b.cond_bias, H, nullptr, b.hs, B, T, H, H, 1, conv_lens, EV_ACT_NONE, st));
   // predictors (model_open_source.py:120-121,130)
   const float* pin = b.hs;
   if (!invariant) {   // literal batch: masked_fill on the input only (variance.py:38-39); pads of hs are live data
     EV_TRY(launch_mask_rows(b.hs, lens, b.pm, B, T, H, st));
     pin = b.pm;
   }
-  EV_TRY(run_predictor(ctx, ctx->pitch, pin, b.p1[0], b.p2[0], B, T, lens, conv_lens, 0, pitch_out, nullptr, prefix_mode, st));
-  EV_TRY(run_predictor(ctx, ctx->energy, pin, b.p1[1], b.p2[1], B, T, lens, conv_lens, 0, energy_out, nullptr, prefix_mode, st));
-  EV_TRY(run_predictor(ctx, ctx->dur, pin, b.p1[2], b.p2[2], B, T, lens, conv_lens, 1, nullptr, dur_out, prefix_mode, st));
+  EV_TRY(run_predictor(ctx, ctx->pitch, pin, b.p1[0], b.p2[0], B, T, lens, conv_lens, 0, pitch_out, nullptr, ws, st));
+  EV_TRY(run_predictor(ctx, ctx->energy, pin, b.p1[1], b.p2[1], B, T, lens, conv_lens, 0, energy_out, nullptr, ws, st));
+  EV_TRY(run_predictor(ctx, ctx->dur, pin, b.p1[2], b.p2[2], B, T, lens, conv_lens, 1, nullptr, dur_out, ws, st));
   // x = x + pitch_embed + energy_embed (model_open_source.py:131-134), the tracks shifted / scaled per item when prosody is given
   EV_TRY(launch_var_embed_add(b.hs, pitch_out, energy_out, ctx->pemb_w, ctx->pemb_b, ctx->eemb_w, ctx->eemb_b, prosody, conv_lens,
                               B, T, H, g.embed_kernel, st));
@@ -851,17 +819,14 @@ int ev_am_phase2(ev_ctx* ctx, const void* phase1_workspace, const int32_t* lens,
   carve_phase2(ctx, cv, B, F, &b);
   if (cv.off > workspace_bytes) { set_error("ev_am_phase2: workspace %zu < %zu bytes", workspace_bytes, cv.off); return EV_EWORKSPACE; }
   const int32_t* flens = invariant ? mel_lens : nullptr;
-  EV_TRY(set_split_ws(b.part, b.part_cap, 2));
+  const SplitWs ws{b.part, b.part_cap};
   Range r_phase("ev:am_phase2");
   // length regulator + the decoder's positional encoding (alignment.py:198-211, encoder.py:257-261)
   EV_TRY(launch_gauss_upsample(b1.hs, b1.centers, lens, mel_lens, B, T, H, F, invariant, ctx->pe, ctx->dec.alpha, b.x, st));
   // decoder (model_open_source.py:146: mask None in the reference; per-item lengths under the invariant contract)
-  const int mode = body_mode(ctx);
-  EV_TRY(run_stack(ctx, ctx->dec, b.x, b.y, b.qkv, b.ctx, b.h, B, F, flens, flens, false, mode, kDecSplits, st));
-  g_split_ws.ksplit = 2;
+  EV_TRY(run_stack(ctx, ctx->dec, b.x, b.y, b.qkv, b.ctx, b.h, B, F, flens, flens, false, false, kDecSplits, ws, st));
   // to_mel (model_open_source.py:147)
-  EV_TRY(conv_x(mode, ctx->mel_w_tc, ctx->mel_w_h, b.y, ctx->mel_w, ctx->mel_b, 0, nullptr, mel_out, B, F, H, g.n_mels, 1, 1, flens, 1,
-                EV_ACT_NONE, 0.f, EV_ACT_NONE, EV_ACC_STORE, 1.f, st, ctx->mel_w_x2));
+  EV_TRY(conv_x(ctx, ctx->mel_w, false, 2, ws, b.y, ctx->mel_b, 0, nullptr, mel_out, B, F, H, g.n_mels, 1, flens, EV_ACT_NONE, st));
   return EV_OK;
 }
 
@@ -877,33 +842,29 @@ int ev_vocoder(ev_ctx* ctx, const float* mel, int mel_time_major, const int32_t*
   VocBufs v;
   carve_voc(ctx, cv, B, F, &v);
   if (cv.off > workspace_bytes) { set_error("ev_vocoder: workspace %zu < %zu bytes", workspace_bytes, cv.off); return EV_EWORKSPACE; }
-  const int mode = body_mode(ctx);
-  if (mode != 0 && voc_gp_enabled()) {
-    // ---- granule-planar path: [b][C/cpg][l][cpg] activations, bulk-copied A operands, direct coalesced epilogues ----
+  static const char* const kStageNames[8] = {"voc:stage1", "voc:stage2", "voc:stage3", "voc:stage4", "voc:stage5", "voc:stage6",
+                                             "voc:stage7", "voc:stage8"};
+  int L = F, mul = 1;
+  if (ctx->precision == EV_PREC_FP32_FFMA) {
+    // ---- "fp32_ffma": time-major activations and the fp32 FFMA kernel ----
+    const float* m = mel;
+    if (!mel_time_major) {
+      EV_TRY(launch_transpose_cf_to_tm(mel, v.Tm, B, g.n_mels, F, st));
+      m = v.Tm;
+    }
     Range r_phase("ev:vocoder");
-    const int bf = (mode == 2) ? 1 : 0;
-    // mel (B,F,n_mels) time-major or (B,n_mels,F) channels-first -> GP
-    EV_TRY(launch_to_gp(mel, (long long)F * g.n_mels, mel_time_major ? g.n_mels : 1, mel_time_major ? 1 : F, v.Tm, B, F, g.n_mels, bf, st));
     // conv_pre (hifigan/models.py:116)
-    EV_TRY(conv_gp(mode, ctx->pre.w_tc, ctx->pre.w_h, ctx->pre.w_x2, v.Tm, ctx->pre.b, nullptr, v.ACC, B, F, g.n_mels, g.voc_c0, ctx->pre.K, 1, 1, mel_lens, 1,
-                   EV_ACT_NONE, 0.f, EV_ACC_STORE, 1.f, st));
-    int L = F, mul = 1;
+    EV_TRY(conv(m, ctx->pre.w.w, ctx->pre.b, 0, nullptr, v.ACC, B, F, g.n_mels, g.voc_c0, ctx->pre.K, 1, mel_lens, 1, EV_ACT_NONE, 0.f,
+                EV_ACT_NONE, EV_ACC_STORE, 1.f, st));
     size_t rb = 0;
-    static const char* const kNames[8] = {"voc:stage1", "voc:stage2", "voc:stage3", "voc:stage4", "voc:stage5", "voc:stage6", "voc:stage7", "voc:stage8"};
     for (int s = 0; s < g.n_ups; ++s) {
-      Range r_stage(kNames[s & 7]);
+      Range r_stage(kStageNames[s & 7]);
       const UpW& u = ctx->ups[s];
-      // x = ups[i](leaky_relu(x, 0.1)) (:118-119): polyphase transposed conv, the `rate` output phases are GEMM column groups
-      EV_TRY(conv_gp(mode, u.w_tc, u.w_h, u.w_x2, v.ACC, u.b, nullptr, v.X, B, L, u.cin, u.cout_packed, u.K, 1, u.rate, mel_lens, mul, EV_ACT_LRELU, 0.1f,
-                     EV_ACC_STORE, 1.f, st));
+      // x = ups[i](leaky_relu(x, 0.1)) (:118-119): polyphase-packed transposed conv, output viewed (L, rate*Cout)
+      EV_TRY(conv(v.ACC, u.w.w, u.b, 0, nullptr, v.X, B, L, u.cin, u.cout_packed, u.K, 1, mel_lens, mul, EV_ACT_LRELU, 0.1f, EV_ACT_NONE,
+                  EV_ACC_STORE, 1.f, st));
       L *= u.rate; mul *= u.rate;
       const int C = u.cout;
-      int grc = EV_OK;
-      if (try_grouped_stage(ctx, v, mode, rb, B, L, C, mel_lens, mul, st, &grc)) {
-        EV_TRY(grc);
-        rb += (size_t)g.n_resk * g.n_dil;
-        continue;
-      }
       for (int j = 0; j < g.n_resk; ++j) {
         const float* src = v.X;
         for (int l = 0; l < g.n_dil; ++l, ++rb) {
@@ -913,76 +874,40 @@ int ev_vocoder(ev_ctx* ctx, const float* mel, int mel_time_major, const int32_t*
           float* dst = last ? v.ACC : ((l & 1) ? v.R2 : v.R1);
           int acc = EV_ACC_STORE;
           if (last && j > 0) acc = (j == g.n_resk - 1) ? EV_ACC_ADD_DIV : EV_ACC_ADD;   // xs += ...; x = xs / n (:120-126)
-          if (last && g.n_resk == 1) acc = EV_ACC_STORE;
-          // xt = c1(lrelu(x)) ; x = c2(lrelu(xt)) + x   (:50-57): one fused kernel where the shape fits, else two launches
-          int frc = EV_OK;
-          if (try_gp_pair(mode, c1, c2, src, dst, B, L, C, mel_lens, mul, acc, (float)g.n_resk, st, &frc)) {
-            EV_TRY(frc);
-            src = dst;
-            continue;
-          }
-          EV_TRY(conv_gp(mode, c1.w_tc, c1.w_h, c1.w_x2, src, c1.b, nullptr, v.Tm, B, L, C, C, c1.K, c1.dil, 1, mel_lens, mul, EV_ACT_LRELU, 0.1f,
-                         EV_ACC_STORE, 1.f, st));
-          EV_TRY(conv_gp(mode, c2.w_tc, c2.w_h, c2.w_x2, v.Tm, c2.b, src, dst, B, L, C, C, c2.K, 1, 1, mel_lens, mul, EV_ACT_LRELU, 0.1f, acc,
-                         (float)g.n_resk, st));
+          // xt = c1(lrelu(x)) ; x = c2(lrelu(xt)) + x   (:50-57)
+          EV_TRY(conv(src, c1.w.w, c1.b, 0, nullptr, v.Tm, B, L, C, C, c1.K, c1.dil, mel_lens, mul, EV_ACT_LRELU, 0.1f, EV_ACT_NONE,
+                      EV_ACC_STORE, 1.f, st));
+          EV_TRY(conv(v.Tm, c2.w.w, c2.b, 0, src, dst, B, L, C, C, c2.K, 1, mel_lens, mul, EV_ACT_LRELU, 0.1f, EV_ACT_NONE, acc,
+                      (float)g.n_resk, st));
           src = dst;
         }
       }
     }
     EV_CHECK_ARG(mul == ctx->total_up, "ev_vocoder: internal rate mismatch");
     // x = leaky_relu(x) [slope 0.01]; conv_post; tanh (:127-129)
-    return launch_conv_post_gp(v.ACC, bf, ctx->post_w, ctx->post_b, mel_lens, mul, B, L, ctx->ups.back().cout, ctx->post_k, 0.01f, wav_out, st);
+    return launch_conv_post(v.ACC, ctx->post_w, ctx->post_b, mel_lens, mul, B, L, ctx->ups.back().cout, ctx->post_k, 0.01f, wav_out, st);
   }
-  EV_TRY(set_split_ws(v.part, v.part_cap, 0));
-  const float* m = mel;
-  if (!mel_time_major) {
-    EV_TRY(launch_transpose_cf_to_tm(mel, v.Tm, B, g.n_mels, F, st));
-    m = v.Tm;
-  }
+  // ---- tensor cores: granule-planar [b][C/cpg][l][cpg] activations, bulk-copied A operands, direct coalesced epilogues ----
   Range r_phase("ev:vocoder");
+  const LayerRun pre = layer_run(ctx->pre.w, ctx->precision, false);
+  const int mode = pre.mode, bf = (mode == 2) ? 1 : 0;      // bf16: bf16 activations in HBM
+  // mel (B,F,n_mels) time-major or (B,n_mels,F) channels-first -> GP
+  EV_TRY(launch_to_gp(mel, (long long)F * g.n_mels, mel_time_major ? g.n_mels : 1, mel_time_major ? 1 : F, v.Tm, B, F, g.n_mels, bf, st));
   // conv_pre (hifigan/models.py:116)
-  EV_TRY(conv_x(mode, ctx->pre.w_tc, ctx->pre.w_h, m, ctx->pre.w, ctx->pre.b, 0, nullptr, v.ACC, B, F, g.n_mels, g.voc_c0, ctx->pre.K, 1,
-                mel_lens, 1, EV_ACT_NONE, 0.f, EV_ACT_NONE, EV_ACC_STORE, 1.f, st));
-  int L = F, mul = 1;
-  size_t rb = 0;
-  static const char* const kStageNames[8] = {"voc:stage1", "voc:stage2", "voc:stage3", "voc:stage4", "voc:stage5", "voc:stage6",
-                                             "voc:stage7", "voc:stage8"};
+  EV_TRY(launch_conv1d_gp(gp_params(pre.w, v.Tm, ctx->pre.b, nullptr, v.ACC, B, F, g.n_mels, g.voc_c0, ctx->pre.K, 1, 1, mel_lens, 1,
+                                    EV_ACT_NONE, 0.f, EV_ACC_STORE, 1.f), mode, st));
   for (int s = 0; s < g.n_ups; ++s) {
     Range r_stage(kStageNames[s & 7]);
     const UpW& u = ctx->ups[s];
-    // no K-split in the vocoder: outputs are large, the partial-sum traffic costs more than the shorter reduction gains
-    // (measured: 2-slice K-split of stage 1 gains 4.6 % at batch 1 and costs 6 % at batch 32)
-    g_split_ws.ksplit = 0;
-    // x = ups[i](leaky_relu(x, 0.1)) (:118-119): polyphase-packed transposed conv, output viewed (L, rate*Cout)
-    EV_TRY(conv_x(mode, u.w_tc, u.w_h, v.ACC, u.w, u.b, 0, nullptr, v.X, B, L, u.cin, u.cout_packed, u.K, 1, mel_lens, mul,
-                  EV_ACT_LRELU, 0.1f, EV_ACT_NONE, EV_ACC_STORE, 1.f, st));
+    // x = ups[i](leaky_relu(x, 0.1)) (:118-119): polyphase transposed conv, the `rate` output phases are GEMM column groups
+    EV_TRY(launch_conv1d_gp(gp_params(layer_run(u.w, ctx->precision, false).w, v.ACC, u.b, nullptr, v.X, B, L, u.cin, u.cout_packed, u.K, 1,
+                                      u.rate, mel_lens, mul, EV_ACT_LRELU, 0.1f, EV_ACC_STORE, 1.f), mode, st));
     L *= u.rate; mul *= u.rate;
-    const int C = u.cout;
-    for (int j = 0; j < g.n_resk; ++j) {
-      const float* src = v.X;
-      for (int l = 0; l < g.n_dil; ++l, ++rb) {
-        const ConvW& c1 = ctx->rb_c1[rb];
-        const ConvW& c2 = ctx->rb_c2[rb];
-        const bool last = (l == g.n_dil - 1);
-        float* dst = last ? v.ACC : ((l & 1) ? v.R2 : v.R1);
-        int acc = EV_ACC_STORE;
-        if (last && j > 0) acc = (j == g.n_resk - 1) ? EV_ACC_ADD_DIV : EV_ACC_ADD;   // xs += ...; x = xs / n (:120-126)
-        const float div = (float)g.n_resk;
-        if (last && g.n_resk == 1) acc = EV_ACC_STORE;
-        // xt = c1(lrelu(x)) ; x = c2(lrelu(xt)) + x   (:50-57)
-        EV_TRY(conv_x(mode, c1.w_tc, c1.w_h, src, c1.w, c1.b, 0, nullptr, v.Tm, B, L, C, C, c1.K, c1.dil, mel_lens, mul,
-                      EV_ACT_LRELU, 0.1f, EV_ACT_NONE, EV_ACC_STORE, 1.f, st));
-        EV_TRY(conv_x(mode, c2.w_tc, c2.w_h, v.Tm, c2.w, c2.b, 0, src, dst, B, L, C, C, c2.K, 1, mel_lens, mul, EV_ACT_LRELU, 0.1f,
-                      EV_ACT_NONE, acc, div, st));
-        src = dst;
-      }
-    }
+    EV_TRY(run_resblocks(ctx, v, (size_t)s * g.n_resk * g.n_dil, mode, B, L, u.cout, mel_lens, mul, st));
   }
-  // x = leaky_relu(x) [slope 0.01]; conv_post; tanh (:127-129)
   EV_CHECK_ARG(mul == ctx->total_up, "ev_vocoder: internal rate mismatch");
-  const int Cl = ctx->ups.back().cout;
-  EV_TRY(launch_conv_post(v.ACC, ctx->post_w, ctx->post_b, mel_lens, mul, B, L, Cl, ctx->post_k, 0.01f, wav_out, st));
-  return EV_OK;
+  // x = leaky_relu(x) [slope 0.01]; conv_post; tanh (:127-129)
+  return launch_conv_post_gp(v.ACC, bf, ctx->post_w, ctx->post_b, mel_lens, mul, B, L, ctx->ups.back().cout, ctx->post_k, 0.01f, wav_out, st);
 }
 
 int ev_wav_to_pcm16(const float* wav, int16_t* pcm, size_t n, void* stream) {
@@ -1014,21 +939,15 @@ int ev_op_conv1d_tc_ks(const float* x, const float* w_tc, int split3, const floa
                        size_t splitk_floats, void* stream) {
   EV_CHECK_ARG(x && w_tc && out, "ev_op_conv1d_tc: null argument");
   EV_CHECK_ARG(ksplit <= 1 || splitk_ws, "ev_op_conv1d_tc: ksplit=%d needs split-K scratch", ksplit);
+  EV_CHECK_ARG(split3 >= 0 && split3 <= 3, "ev_op_conv1d_tc: split3=%d is not a kernel mode (0..3)", split3);
   EV_TRY(use_device_of(x));
-  EV_TRY(set_split_ws(splitk_ws, splitk_floats, splitk_ws ? ksplit : 0));
   EV_CHECK_ARG(Cin % 8 == 0 && Cout % 16 == 0 && (Cout <= 128 || Cout % 128 == 0),
                "ev_op_conv1d_tc: needs Cin %% 8 == 0, Cout %% 16 == 0 and Cout <= 128 or a multiple of 128 (Cin=%d Cout=%d)", Cin, Cout);
   EV_CHECK_ARG(split3 < 2 || Cin % 16 == 0, "ev_op_conv1d_tc: the bf16 / bf16x3 modes need Cin %% 16 == 0 (Cin=%d)", Cin);
-  if (split3 == 3) {      // bf16x3: w_tc holds the two bf16 planes
-    ConvParams p;
-    p.x = x; p.w = w_tc; p.bias = bias; p.res = res; p.out = out; p.bias_bs = (long long)bias_bstride;
-    p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil; p.lens = lens; p.lens_mul = lens_mul; p.in_act = in_act; p.in_slope = in_slope;
-    p.out_act = out_act; p.acc = acc; p.div = div;
-    p.splitk_ws = g_split_ws.p; p.splitk_cap = g_split_ws.cap; p.ksplit = g_split_ws.ksplit;
-      return launch_conv1d_tc(p, 3, reinterpret_cast<cudaStream_t>(stream));
-  }
-  return conv_x(split3 == 2 ? 2 : (split3 ? 3 : 1), w_tc, w_tc, x, nullptr, bias, (long long)bias_bstride, res, out, B, L, Cin, Cout, K, dil, lens, lens_mul,
-                in_act, in_slope, out_act, acc, div, reinterpret_cast<cudaStream_t>(stream));
+  ConvParams p = conv_params(x, w_tc, bias, (long long)bias_bstride, res, out, B, L, Cin, Cout, K, dil, lens, lens_mul, in_act, in_slope,
+                             out_act, acc, div);
+  p.splitk_ws = splitk_ws; p.splitk_cap = splitk_ws ? splitk_floats : 0; p.ksplit = splitk_ws ? ksplit : 0;
+  return launch_conv1d_tc(p, split3, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ev_debug_tc_plan(int B, int L, int Cin, int Cout, int K, int dil, int split3, int ksplit, int* out11) {
@@ -1043,10 +962,8 @@ int ev_op_conv1d_gp(const void* x, const float* w, int mode, const float* bias, 
                     int K, int dil, int rate, const int32_t* lens, int lens_mul, int in_act, float in_slope, int acc, float div, void* stream) {
   EV_CHECK_ARG(x && w && out, "ev_op_conv1d_gp: null argument");
   EV_TRY(use_device_of(x));
-  GpConvParams p;
-  p.x = x; p.w = w; p.bias = bias; p.res = res; p.out = out; p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil; p.rate = rate;
-  p.lens = lens; p.lens_mul = lens_mul; p.in_act = in_act; p.in_slope = in_slope; p.acc = acc; p.div = div;
-  return launch_conv1d_gp(p, mode, reinterpret_cast<cudaStream_t>(stream));
+  return launch_conv1d_gp(gp_params(w, x, bias, res, out, B, L, Cin, Cout, K, dil, rate, lens, lens_mul, in_act, in_slope, acc, div), mode,
+                          reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ev_op_conv1d_gp_group(int n, const void* const* x, const float* const* w, int mode, const float* const* bias, const void* const* res, void* const* out,
@@ -1151,35 +1068,7 @@ int ev_set_precision(ev_ctx* ctx, int precision) {
   EV_CHECK_ARG(ctx, "ev_set_precision: null context");
   EV_CHECK_ARG(precision == EV_PREC_FP32 || precision == EV_PREC_TF32 || precision == EV_PREC_FP32_FFMA || precision == EV_PREC_BF16,
                "ev_set_precision: unknown precision %d", precision);
-  if (precision != EV_PREC_FP32_FFMA && ctx->bound) {
-    bool ok = true;
-    if (ctx->has_am) {
-      ok = ok && ctx->mel_w_tc && ctx->cond_wx_tc;
-      for (const auto* st : {&ctx->enc, &ctx->dec})
-        for (const auto& l : st->layers) ok = ok && l.wqkv_tc && l.wo_tc && l.w1_tc && l.w2_tc;
-      for (const auto* pr : {&ctx->dur, &ctx->pitch, &ctx->energy})
-        for (const float* w : pr->w_tc) ok = ok && w;
-    }
-    if (ctx->has_voc) {
-      ok = ok && ctx->pre.w_tc;
-      for (const auto& u : ctx->ups) ok = ok && u.w_tc;
-      for (const auto& c1 : ctx->rb_c1) ok = ok && c1.w_tc;
-      for (const auto& c2 : ctx->rb_c2) ok = ok && c2.w_tc;
-    }
-    if (precision == EV_PREC_BF16) {
-      if (ctx->has_am) {
-        ok = ok && ctx->mel_w_h;
-        for (const auto& l : ctx->dec.layers) ok = ok && l.wqkv_h && l.wo_h && l.w1_h && l.w2_h;
-      }
-      if (ctx->has_voc) {
-        ok = ok && ctx->pre.w_h;
-        for (const auto& u : ctx->ups) ok = ok && u.w_h;
-        for (const auto& c1 : ctx->rb_c1) ok = ok && c1.w_h;
-        for (const auto& c2 : ctx->rb_c2) ok = ok && c2.w_h;
-      }
-    }
-    if (!ok) { set_error("ev_set_precision: the bound blob lacks the '.tc' / '.tc16' (tensor-core layout) weights"); return EV_ENOWEIGHT; }
-  }
+  if (ctx->bound) EV_TRY(check_weights(ctx, precision, "ev_set_precision"));
   ctx->precision = precision;
   return EV_OK;
 }

@@ -17,7 +17,6 @@ ABI in include/emotivoice_b200.h.  PyTorch provides device memory and the stream
 is no CPU path: calling ``forward`` on CPU tensors raises.
 """
 import ctypes
-import os
 import threading
 
 import numpy as np
@@ -34,7 +33,6 @@ class _Holder(nn.Module):
         raise RuntimeError("parameter holder: compute happens in libemotivoice_b200.so")
 
 
-_HOST_WAIT_BLOCK = os.environ.get("EV_HOST_WAIT", "") == "block"
 _TLS = threading.local()          # per-thread pinned read-back buffer + event
 
 
@@ -157,9 +155,9 @@ class _Engine:
             self.index = packing.index_from_meta(index_meta)
             self.blob = blob
             assert blob.device == self.device and blob.dtype == torch.float32 and blob.is_contiguous()
+        self.set_precision(precision)         # first: binding checks that the blob carries the weight copies this precision reads
         _abi.check(self.lib.ev_bind_weights(self.handle, self.blob.data_ptr(), self.blob.numel(),
                                             ctypes.cast(self.index, ctypes.c_void_p), len(self.index)))
-        self.set_precision(precision)
         self.pe = None
         self._arena = {}              # (stream, kind) -> uint8 workspace, grow-only
         self.call_lock = threading.RLock()      # one forward at a time enqueues on an engine (its workspaces are reused, stream-ordered)
@@ -217,9 +215,7 @@ class _Engine:
             self._ws("p2", max(lib.ev_phase2_workspace_bytes(self.handle, int(batch), f) for f in fs))
 
     def _read_back(self, t):
-        """Device int32 vector -> host tensor, waiting by polling (EV_HOST_WAIT=block: a blocking copy)."""
-        if _HOST_WAIT_BLOCK:
-            return t.cpu()
+        """Device int32 vector -> host tensor, waiting by polling."""
         tl = _TLS
         n = t.numel()
         if getattr(tl, "pin", None) is None or tl.pin.numel() < n:

@@ -103,15 +103,19 @@ EV_API int ev_bind_weights(ev_ctx* ctx, const float* blob, size_t n_floats,
 EV_API int ev_bind_pe(ev_ctx* ctx, const float* pe, int pe_len);
 
 /* Arithmetic of the GEMM-shaped layers (linear / conv / transposed conv):
- *   EV_PREC_FP32 (default): fp32-accurate on the tensor cores by 3xTF32 splitting (x = hi + lo,
- *     three tf32 MMAs per K step, fp32 accumulation); error ~1e-6 relative, like an fp32 FFMA chain.
+ *   EV_PREC_FP32 (default): fp32-accurate on the tensor cores: the duration-critical prefix (encoder, conditioning,
+ *     predictors) by 3xTF32 splitting (x = hi + lo, three tf32 MMAs per K step), decoder + vocoder by bf16x3 splitting
+ *     (two bf16 planes, three bf16 MMAs per K step); fp32 accumulation, error ~1e-6 / ~1e-5 relative.
  *   EV_PREC_TF32: decoder + vocoder with ONE tf32 MMA per K step (operands rounded to nearest tf32) -- the
  *     arithmetic the reference's eager PyTorch uses for convolutions on a GPU (cudnn.allow_tf32 default);
  *     the duration-critical prefix (encoder, conditioning, predictors) stays 3xTF32.
  *   EV_PREC_BF16: decoder + vocoder with bf16 operands (wgmma bf16, fp32 accumulation; activations stay fp32
  *     in HBM and are rounded by the staging warps); prefix 3xTF32 like EV_PREC_TF32.  BASELINE.json configs[2].
  *   EV_PREC_FP32_FFMA: plain fp32 FFMA kernels everywhere (no tensor cores; the round-1 baseline path).
- * Attention, LayerNorm, softmax, upsampling and the heads are fp32 in every mode. */
+ * Attention, LayerNorm, softmax, upsampling and the heads are fp32 in every mode.
+ * Each mode reads one weight copy per layer ('.tc', '.tc16' or '.tc16x2'; packing.add_tc_weights writes all of them):
+ * ev_bind_weights checks the blob against the context's mode and ev_set_precision a bound blob against the new mode: a missing
+ * copy returns EV_ENOWEIGHT, leaving the context unbound / in its previous mode. */
 enum { EV_PREC_FP32 = 0, EV_PREC_TF32 = 1, EV_PREC_FP32_FFMA = 2, EV_PREC_BF16 = 3 };
 EV_API int ev_set_precision(ev_ctx* ctx, int precision);
 

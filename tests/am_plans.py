@@ -6,20 +6,18 @@ the reference configuration:
     mask_rows in the literal batch (invariant = 0), the pitch / energy / duration predictors (run_predictor), var_embed_add and
     the duration scan;
   * ev_am_phase2: the Gaussian upsampling, the decoder (run_stack) and to_mel;
-  * conv_x's choice of the kernel MODE: the duration-critical prefix (encoder, cond.wx, predictors) always runs 3xTF32
-    (MODE 1); the decoder and to_mel run bf16x3 (MODE 3; MODE 1 under EV_AM_FP32=tf32x3) in "fp32", 1xTF32 (MODE 0) in "tf32"
-    and bf16 (MODE 2) in "bf16";
+  * layer_run's choice of the kernel MODE: the duration-critical prefix (encoder, cond.wx, predictors) always runs 3xTF32
+    (MODE 1); the decoder and to_mel run bf16x3 (MODE 3) in "fp32", 1xTF32 (MODE 0) in "tf32" and bf16 (MODE 2) in "bf16";
   * every layer's K-split factor S (kEncSplits, kDecSplits, 8 for the predictors, 4 for cond.wx, 2 for to_mel), clamped to
     the layer's C_in blocks, with one splitk_reduce launch after the convolution whenever the clamped S is > 1;
-  * attention_tc (tc_mode 1 where the layer runs fp32-accurate, 0 otherwise) for d_k = 48, the FFMA attention under
-    EV_ATTN=ffma.
+  * attention_tc (tc_mode 1 where the layer runs fp32-accurate, 0 otherwise) for d_k = 48, the FFMA attention for other
+    head sizes.
 A GPU test holds the length of this list to ev_launch_count(), so it cannot drift from engine.cu unnoticed.
 
 The plan key of a convolution is (MODE, MT, KBG, BN, a_stages, b_stages, producer groups, ksplit): the template instantiation,
 the tile width, and the ring depths and producer groups that fix the mbarrier protocol the kernel runs.
 """
 import ctypes
-import os
 
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 2, 3           # _abi.ACT_*
 ENC_SPLITS = dict(qkv=4, wo=8, ffn1=4, ffn2=16)  # engine.cu kEncSplits
@@ -30,13 +28,7 @@ PREFIX_MODE = 1
 
 def decoder_mode(prec):
     """Kernel MODE of the decoder's and to_mel's convolutions in a precision."""
-    if prec == "fp32":
-        return 1 if os.environ.get("EV_AM_FP32", "").startswith("t") else 3
-    return {"tf32": 0, "bf16": 2}[prec]
-
-
-def attn_tc():
-    return not os.environ.get("EV_ATTN", "").startswith("f")
+    return {"fp32": 3, "tf32": 0, "bf16": 2}[prec]
 
 
 def tc_plan(lib, B, L, Cin, Cout, K, mode, ksplit):
@@ -70,7 +62,7 @@ def _stack(sh, tag, B, L, mode, splits, first_ln_done, conv_lens, attn_mode, out
         if not (i == 0 and first_ln_done):
             out.append(("layernorm",))
         out.append(layer(tag + ".qkv", B, L, H, 3 * H, 1, mode, splits["qkv"], lens=conv_lens))
-        out.append(("attention_tc", attn_mode) if attn_tc() and H // sh["heads"] == 48 else ("attention",))
+        out.append(("attention_tc", attn_mode) if H // sh["heads"] == 48 else ("attention",))
         out.append(layer(tag + ".wo", B, L, H, H, 1, mode, splits["wo"], inplace=True, lens=conv_lens))
         out.append(("layernorm",))
         out.append(layer(tag + ".ffn1", B, L, H, 4 * H, K, mode, splits["ffn1"], out_act=ACT_GELU, lens=conv_lens))

@@ -122,7 +122,7 @@ def test_bounds_separate_the_modes():
 
 
 # ---- the launch list of one ev_vocoder call ------------------------------------------------------------------------------
-_KERNEL_MODE = {"tf32": 0, "bf16": 2, "fp32": 1 if os.environ.get("EV_VOC_FP32", "").startswith("t") else 3}
+_KERNEL_MODE = {"tf32": 0, "bf16": 2, "fp32": 3}
 POINTS = [  # (B, frames per item): grouped / ungrouped, 64-channel k11 unfused / 128-channel k11 unfused as well
     (1, (1024,)),
     (3, (900, 517, 1)),
