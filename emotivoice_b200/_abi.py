@@ -85,6 +85,14 @@ SIGNATURES = {
     "ev_op_attention_tc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ev_op_gauss_upsample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ev_op_duration_scan": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "ev_op_gauss_upsample_centers": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "ev_op_layernorm_embed": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "ev_op_cond_bias": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "ev_op_rowdot": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "ev_op_mask_rows": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "ev_op_var_embed_add": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "ev_op_bert_embed_ln": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "ev_op_row_gemv": (_i, [_vp, _sz, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ev_op_mas": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_op_average_by_duration": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "ev_op_align_logp": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),

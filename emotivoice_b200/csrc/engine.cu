@@ -1105,6 +1105,56 @@ int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* len
   return launch_gauss_upsample(hs, centers_tmp, lens, mel_lens_tmp, B, T, H, F, invariant, pe, alpha, out, st);
 }
 
+int ev_op_gauss_upsample_centers(const float* hs, const float* centers, const int32_t* lens, const int32_t* mel_lens, int B, int T,
+                                 int H, int F, int invariant, const float* pe, const float* alpha, float* out, void* stream) {
+  EV_CHECK_ARG(hs && centers && out && (mel_lens || !invariant) && (alpha || !pe), "ev_op_gauss_upsample_centers: null argument");
+  EV_CHECK_ARG(B > 0, "ev_op_gauss_upsample_centers: B=%d", B);
+  EV_TRY(use_device_of(hs));
+  return launch_gauss_upsample(hs, centers, lens, mel_lens, B, T, H, F, invariant, pe, alpha, out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ev_op_layernorm_embed(const int64_t* ids, const float* emb, int n_emb, const float* pe, const float* alpha, int L, float* x_out,
+                          const float* w, const float* b, float* y, int rows, int C, void* stream) {
+  EV_CHECK_ARG(ids && emb && pe && alpha && x_out && w && b && y, "ev_op_layernorm_embed: null argument");
+  EV_CHECK_ARG(L > 0, "ev_op_layernorm_embed: L=%d", L);
+  EV_TRY(use_device_of(emb));
+  return launch_layernorm(nullptr, ids, emb, pe, alpha, x_out, w, b, y, rows, L, C, reinterpret_cast<cudaStream_t>(stream), n_emb);
+}
+
+int ev_op_cond_bias(const int64_t* spk, const float* spk_emb, int n_spk, const float* style, const float* content, int B, int H, int bert,
+                    const float* w, const float* bias, float* cond_in, float* out, void* stream) {
+  EV_CHECK_ARG(spk && spk_emb && style && content && w && bias && cond_in && out, "ev_op_cond_bias: null argument");
+  EV_CHECK_ARG(n_spk > 0 && H > 0 && H % 8 == 0 && bert >= 0 && B > 0 && B <= 65535, "ev_op_cond_bias: B=%d n_spk=%d H=%d bert=%d", B,
+               n_spk, H, bert);
+  EV_TRY(use_device_of(w));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  EV_TRY(launch_cond_gather(spk, spk_emb, style, content, cond_in, B, H, bert, n_spk, st));
+  return launch_cond_gemv(cond_in, w, bias, out, B, H + 2 * bert, H, st);
+}
+
+int ev_op_rowdot(const float* x, const float* w, const float* b, const int32_t* lens, int B, int T, int C, int mode, float* out_f,
+                 int64_t* out_i, void* stream) {
+  EV_CHECK_ARG(x && w && b && (mode == 0 ? out_f != nullptr : (mode == 1 && out_i)), "ev_op_rowdot: null argument or mode %d", mode);
+  EV_CHECK_ARG(B > 0 && T > 0, "ev_op_rowdot: B=%d T=%d", B, T);
+  EV_TRY(use_device_of(x));
+  return launch_rowdot(x, w, b, lens, B, T, C, mode, out_f, out_i, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ev_op_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T, int C, void* stream) {
+  EV_CHECK_ARG(x && y, "ev_op_mask_rows: null argument");
+  EV_CHECK_ARG(B > 0 && T > 0 && C > 0, "ev_op_mask_rows: B=%d T=%d C=%d", B, T, C);
+  EV_TRY(use_device_of(x));
+  return launch_mask_rows(x, lens, y, B, T, C, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ev_op_var_embed_add(float* x, const float* pitch, const float* energy, const float* wp, const float* bp, const float* we, const float* be,
+                        const float* prosody, const int32_t* lens, int B, int T, int C, int K, void* stream) {
+  EV_CHECK_ARG(x && pitch && energy && wp && bp && we && be, "ev_op_var_embed_add: null argument");
+  EV_CHECK_ARG(B > 0 && T > 0 && C > 0 && K > 0 && (K & 1), "ev_op_var_embed_add: B=%d T=%d C=%d K=%d", B, T, C, K);
+  EV_TRY(use_device_of(x));
+  return launch_var_embed_add(x, pitch, energy, wp, bp, we, be, prosody, lens, B, T, C, K, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int invariant, int B, int T, float* centers,
                         float* ds, int32_t* mel_lens, void* stream) {
   EV_CHECK_ARG(dur && centers && ds && mel_lens, "ev_op_duration_scan: null argument");

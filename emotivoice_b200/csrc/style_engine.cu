@@ -341,4 +341,20 @@ int ev_style_forward(ev_style_ctx* c, const int64_t* ids, const int64_t* type_id
   return EV_OK;
 }
 
+int ev_op_bert_embed_ln(const int64_t* ids, const int64_t* type_ids, const float* word, const float* type, const float* pos, const float* w,
+                        const float* b, float* y, int rows, int N, int C, void* stream) {
+  EV_CHECK_ARG(ids && type_ids && word && type && pos && w && b && y, "ev_op_bert_embed_ln: null argument");
+  EV_CHECK_ARG(N > 0, "ev_op_bert_embed_ln: N=%d", N);
+  EV_TRY(use_device_of(word));
+  return launch_bert_embed_ln(ids, type_ids, word, type, pos, w, b, y, rows, N, C, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ev_op_row_gemv(const float* x, size_t x_stride, const float* w, const float* bias, float* out, int B, int K, int N, int act,
+                   void* stream) {
+  EV_CHECK_ARG(x && w && bias && out, "ev_op_row_gemv: null argument");
+  EV_CHECK_ARG(K > 0 && (act == EV_ACT_NONE || act == EV_ACT_TANH), "ev_op_row_gemv: K=%d act=%d", K, act);
+  EV_TRY(use_device_of(x));
+  return launch_row_gemv(x, x_stride, w, bias, out, B, K, N, act, reinterpret_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

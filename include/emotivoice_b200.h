@@ -295,6 +295,33 @@ EV_API int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const fl
 EV_API int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* lens, int B, int T, int H,
                                 int F, int invariant, const float* pe, const float* alpha, float* centers_tmp,
                                 int32_t* mel_lens_tmp, float* out, void* stream);
+/* The Gaussian upsampling launch of ev_am_phase2 alone, on given centres (B,T) f32 and frame counts mel_lens (B) i32 (the
+ * outputs of ev_op_duration_scan): out (B,F,H); frames >= mel_lens[b] are zeros when invariant != 0; adds alpha*pe[f] when
+ * pe != NULL. */
+EV_API int ev_op_gauss_upsample_centers(const float* hs, const float* centers, const int32_t* lens, const int32_t* mel_lens, int B,
+                                        int T, int H, int F, int invariant, const float* pe, const float* alpha, float* out,
+                                        void* stream);
+/* The encoder's first LayerNorm with its embedding prologue, as ev_am_phase1 launches it:
+ * x_out[r] = emb[clamp(ids[r], 0, n_emb - 1)] + alpha[0] * pe[r % L] (product and sum rounded separately),
+ * y[r] = LayerNorm(x_out[r]) * w + b, eps 1e-12.  rows x C. */
+EV_API int ev_op_layernorm_embed(const int64_t* ids, const float* emb, int n_emb, const float* pe, const float* alpha, int L,
+                                 float* x_out, const float* w, const float* b, float* y, int rows, int C, void* stream);
+/* The per-utterance conditioning bias of ev_am_phase1 (model_open_source.py:109-111):
+ * cond_in (B, H + 2*bert) = [spk_emb[clamp(spk[b], 0, n_spk - 1)] | style[b] | content[b]], out (B,H) = cond_in w + bias with
+ * w (H + 2*bert, H) row-major. */
+EV_API int ev_op_cond_bias(const int64_t* spk, const float* spk_emb, int n_spk, const float* style, const float* content, int B, int H,
+                           int bert, const float* w, const float* bias, float* cond_in, float* out, void* stream);
+/* Predictor head (variance.py:46-56): s = x[b,t,:] . w + b[0]; mode 0: out_f[b,t] = s; mode 1: out_i[b,t] =
+ * clamp(rint(exp(s) - 1), 0) (the durations).  Rows t >= lens[b] give 0 (lens may be NULL).  x (B,T,C). */
+EV_API int ev_op_rowdot(const float* x, const float* w, const float* b, const int32_t* lens, int B, int T, int C, int mode,
+                        float* out_f, int64_t* out_i, void* stream);
+/* y = x with rows t >= lens[b] set to zero (variance.py:38-39).  (B,T,C). */
+EV_API int ev_op_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T, int C, void* stream);
+/* x (B,T,C) += Conv1d(1->C, K)(p') + bp + Conv1d(1->C, K)(e') + be (model_open_source.py:131-134), wp / we tap-major (K,C),
+ * p' = pitch * prosody[b,1] + prosody[b,2] and e' = energy * prosody[b,3] + prosody[b,4] (prosody (B,5) or NULL: p' = pitch).
+ * With prosody and lens both given the window ends at lens[b]; otherwise at T. */
+EV_API int ev_op_var_embed_add(float* x, const float* pitch, const float* energy, const float* wp, const float* bp, const float* we,
+                               const float* be, const float* prosody, const int32_t* lens, int B, int T, int C, int K, void* stream);
 
 /* ---- style encoder (the callers' prompt / content embedding: simbert.py:33-72 -> transformers BertModel) ---------------
  * Next-row widening (SURVEY.md s8f rank 1): the reference runs this BERT-base on the CPU twice per utterance
@@ -326,6 +353,13 @@ EV_API size_t ev_style_workspace_bytes(const ev_style_ctx* ctx, int B, int N);
  * heads (B, n_head_out) = the four classification heads side by side, or NULL to skip them. */
 EV_API int ev_style_forward(ev_style_ctx* ctx, const int64_t* ids, const int64_t* type_ids, const int64_t* lens, int B, int N,
                             float* pooled, float* heads, void* workspace, size_t workspace_bytes, void* stream);
+/* The style encoder's two own kernels alone (single-operator tests).  BertEmbeddings: y[r] = LayerNorm((word[ids[r]] +
+ * type[type_ids[r]]) + pos[r % N]) * w + b, eps 1e-12, rows x C; ids must be in range (ev_style_forward does not check them
+ * either).  Row GEMV: out[b,n] = act(x[b*x_stride : +K] . w[:,n] + bias[n]), w (K,N) row-major, act EV_ACT_NONE or EV_ACT_TANH. */
+EV_API int ev_op_bert_embed_ln(const int64_t* ids, const int64_t* type_ids, const float* word, const float* type, const float* pos,
+                               const float* w, const float* b, float* y, int rows, int N, int C, void* stream);
+EV_API int ev_op_row_gemv(const float* x, size_t x_stride, const float* w, const float* bias, float* out, int B, int K, int N, int act,
+                          void* stream);
 
 /* ---- training-mode alignment helpers (SURVEY.md s8f rank 4; not used by any inference path) --------------------------------
  * viterbi_decode (alignment.py:124-142): monotonic alignment search per item on log_p_attn (B, T_mel, T_inp) float32 restricted

@@ -136,44 +136,6 @@ def test_polyphase_transposed_conv(lib, dev, u, k, cin, cout):
     assert rel_max(out.cpu().reshape(B, L * u, cout), ref) <= TOL
 
 
-@pytest.mark.parametrize("rows,C", [(7, 384), (1000, 384), (33, 128), (64, 512)])
-def test_layernorm(lib, dev, rows, C):
-    g = torch.Generator().manual_seed(rows)
-    x = torch.randn(rows, C, generator=g) * 3 + 0.5
-    w, b = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    y = torch.empty(rows, C, device=dev)
-    xd, wd, bd = x.to(dev), w.to(dev), b.to(dev)     # keep the device tensors alive across the call
-    _abi.check(lib.ev_op_layernorm(xd.data_ptr(), wd.data_ptr(), bd.data_ptr(), y.data_ptr(), rows, C, _stream()))
-    torch.cuda.synchronize()
-    assert rel_max(y.cpu(), O.layer_norm(x, w, b)) <= TOL
-
-
-@pytest.mark.parametrize("B,L,masked", [(1, 100, False), (2, 537, False), (3, 150, True), (1, 1, False), (2, 64, True), (1, 2049, False)])
-def test_attention(lib, dev, B, L, masked):
-    """encoder.py:84-109 with and without the key-padding mask (heads 8, d_k 48)."""
-    H, heads, dk = 384, 8, 48
-    g = torch.Generator().manual_seed(L)
-    qkv = torch.randn(B, L, 3 * H, generator=g)
-    lens = torch.randint(1, L + 1, (B,), generator=g, dtype=torch.int32) if masked else None
-    if masked:
-        lens[0] = L
-    q, k, v = [t.reshape(B, L, heads, dk).transpose(1, 2) for t in qkv.split(H, dim=-1)]
-    scores = q @ k.transpose(-2, -1) / math.sqrt(dk)
-    if masked:
-        m = (torch.arange(L)[None, :] >= lens[:, None])[:, None, None, :]
-        scores = scores.masked_fill(m, torch.finfo(torch.float32).min)
-        attn = torch.softmax(scores, -1).masked_fill(m, 0.0)
-    else:
-        attn = torch.softmax(scores, -1)
-    ref = (attn @ v).transpose(1, 2).reshape(B, L, H)
-    out = torch.empty(B, L, H, device=dev)
-    qd = qkv.to(dev)
-    ld = lens.to(dev) if masked else None
-    _abi.check(lib.ev_op_attention(qd.data_ptr(), _ptr(ld), out.data_ptr(), B, L, H, heads, _stream()))
-    torch.cuda.synchronize()
-    assert rel_max(out.cpu(), ref) <= TOL
-
-
 @pytest.mark.parametrize("tc_mode,tol", [(1, 2e-5), (0, 3e-3)], ids=["3xtf32", "tf32"])
 @pytest.mark.parametrize("B,L,masked", [(1, 7, False), (1, 64, False), (1, 129, False), (2, 500, True), (3, 1300, True), (1, 2049, False), (4, 65, True)])
 def test_attention_tc(lib, dev, B, L, masked, tc_mode, tol):
