@@ -1,17 +1,23 @@
-"""Operator cases of the acoustic model's tensor-core kernels, and the child process that runs them on the GPU.
+"""Operator cases of the acoustic model's and the style encoder's tensor-core kernels, and the child process that runs them on
+the GPU.
 
     python tests/am_cases.py <family>
 
-runs one kernel family ("tc": conv1d_tc + splitk_reduce through ev_op_conv1d_tc_ks; "attn": attention_tc) and prints one
-JSON row per case: the plan, the item lengths, the largest per-element error relative to the fp64 bound (am_ref), the bitwise
-cross-checks and whether rows past each item came out as the contract says.  tests/test_am_kernels_gpu.py runs each family once
-in its own process under a timeout and asserts every row.
+runs one kernel family ("tc": the acoustic model's conv1d_tc + splitk_reduce through ev_op_conv1d_tc_ks; "attn": attention_tc;
+"style": the style encoder's GEMMs, the same kernels at its layers) and prints one JSON row per case: the plan, the item
+lengths, the largest per-element error relative to the fp64 bound (am_ref), the bitwise cross-checks and whether rows past each
+item came out as the contract says.  tests/test_am_kernels_gpu.py and tests/test_style_kernels_gpu.py run each family once in
+its own process under a timeout and assert every row.
 
 Inputs hold NaN in every row at or past an item's length: a kernel that read such a row, even to mask it afterwards, would turn
-a valid output into NaN (0 * NaN).  Outputs are prefilled with NaN (with the residual where the engine adds it in place), and
-the split-K scratch with NaN as well.  Valid conv rows must be finite and within the bound; conv rows at or past an item's
-length must be exact zeros (conv1d_tc's epilogue and splitk_reduce_store).  Attention rows below klen must be finite and within
-the bound.
+a valid output into NaN (0 * NaN); residual rows there hold NaN too.  Outputs are prefilled with NaN (with the residual where
+the engine adds it in place), and the split-K scratch with NaN as well.  Valid conv rows must be finite and within the bound;
+conv rows at or past an item's length must be exact zeros (conv1d_tc's epilogue and splitk_reduce_store).  Attention rows below
+klen must be finite and within the bound.
+
+The longest fp32 chain of the style cases: a 3xTF32 ffn2 slice of BERT-base at C_in = 3072 and S = 4 is 768 products, so the
+worst-case fp32 accumulation error is 767 * 2^-24 ~ 2^-14.4 of m, plus ~2^-21 of 3xTF32 operand error: under tau = 2^-14 of
+MODE 1, with little margin in that worst case (typical rounding errors grow like the square root of the chain, far below it).
 """
 import json
 import math
@@ -19,20 +25,27 @@ import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(1, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))      # emotivoice_b200 (the style layer shapes)
 
 import am_plans  # noqa: E402
+import style_plans  # noqa: E402
 import voc_cases  # noqa: E402
 
 H, N_MELS = 384, 80
 ACT_NONE, ACT_RELU, ACT_GELU = am_plans.ACT_NONE, am_plans.ACT_RELU, am_plans.ACT_GELU
-# kind -> (Cin, Cout, K, out_act, in-place residual, per-item bias): the layers of am_plans.am_layers
-KINDS = {"qkv": (H, 3 * H, 1, ACT_NONE, False, False),
-         "wo": (H, H, 1, ACT_NONE, True, False),
-         "ffn1": (H, 4 * H, 3, ACT_GELU, False, False),
-         "ffn2": (4 * H, H, 3, ACT_NONE, True, False),
-         "cond.wx": (H, H, 1, ACT_NONE, False, True),
-         "pred": (H, H, 3, ACT_RELU, False, False),
-         "to_mel": (H, N_MELS, 1, ACT_NONE, False, False)}
+# kind -> (Cin, Cout, K, out_act, residual, per-item bias, input is a GELU output): the layers of am_plans.am_layers.  residual:
+# None, "inplace" (the engine adds it in place: out == res) or "separate" (read from another buffer than the output)
+KINDS = {"qkv": (H, 3 * H, 1, ACT_NONE, None, False, False),
+         "wo": (H, H, 1, ACT_NONE, "inplace", False, False),
+         "ffn1": (H, 4 * H, 3, ACT_GELU, None, False, False),
+         "ffn2": (4 * H, H, 3, ACT_NONE, "inplace", False, False),
+         "cond.wx": (H, H, 1, ACT_NONE, None, True, False),
+         "pred": (H, H, 3, ACT_RELU, None, False, False),
+         "to_mel": (H, N_MELS, 1, ACT_NONE, None, False, False)}
+# every layer an operator case can run: the acoustic model's and the style encoder's of both configurations
+LAYERS = dict(KINDS)
+for _cfg in style_plans.CONFIGS:
+    LAYERS.update(style_plans.layer_table(_cfg))
 PREFIX = [("qkv", am_plans.ENC_SPLITS["qkv"]), ("wo", am_plans.ENC_SPLITS["wo"]), ("ffn1", am_plans.ENC_SPLITS["ffn1"]),
           ("ffn2", am_plans.ENC_SPLITS["ffn2"]), ("cond.wx", am_plans.COND_SPLIT), ("pred", am_plans.PRED_SPLIT)]
 DECODER = [("qkv", am_plans.DEC_SPLITS["qkv"]), ("wo", am_plans.DEC_SPLITS["wo"]), ("ffn1", am_plans.DEC_SPLITS["ffn1"]),
@@ -74,21 +87,53 @@ def _attn_cases():
     return cs
 
 
-FAMILIES = {"tc": _tc_cases, "attn": _attn_cases}
-MODES = {"tc": None, "attn": (1, 0)}
+# The style encoder's GEMMs (style_plans): the four layers of both configurations in MODE 1 ("fp32") and MODE 0 ("tf32"), each at
+# the engine's own S, bias, GELU and residual.  Batch-1 lengths: every N tile width the planner picks at B = 1 and the 128-row
+# edges next to each change (BERT-base: wo and ffn2 take BN = 32 up to 128 tokens, 64 for 129-384 and 128 above; qkv 64 up to
+# 128 tokens and 128 above; ffn1 always 128.  The small model stays at BN = 32 at B = 1 over its 128 positions).  Ragged
+# batches: items on the edges first, then random lengths; they run at BN = 128, except the small model's batch of 8 (wo, ffn2
+# at BN = 64) and of 2 (qkv, ffn1 at BN = 64; wo, ffn2 at 32).
+STYLE_L1 = {"base": (1, 20, 128, 129, 384, 385, 512), "small": (1, 20, 127, 128)}
+STYLE_RAGGED = {"base": ((32, (64, 1, 2, 31, 32, 33, 63)), (8, (512, 1, 127, 128, 129, 255, 256, 257))),
+                "small": ((32, (64, 1, 2, 31, 32, 33, 63)), (8, (128, 1, 127, 2, 63, 64, 65)), (2, (128, 1)))}
+
+
+def style_lens(B, head, seed):
+    """Item lengths of a ragged style case: `head` (the longest first), then random lengths in [1, head[0]]."""
+    import random
+    rnd = random.Random(seed)
+    return list(head) + [rnd.randint(1, head[0]) for _ in range(B - len(head))]
+
+
+def _style_cases():
+    cs = []
+    for cfg in style_plans.CONFIGS:
+        for mode in (1, 0):
+            for kind in style_plans.KINDS:
+                S, k = style_plans.SPLITS[kind], style_plans.kind_name(cfg, kind)
+                for L in STYLE_L1[cfg]:
+                    cs.append(dict(name="%s_%s_S%d_B1_L%d" % (cfg, kind, S, L), kind=k, S=S, mode=mode, B=1, L=L))
+                for B, head in STYLE_RAGGED[cfg]:
+                    cs.append(dict(name="%s_%s_S%d_B%d_L%d" % (cfg, kind, S, B, head[0]), kind=k, S=S, mode=mode, B=B, L=head[0],
+                                   lens=style_lens(B, head, seed=B + head[0]), edges=len(head)))
+    return cs
+
+
+FAMILIES = {"tc": _tc_cases, "attn": _attn_cases, "style": _style_cases}
+MODES = {"tc": None, "attn": (1, 0), "style": None}
 
 
 def case_ids(family):
-    if family == "tc":
-        return ["tc-%s-m%d" % (c["name"], c["mode"]) for c in _tc_cases()]
-    return ["attn-%s-m%d" % (c["name"], m) for c in _attn_cases() for m in MODES["attn"]]
+    if MODES[family] is None:
+        return ["%s-%s-m%d" % (family, c["name"], c["mode"]) for c in FAMILIES[family]()]
+    return ["%s-%s-m%d" % (family, c["name"], m) for c in FAMILIES[family]() for m in MODES[family]]
 
 
-def case_plans(lib):
-    """{(layer kind, plan key)} of every tc case's launch (host-only), for the coverage test."""
+def case_plans(lib, family="tc"):
+    """{(layer kind, plan key)} of every case's launch of a GEMM family ("tc" or "style"; host-only), for the coverage tests."""
     keys = set()
-    for c in _tc_cases():
-        Cin, Cout, K = KINDS[c["kind"]][:3]
+    for c in FAMILIES[family]():
+        Cin, Cout, K = LAYERS[c["kind"]][:3]
         keys.add((c["kind"], am_plans.tc_plan(lib, c["B"], c["L"], Cin, Cout, K, c["mode"], c["S"])["key"]))
     return keys
 
@@ -141,15 +186,17 @@ def run_tc(R, c, seed):
     import am_ref
     lib, dev = R.lib, R.dev
     B, L, mode, S = c["B"], c["L"], c["mode"], c["S"]
-    Cin, Cout, K, oact, inplace, per_item = KINDS[c["kind"]]
+    Cin, Cout, K, oact, res_kind, per_item, gelu_in = LAYERS[c["kind"]]
+    inplace = res_kind == "inplace"
     pl = am_plans.tc_plan(lib, B, L, Cin, Cout, K, mode, S)
-    valid = ragged_lens(L, B, seed) if B > 1 else [L]
-    row = dict(plan=list(pl["key"]), B=B, L=L, lens=valid)
+    valid = c.get("lens") or (ragged_lens(L, B, seed) if B > 1 else [L])
+    row = dict(kind=c["kind"], plan=list(pl["key"]), B=B, L=L, lens=valid)
     g = torch.Generator().manual_seed(seed)
-    x = _nan_past(torch.randn(B, L, Cin, generator=g), valid)
+    x = torch.randn(B, L, Cin, generator=g)          # LayerNorm-like rows; a GELU output where the layer reads one
+    x = _nan_past(torch.nn.functional.gelu(x) if gelu_in else x, valid)
     w = torch.randn(K, Cin, Cout, generator=g) / math.sqrt(Cin * K)
     bias = torch.randn(B if per_item else 1, Cout, generator=g)
-    res = _nan_past(torch.randn(B, L, Cout, generator=g), valid) if inplace else None
+    res = _nan_past(torch.randn(B, L, Cout, generator=g), valid) if res_kind else None
     xd, wd, bd = x.to(dev), voc_cases._pack(mode)(w).to(dev), bias.to(dev)
     lens_d = torch.tensor(valid, dtype=torch.int32, device=dev) if B > 1 else None
     bias_bs = Cout if per_item else 0
@@ -194,16 +241,17 @@ def run_tc(R, c, seed):
         # an item of the ragged batch == its own batch-1 launch (another BN and other rings, the same KBG and slices)
         same = True
         for b, n in enumerate(valid):
-            if n not in EDGE_LENS + (L,) or valid.index(n) != b:
+            if b >= c["edges"] if "edges" in c else (n not in EDGE_LENS + (L,) or valid.index(n) != b):
                 continue
             x1 = xd[b:b + 1, :n].contiguous()
             o1 = res[b:b + 1, :n].contiguous().to(dev) if inplace else torch.full((1, n, Cout), float("nan"), device=dev)
+            r1 = o1 if inplace else (res[b:b + 1, :n].contiguous().to(dev) if res_kind else None)
             if per_item:
                 b1 = bd[b:b + 1].contiguous()
-            R.keep += [x1, o1]
+            R.keep += [x1, o1, r1]
             ws = torch.full((pl["S"] * n * Cout,), float("nan"), device=dev) if S > 1 else None
             R.keep.append(ws)
-            rc1 = lib.ev_op_conv1d_tc_ks(R.ptr(x1), R.ptr(wd), mode, R.ptr(b1 if per_item else bd), bias_bs, R.ptr(o1) if inplace else None,
+            rc1 = lib.ev_op_conv1d_tc_ks(R.ptr(x1), R.ptr(wd), mode, R.ptr(b1 if per_item else bd), bias_bs, R.ptr(r1),
                                          R.ptr(o1), 1, n, Cin, Cout, K, 1, None, 1, 0, 0.0, oact, 0, 1.0, S, R.ptr(ws),
                                          0 if ws is None else ws.numel(), R.st)
             torch.cuda.synchronize()
@@ -267,9 +315,9 @@ def main(family):
     lib = voc_cases._setup()
     import torch
     R = voc_cases.Runner(lib)
-    if family == "tc":
-        for i, c in enumerate(_tc_cases()):
-            cid = "tc-%s-m%d" % (c["name"], c["mode"])
+    if family in ("tc", "style"):
+        for i, c in enumerate(FAMILIES[family]()):
+            cid = "%s-%s-m%d" % (family, c["name"], c["mode"])
             try:
                 row = run_tc(R, c, 1000 * i + 7)
             except Exception as e:      # a Python-side error in one case must not hide the others' rows

@@ -33,7 +33,7 @@ from conftest import ROOT
 
 pytestmark = pytest.mark.gpu
 
-TIMEOUT = {"tc": 1200, "attn": 600}
+TIMEOUT = {"tc": 1200, "attn": 600, "style": 1200}
 _ROWS = {}
 
 
