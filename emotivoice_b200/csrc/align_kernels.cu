@@ -16,6 +16,7 @@ __global__ void __launch_bounds__(256) mas_kernel(const float* __restrict__ log_
                                                   const int64_t* __restrict__ feats_lens, int T_mel, int T_inp,
                                                   int32_t* __restrict__ path, float* __restrict__ durations,
                                                   float* __restrict__ bin_loss, uint8_t* __restrict__ dec_ws) {
+  pdl_entry();
   extern __shared__ __align__(16) unsigned char mas_smem[];
   double* q0 = reinterpret_cast<double*>(mas_smem);
   double* q1 = q0 + T_inp;
@@ -81,9 +82,7 @@ int launch_mas(const float* log_p, const int64_t* text_lens, const int64_t* feat
   EV_CHECK_ARG(smem <= 200 * 1024, "mas: %d tokens exceed the shared-memory budget", T_inp);
   static std::atomic<uint64_t> attr_devs{0};
   if (first_use_on_device(attr_devs)) cudaFuncSetAttribute(mas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  mas_kernel<<<B, 256, smem, st>>>(log_p, text_lens, feats_lens, T_mel, T_inp, path, durations, bin_loss, dec_ws);
-  EV_CUDA_LAUNCH_CHECK("mas_kernel");
-  return EV_OK;
+  return launch("mas_kernel", mas_kernel, B, 256, smem, st, log_p, text_lens, feats_lens, T_mel, T_inp, path, durations, bin_loss, dec_ws);
 }
 
 // out[b, n] = mean(xs[b, start_n : start_n + d_n]) (0 when d_n == 0), start = exclusive cumsum of the durations; tokens past
@@ -91,6 +90,7 @@ int launch_mas(const float* log_p, const int64_t* text_lens, const int64_t* feat
 __global__ void __launch_bounds__(256) avg_by_duration_kernel(const float* __restrict__ durations, const float* __restrict__ xs,
                                                               const int64_t* __restrict__ text_lens, const int64_t* __restrict__ feats_lens,
                                                               int T_mel, int T_inp, float* __restrict__ out) {
+  pdl_entry();
   extern __shared__ int abd_start[];     // T_inp + 1
   const int b = blockIdx.x, tid = threadIdx.x;
   const int T = (int)min((long long)T_inp, max(0ll, (long long)text_lens[b]));
@@ -123,9 +123,7 @@ int launch_avg_by_duration(const float* durations, const float* xs, const int64_
   EV_CHECK_ARG(B > 0 && T_mel > 0 && T_inp > 0, "average_by_duration: B=%d T_mel=%d T_inp=%d", B, T_mel, T_inp);
   const size_t smem = (size_t)(T_inp + 1) * sizeof(int);
   EV_CHECK_ARG(smem <= 48 * 1024, "average_by_duration: %d tokens exceed the shared-memory budget", T_inp);
-  avg_by_duration_kernel<<<B, 256, smem, st>>>(durations, xs, text_lens, feats_lens, T_mel, T_inp, out);
-  EV_CUDA_LAUNCH_CHECK("avg_by_duration_kernel");
-  return EV_OK;
+  return launch("avg_by_duration_kernel", avg_by_duration_kernel, B, 256, smem, st, durations, xs, text_lens, feats_lens, T_mel, T_inp, out);
 }
 
 
@@ -140,6 +138,7 @@ template <int NC>
 __global__ void __launch_bounds__(128) align_logp_kernel(const float* __restrict__ text, const float* __restrict__ feats,
                                                          const int64_t* __restrict__ text_lens, const float* __restrict__ prior, int F, int T,
                                                          float* __restrict__ out) {
+  pdl_entry();
   constexpr int A = NC * 128;
   extern __shared__ float alp_sc[];            // [4 warps][T]
   const int b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -186,20 +185,20 @@ int launch_align_logp(const float* text, const float* feats, const int64_t* text
   EV_CHECK_ARG(A % 128 == 0 && A <= 512, "align_logp: feature width %d must be a multiple of 128, <= 512", A);
   dim3 grid((F + 3) / 4, B);
   const size_t smem = (size_t)4 * T * sizeof(float);
+  auto k = align_logp_kernel<4>;
   switch (A / 128) {
-    case 1: align_logp_kernel<1><<<grid, 128, smem, st>>>(text, feats, text_lens, prior, F, T, out); break;
-    case 2: align_logp_kernel<2><<<grid, 128, smem, st>>>(text, feats, text_lens, prior, F, T, out); break;
-    case 3: align_logp_kernel<3><<<grid, 128, smem, st>>>(text, feats, text_lens, prior, F, T, out); break;
-    default: align_logp_kernel<4><<<grid, 128, smem, st>>>(text, feats, text_lens, prior, F, T, out); break;
+    case 1: k = align_logp_kernel<1>; break;
+    case 2: k = align_logp_kernel<2>; break;
+    case 3: k = align_logp_kernel<3>; break;
   }
-  EV_CUDA_LAUNCH_CHECK("align_logp_kernel");
-  return EV_OK;
+  return launch("align_logp_kernel", k, grid, 128, smem, st, text, feats, text_lens, prior, F, T, out);
 }
 
 // get_segments (models/hifigan/get_random_segments.py:19-27): out[b, c, i] = x[b, c, start[b] + i] while start[b] + i < T, else 0.
 // x is (B, C, T) channels-first like the reference's z = dec_outputs.transpose(1, 2) (jets.py:55-60).
 __global__ void __launch_bounds__(256) segments_kernel(const float* __restrict__ x, const int64_t* __restrict__ start, int C, int T, int seg,
                                                        float* __restrict__ out, size_t n) {
+  pdl_entry();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int k = (int)(i % seg);
@@ -212,9 +211,7 @@ __global__ void __launch_bounds__(256) segments_kernel(const float* __restrict__
 int launch_segments(const float* x, const int64_t* start, int B, int C, int T, int seg, float* out, cudaStream_t st) {
   EV_CHECK_ARG(B > 0 && C > 0 && T > 0 && seg > 0, "get_segments: B=%d C=%d T=%d segment=%d", B, C, T, seg);
   const size_t n = (size_t)B * C * seg;
-  segments_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, start, C, T, seg, out, n);
-  EV_CUDA_LAUNCH_CHECK("segments_kernel");
-  return EV_OK;
+  return launch("segments_kernel", segments_kernel, (unsigned)((n + 255) / 256), 256, 0, st, x, start, C, T, seg, out, n);
 }
 
 }  // namespace ev

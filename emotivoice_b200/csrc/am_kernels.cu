@@ -22,13 +22,13 @@ __device__ __forceinline__ float warp_max(float v) {
 // layer of the encoder: x = word_emb[id] + alpha * pe[t]  (model_open_source.py:107,
 // encoder.py:257-261), which is also written back as the residual stream.
 // ---------------------------------------------------------------------------------------------
-template <int NV, bool PDL>  // float4 per lane
+template <int NV>  // float4 per lane
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, const int64_t* __restrict__ ids,
                                                         const float* __restrict__ emb, const float* __restrict__ pe,
                                                         const float* __restrict__ alpha, float* __restrict__ x_out,
                                                         const float* __restrict__ w, const float* __restrict__ b,
                                                         float* __restrict__ y, int rows, int L, int n_emb) {
-  pdl_entry<PDL>();
+  pdl_entry();
   constexpr int C = NV * 128;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -88,16 +88,15 @@ int launch_layernorm(const float* x, const int64_t* ids, const float* emb, const
   EV_CHECK_ARG(C % 128 == 0 && C <= 768, "layernorm: C=%d must be a multiple of 128 and <= 768", C);
   const int wpb = 8;
   dim3 grid((rows + wpb - 1) / wpb);
+  auto k = layernorm_kernel<6>;
   switch (C / 128) {
-    case 1: launch_k(layernorm_kernel<1, true>, layernorm_kernel<1, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
-    case 2: launch_k(layernorm_kernel<2, true>, layernorm_kernel<2, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
-    case 3: launch_k(layernorm_kernel<3, true>, layernorm_kernel<3, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
-    case 4: launch_k(layernorm_kernel<4, true>, layernorm_kernel<4, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
-    case 5: launch_k(layernorm_kernel<5, true>, layernorm_kernel<5, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
-    default: launch_k(layernorm_kernel<6, true>, layernorm_kernel<6, false>, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb); break;
+    case 1: k = layernorm_kernel<1>; break;
+    case 2: k = layernorm_kernel<2>; break;
+    case 3: k = layernorm_kernel<3>; break;
+    case 4: k = layernorm_kernel<4>; break;
+    case 5: k = layernorm_kernel<5>; break;
   }
-  EV_CUDA_LAUNCH_CHECK("layernorm_kernel");
-  return EV_OK;
+  return launch("layernorm_kernel", k, grid, 256, 0, st, x, ids, emb, pe, alpha, x_out, w, b, y, rows, L, n_emb);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -108,10 +107,10 @@ int launch_layernorm(const float* x, const int64_t* ids, const float* emb, const
 // [h*DK, (h+1)*DK) of each third (encoder.py:72-82).  Query rows >= key_len are computed like
 // the reference computes them (they attend to the valid keys).
 // ---------------------------------------------------------------------------------------------
-template <int DK, int BQ, bool PDL>
+template <int DK, int BQ>
 __global__ void __launch_bounds__(128) attention_kernel(const float* __restrict__ qkv, const int32_t* __restrict__ key_lens,
                                                         float* __restrict__ ctx, int L, int H) {
-  pdl_entry<PDL>();
+  pdl_entry();
   constexpr int BK = 64, LDQ = BQ + 1, LDT = BK + 1;
   constexpr int RQ = BQ / 16;   // query rows per thread
   constexpr int OC = DK / 8;    // output columns per thread
@@ -243,14 +242,10 @@ static int launch_attention_dk(const float* qkv, const int32_t* key_lens, float*
                                cudaStream_t st) {
   const size_t smem = (size_t)(DK * (BQ + 1) + DK * 65 + 64 * DK + BQ * 65) * sizeof(float);
   static std::atomic<uint64_t> attr_devs{0};
-  if (first_use_on_device(attr_devs)) {
-    cudaFuncSetAttribute(attention_kernel<DK, BQ, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(attention_kernel<DK, BQ, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  }
+  if (first_use_on_device(attr_devs))
+    cudaFuncSetAttribute(attention_kernel<DK, BQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((L + BQ - 1) / BQ, heads, B);
-  launch_k(attention_kernel<DK, BQ, true>, attention_kernel<DK, BQ, false>, grid, 128, smem, st, qkv, key_lens, ctx, L, H);
-  EV_CUDA_LAUNCH_CHECK("attention_kernel");
-  return EV_OK;
+  return launch("attention_kernel", attention_kernel<DK, BQ>, grid, 128, smem, st, qkv, key_lens, ctx, L, H);
 }
 
 int launch_attention(const float* qkv, const int32_t* key_lens, float* ctx, int B, int L, int H, int heads,
@@ -275,11 +270,10 @@ int launch_attention(const float* qkv, const int32_t* key_lens, float* ctx, int 
 // The 2304->384 projection (:111) is split: W_x x_t + (W_c c_b + bias); the second term is a
 // per-utterance bias computed once per item by the generic GEMM on this gathered vector.
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void cond_gather_kernel(const int64_t* __restrict__ spk, const float* __restrict__ spk_emb,
                                    const float* __restrict__ style, const float* __restrict__ content,
                                    float* __restrict__ out, int H, int bert, int n_spk) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const int b = blockIdx.x;
   const int W = H + 2 * bert;
   const long long sid_raw = spk[b];      // range errors are reported by validate_inputs_kernel; clamp keeps the read in bounds
@@ -294,9 +288,7 @@ __global__ void cond_gather_kernel(const int64_t* __restrict__ spk, const float*
 }
 int launch_cond_gather(const int64_t* spk, const float* spk_emb, const float* style, const float* content,
                        float* out, int B, int H, int bert, int n_spk, cudaStream_t st) {
-  launch_k(cond_gather_kernel<true>, cond_gather_kernel<false>, B, 256, 0, st, spk, spk_emb, style, content, out, H, bert, n_spk);
-  EV_CUDA_LAUNCH_CHECK("cond_gather_kernel");
-  return EV_OK;
+  return launch("cond_gather_kernel", cond_gather_kernel, B, 256, 0, st, spk, spk_emb, style, content, out, H, bert, n_spk);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -305,11 +297,10 @@ int launch_cond_gather(const int64_t* spk, const float* spk_emb, const float* st
 // per (8 output columns, batch item); the K axis is split over the CTA's threads and reduced in a
 // fixed order (deterministic).  w is (K, N) row-major.
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void __launch_bounds__(256) cond_gemv_kernel(const float* __restrict__ c, const float* __restrict__ w,
                                                         const float* __restrict__ bias, float* __restrict__ out, int K,
                                                         int N) {
-  pdl_entry<PDL>();
+  pdl_entry();
   __shared__ float red[8][8][33];
   const int b = blockIdx.y, n0 = blockIdx.x * 8;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -340,21 +331,18 @@ __global__ void __launch_bounds__(256) cond_gemv_kernel(const float* __restrict_
 int launch_cond_gemv(const float* c, const float* w, const float* bias, float* out, int B, int K, int N, cudaStream_t st) {
   EV_CHECK_ARG(N % 8 == 0 && B > 0 && B <= 65535, "cond_gemv: N=%d B=%d", N, B);
   dim3 grid(N / 8, B);
-  launch_k(cond_gemv_kernel<true>, cond_gemv_kernel<false>, grid, 256, 0, st, c, w, bias, out, K, N);
-  EV_CUDA_LAUNCH_CHECK("cond_gemv_kernel");
-  return EV_OK;
+  return launch("cond_gemv_kernel", cond_gemv_kernel, grid, 256, 0, st, c, w, bias, out, K, N);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Predictor head: Linear(C -> 1) + output mask (variance.py:46-56, :119-124).
 // mode 0: float (pitch / energy);  mode 1: duration = clamp(rint(exp(y) - 1), 0) as int64.
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void __launch_bounds__(256) rowdot_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                      const float* __restrict__ bias, const int32_t* __restrict__ lens,
                                                      int rows, int T, int C, int mode, float* __restrict__ out_f,
                                                      int64_t* __restrict__ out_i) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -380,9 +368,7 @@ int launch_rowdot(const float* x, const float* w, const float* b, const int32_t*
                   int mode, float* out_f, int64_t* out_i, cudaStream_t st) {
   EV_CHECK_ARG(C % 4 == 0, "rowdot: C=%d", C);
   const int rows = B * T;
-  launch_k(rowdot_kernel<true>, rowdot_kernel<false>, (rows + 7) / 8, 256, 0, st, x, w, b, lens, rows, T, C, mode, out_f, out_i);
-  EV_CUDA_LAUNCH_CHECK("rowdot_kernel");
-  return EV_OK;
+  return launch("rowdot_kernel", rowdot_kernel, (rows + 7) / 8, 256, 0, st, x, w, b, lens, rows, T, C, mode, out_f, out_i);
 }
 
 // Input validation + length conversion, ONE CTA (B*T is a few thousand elements at most).  The reference raises
@@ -391,11 +377,10 @@ int launch_rowdot(const float* x, const float* w, const float* b, const int32_t*
 // the path's single sync (no extra round trip), and every consumer clamps so nothing is read out of bounds meanwhile.
 // status bits: 1 = token id outside [0, n_vocab), 2 = speaker id outside [0, n_speaker), 4 = length outside [1, T].
 // lens arrive as int64 (inference_am_vocoder_joint.py:114); the kernels take int32 clamped to [0, T].
-template <bool PDL>
 __global__ void __launch_bounds__(1024) validate_inputs_kernel(const int64_t* __restrict__ ling, const int64_t* __restrict__ lens,
                                                                const int64_t* __restrict__ spk, int32_t* __restrict__ lens_out,
                                                                int32_t* __restrict__ status, int B, int T, int n_vocab, int n_spk) {
-  pdl_entry<PDL>();
+  pdl_entry();
   __shared__ int s_flags;
   if (threadIdx.x == 0) s_flags = 0;
   __syncthreads();
@@ -418,16 +403,13 @@ __global__ void __launch_bounds__(1024) validate_inputs_kernel(const int64_t* __
 }
 int launch_validate_inputs(const int64_t* ling, const int64_t* lens, const int64_t* spk, int32_t* lens_out, int32_t* status, int B,
                            int T, int n_vocab, int n_spk, cudaStream_t st) {
-  launch_k(validate_inputs_kernel<true>, validate_inputs_kernel<false>, 1, 1024, 0, st, ling, lens, spk, lens_out, status, B, T, n_vocab, n_spk);
-  EV_CUDA_LAUNCH_CHECK("validate_inputs_kernel");
-  return EV_OK;
+  return launch("validate_inputs_kernel", validate_inputs_kernel, 1, 1024, 0, st, ling, lens, spk, lens_out, status, B, T, n_vocab, n_spk);
 }
 
 // masked_fill(x_masks, 0) on the predictors' input (variance.py:38-39, :109-110)
-template <bool PDL>
 __global__ void mask_rows_kernel(const float4* __restrict__ x, const int32_t* __restrict__ lens, float4* __restrict__ y,
                                  int T, int C4, size_t n4) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
   const size_t row = i / C4;
@@ -437,9 +419,7 @@ __global__ void mask_rows_kernel(const float4* __restrict__ x, const int32_t* __
 int launch_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T, int C, cudaStream_t st) {
   EV_CHECK_ARG(C % 4 == 0, "mask_rows: C=%d", C);
   const size_t n4 = (size_t)B * T * C / 4;
-  launch_k(mask_rows_kernel<true>, mask_rows_kernel<false>, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float4*)x, lens, (float4*)y, T, C / 4, n4);
-  EV_CUDA_LAUNCH_CHECK("mask_rows_kernel");
-  return EV_OK;
+  return launch("mask_rows_kernel", mask_rows_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float4*)x, lens, (float4*)y, T, C / 4, n4);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -450,13 +430,12 @@ int launch_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T
 // prosody and lens (batch-invariant contract) the window ends at lens[b] like the item's own B=1 call,
 // where the conv's zero padding follows the last token; the shifted pads would otherwise leak in.
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void var_embed_add_kernel(float* __restrict__ x, const float* __restrict__ pitch,
                                      const float* __restrict__ energy, const float* __restrict__ wp,
                                      const float* __restrict__ bp, const float* __restrict__ we,
                                      const float* __restrict__ be, const float* __restrict__ prosody,
                                      const int32_t* __restrict__ lens, int T, int C, int K) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const int row = blockIdx.x;   // b*T + t
   const int b = row / T, t = row % T;
   __shared__ float ps[16], es[16];
@@ -489,10 +468,7 @@ int launch_var_embed_add(float* x, const float* pitch, const float* energy, cons
                          const float* we, const float* be, const float* prosody, const int32_t* lens, int B, int T, int C,
                          int K, cudaStream_t st) {
   EV_CHECK_ARG(K <= 16, "var_embed: K=%d > 16", K);
-  launch_k(var_embed_add_kernel<true>, var_embed_add_kernel<false>, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, prosody,
-           lens, T, C, K);
-  EV_CUDA_LAUNCH_CHECK("var_embed_add_kernel");
-  return EV_OK;
+  return launch("var_embed_add_kernel", var_embed_add_kernel, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, prosody, lens, T, C, K);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -509,14 +485,13 @@ int launch_var_embed_add(float* x, const float* pitch, const float* energy, cons
 // batch-invariant contract (its own B=1 call fails in the decoder), or the whole batch otherwise.
 // One CTA (B*T is tiny).
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __restrict__ dur,
                                                              const int32_t* __restrict__ lens,
                                                              const float* __restrict__ alpha, int alpha_stride,
                                                              int invariant, int B, int T, float* __restrict__ centers,
                                                              float* __restrict__ ds_f, int32_t* __restrict__ mel_lens,
                                                              int32_t* __restrict__ status) {
-  pdl_entry<PDL>();
+  pdl_entry();
   __shared__ unsigned long long s_total;
   __shared__ int s_max, s_min;
   const int tid = threadIdx.x, nw = blockDim.x >> 5, lane = tid & 31, wid = tid >> 5;
@@ -574,10 +549,8 @@ __global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __re
 }
 int launch_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int alpha_stride, int invariant, int B,
                          int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, cudaStream_t st) {
-  launch_k(duration_scan_kernel<true>, duration_scan_kernel<false>, 1, 1024, 0, st, dur, lens, alpha, alpha_stride, invariant, B, T,
-           centers, ds_f, mel_lens, status);
-  EV_CUDA_LAUNCH_CHECK("duration_scan_kernel");
-  return EV_OK;
+  return launch("duration_scan_kernel", duration_scan_kernel, 1, 1024, 0, st, dur, lens, alpha, alpha_stride, invariant, B, T,
+                centers, ds_f, mel_lens, status);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -592,13 +565,13 @@ int launch_duration_scan(const int64_t* dur, const int32_t* lens, const float* a
 constexpr int GU_TT = 16;   // tokens per smem chunk
 // GU_FT frames per CTA (16, or 8 when the launch would otherwise leave most SMs idle: batch 1; the per-output token order, hence every
 // bit, does not depend on it)
-template <int NC, int GU_FT, bool PDL>           // channels per thread: H = NC * 128
+template <int NC, int GU_FT>           // channels per thread: H = NC * 128
 __global__ void __launch_bounds__(128) gauss_upsample_kernel(const float* __restrict__ hs, const float* __restrict__ centers,
                                                              const int32_t* __restrict__ lens,
                                                              const int32_t* __restrict__ mel_lens, int T, int F,
                                                              int invariant, const float* __restrict__ pe,
                                                              const float* __restrict__ alpha, float* __restrict__ out) {
-  pdl_entry<PDL>();
+  pdl_entry();
   constexpr int H = NC * 128;
   __shared__ float s_w[GU_FT][GU_TT];
   __shared__ float s_max[GU_FT], s_inv[GU_FT];
@@ -700,18 +673,13 @@ int launch_gauss_upsample(const float* hs, const float* centers, const int32_t* 
   const bool small = (long long)B * ((F + 15) / 16) < 2 * sm_count();
   const int ft = small ? 8 : 16;
   dim3 grid((F + ft - 1) / ft, B);
-#define EV_GU(NC)                                                                                                                              \
-  if (small) launch_k(gauss_upsample_kernel<NC, 8, true>, gauss_upsample_kernel<NC, 8, false>, grid, 128, 0, st, hs, centers, lens, mel_lens, T, F, invariant, pe, alpha, out); \
-  else launch_k(gauss_upsample_kernel<NC, 16, true>, gauss_upsample_kernel<NC, 16, false>, grid, 128, 0, st, hs, centers, lens, mel_lens, T, F, invariant, pe, alpha, out);
+  auto k = small ? gauss_upsample_kernel<4, 8> : gauss_upsample_kernel<4, 16>;
   switch (H / 128) {
-    case 1: EV_GU(1) break;
-    case 2: EV_GU(2) break;
-    case 3: EV_GU(3) break;
-    default: EV_GU(4) break;
+    case 1: k = small ? gauss_upsample_kernel<1, 8> : gauss_upsample_kernel<1, 16>; break;
+    case 2: k = small ? gauss_upsample_kernel<2, 8> : gauss_upsample_kernel<2, 16>; break;
+    case 3: k = small ? gauss_upsample_kernel<3, 8> : gauss_upsample_kernel<3, 16>; break;
   }
-#undef EV_GU
-  EV_CUDA_LAUNCH_CHECK("gauss_upsample_kernel");
-  return EV_OK;
+  return launch("gauss_upsample_kernel", k, grid, 128, 0, st, hs, centers, lens, mel_lens, T, F, invariant, pe, alpha, out);
 }
 
 }  // namespace ev

@@ -297,15 +297,7 @@ static int launch_atc(const float* qkv, const int32_t* key_lens, float* ctx, int
   if (first_use_on_device(attr_devs))
     cudaFuncSetAttribute(atc::attention_tc_kernel<DK, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   dim3 grid((L + atc::BQ - 1) / atc::BQ, heads, B);
-  if (pdl_mode() >= 2) {
-    const cudaError_t e = launch_with_pdl(atc::attention_tc_kernel<DK, MODE>, grid, dim3(atc::ATC_THREADS), (size_t)smem, st, qkv, key_lens, ctx, L, H);
-    if (e != cudaSuccess) { set_error("attention_tc_kernel (PDL launch): %s", cudaGetErrorString(e)); return EV_ECUDA; }
-    count_launch();
-    return EV_OK;
-  }
-  atc::attention_tc_kernel<DK, MODE><<<grid, atc::ATC_THREADS, smem, st>>>(qkv, key_lens, ctx, L, H);
-  EV_CUDA_LAUNCH_CHECK("attention_tc_kernel");
-  return EV_OK;
+  return launch("attention_tc_kernel", atc::attention_tc_kernel<DK, MODE>, grid, atc::ATC_THREADS, (size_t)smem, st, qkv, key_lens, ctx, L, H);
 }
 
 void preload_attention_tc() {      // see preload_conv1d_gp

@@ -724,15 +724,7 @@ static int launch_gp_variant(const GpConvParams& p, const gp::GPlan& pl, const G
     cudaFuncSetAttribute(gp::conv1d_gp_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  if (pdl_mode()) {
-    const cudaError_t e = launch_with_pdl(gp::conv1d_gp_kernel<MODE, MT, KBG>, dim3((unsigned)grid), dim3(gp::GP_THREADS), (size_t)pl.smem_total, st, p, pl, gs);
-    if (e != cudaSuccess) { set_error("conv1d_gp_kernel (PDL launch): %s", cudaGetErrorString(e)); return EV_ECUDA; }
-    count_launch();
-    return EV_OK;
-  }
-  gp::conv1d_gp_kernel<MODE, MT, KBG><<<grid, gp::GP_THREADS, pl.smem_total, st>>>(p, pl, gs);
-  EV_CUDA_LAUNCH_CHECK("conv1d_gp_kernel");
-  return EV_OK;
+  return launch("conv1d_gp_kernel", gp::conv1d_gp_kernel<MODE, MT, KBG>, (unsigned)grid, gp::GP_THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 template <int MODE, int KBG>
@@ -848,18 +840,7 @@ int launch_to_gp(const float* in, long long sb, long long st_, long long sc, voi
   EV_CHECK_ARG(B > 0 && L > 0 && C % (bf16 ? 8 : 4) == 0, "to_gp: B=%d L=%d C=%d", B, L, C);
   const size_t n = (size_t)B * (C / (bf16 ? 8 : 4)) * L;
   const unsigned grid = (unsigned)((n + 255) / 256);
-  cudaError_t e = cudaSuccess;
-  if (pdl_mode()) {
-    e = bf16 ? launch_with_pdl(gp::to_gp_kernel<true>, dim3(grid), dim3(256), 0, st, in, sb, st_, sc, out, B, L, C)
-             : launch_with_pdl(gp::to_gp_kernel<false>, dim3(grid), dim3(256), 0, st, in, sb, st_, sc, out, B, L, C);
-  } else if (bf16) {
-    gp::to_gp_kernel<true><<<grid, 256, 0, st>>>(in, sb, st_, sc, out, B, L, C);
-  } else {
-    gp::to_gp_kernel<false><<<grid, 256, 0, st>>>(in, sb, st_, sc, out, B, L, C);
-  }
-  park_launch_error(e);
-  EV_CUDA_LAUNCH_CHECK("to_gp_kernel");
-  return EV_OK;
+  return launch("to_gp_kernel", bf16 ? gp::to_gp_kernel<true> : gp::to_gp_kernel<false>, grid, 256, 0, st, in, sb, st_, sc, out, B, L, C);
 }
 
 int launch_gp_sum_div(const float* a, const float* b, const float* c, float* out, size_t n_floats, float div, cudaStream_t st) {
@@ -868,18 +849,7 @@ int launch_gp_sum_div(const float* a, const float* b, const float* c, float* out
   const unsigned grid = (unsigned)((n4 + 255) / 256);
   const float4 *a4 = reinterpret_cast<const float4*>(a), *b4 = reinterpret_cast<const float4*>(b), *c4 = reinterpret_cast<const float4*>(c);
   float4* o4 = reinterpret_cast<float4*>(out);
-  cudaError_t e = cudaSuccess;
-  if (pdl_mode()) {
-    e = c ? launch_with_pdl(gp::gp_sum_div_kernel<3>, dim3(grid), dim3(256), 0, st, a4, b4, c4, o4, n4, div)
-          : launch_with_pdl(gp::gp_sum_div_kernel<2>, dim3(grid), dim3(256), 0, st, a4, b4, c4, o4, n4, div);
-  } else if (c) {
-    gp::gp_sum_div_kernel<3><<<grid, 256, 0, st>>>(a4, b4, c4, o4, n4, div);
-  } else {
-    gp::gp_sum_div_kernel<2><<<grid, 256, 0, st>>>(a4, b4, c4, o4, n4, div);
-  }
-  park_launch_error(e);
-  EV_CUDA_LAUNCH_CHECK("gp_sum_div_kernel");
-  return EV_OK;
+  return launch("gp_sum_div_kernel", c ? gp::gp_sum_div_kernel<3> : gp::gp_sum_div_kernel<2>, grid, 256, 0, st, a4, b4, c4, o4, n4, div);
 }
 
 int launch_conv_post_gp(const void* x, int bf16, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B, int L, int C, int K,
@@ -898,32 +868,12 @@ int launch_conv_post_gp(const void* x, int bf16, const float* w, const float* bi
     constexpr int RS = gp::GP4_ROWS + 8;
     const size_t smem4 = (size_t)C * (RS + 8) * sizeof(float);
     dim3 grid4((L + gp::GP4_ROWS - 1) / gp::GP4_ROWS, B);
-    cudaError_t e4 = cudaSuccess;
-    if (pdl_mode()) {
-      e4 = bf16 ? launch_with_pdl(gp::conv_post_gp4_kernel<true, 7>, grid4, dim3(gp::GP4_T), smem4, st, x, w, bias, lens, lens_mul, L, C, slope, wav)
-                : launch_with_pdl(gp::conv_post_gp4_kernel<false, 7>, grid4, dim3(gp::GP4_T), smem4, st, x, w, bias, lens, lens_mul, L, C, slope, wav);
-    } else if (bf16) {
-      gp::conv_post_gp4_kernel<true, 7><<<grid4, gp::GP4_T, smem4, st>>>(x, w, bias, lens, lens_mul, L, C, slope, wav);
-    } else {
-      gp::conv_post_gp4_kernel<false, 7><<<grid4, gp::GP4_T, smem4, st>>>(x, w, bias, lens, lens_mul, L, C, slope, wav);
-    }
-    park_launch_error(e4);
-    EV_CUDA_LAUNCH_CHECK("conv_post_gp4_kernel");
-    return EV_OK;
+    return launch("conv_post_gp4_kernel", bf16 ? gp::conv_post_gp4_kernel<true, 7> : gp::conv_post_gp4_kernel<false, 7>, grid4, gp::GP4_T, smem4,
+                  st, x, w, bias, lens, lens_mul, L, C, slope, wav);
   }
   dim3 grid((L + gp::GPP_BT - 1) / gp::GPP_BT, B);
-  cudaError_t e = cudaSuccess;
-  if (pdl_mode()) {
-    e = bf16 ? launch_with_pdl(gp::conv_post_gp_kernel<true>, grid, dim3(gp::GPP_BT), smem, st, x, w, bias, lens, lens_mul, L, C, K, slope, wav)
-             : launch_with_pdl(gp::conv_post_gp_kernel<false>, grid, dim3(gp::GPP_BT), smem, st, x, w, bias, lens, lens_mul, L, C, K, slope, wav);
-  } else if (bf16) {
-    gp::conv_post_gp_kernel<true><<<grid, gp::GPP_BT, smem, st>>>(x, w, bias, lens, lens_mul, L, C, K, slope, wav);
-  } else {
-    gp::conv_post_gp_kernel<false><<<grid, gp::GPP_BT, smem, st>>>(x, w, bias, lens, lens_mul, L, C, K, slope, wav);
-  }
-  park_launch_error(e);
-  EV_CUDA_LAUNCH_CHECK("conv_post_gp_kernel");
-  return EV_OK;
+  return launch("conv_post_gp_kernel", bf16 ? gp::conv_post_gp_kernel<true> : gp::conv_post_gp_kernel<false>, grid, gp::GPP_BT, smem, st, x, w,
+                bias, lens, lens_mul, L, C, K, slope, wav);
 }
 
 }  // namespace ev

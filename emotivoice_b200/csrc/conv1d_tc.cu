@@ -125,9 +125,7 @@ __device__ __forceinline__ void splitk_reduce_store(const ConvParams& p, int S, 
 // MODE 1: "3xTF32" fp32 emulation: x = hi + lo with hi = tf32(x), lo = tf32(x - hi), three MMAs per K step into the same fp32
 //                 accumulator.  Weights arrive pre-split (two planes, packing.to_tc_layout); activations are split by the producer warps.
 // MT: 128-row accumulator tiles per CTA tile.  KBG: 16-byte K granules (4 tf32 or 8 bf16 channels each) per pipeline stage.
-// PDLM: programmatic dependent launch mode (EV_PDL): 0 = plain launch (no extra instructions),
-//       1 = convolutions only, 2 = every kernel of the engine launches this way (see the note after the set-up below).
-template <int MODE, int MT, int KBG, int PDLM>
+template <int MODE, int MT, int KBG>
 __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Plan pl) {
   constexpr bool SPLIT3 = (MODE == 1);
   constexpr bool X3B = (MODE == 3);       // "bf16x3": fp32 operands split into bf16 hi + lo planes, three bf16 MMAs per K = 16 step
@@ -160,17 +158,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
   }
   __syncthreads();
 
-  // Programmatic dependent launch (EV_PDL, default 2).  The grid is persistent (<= one CTA per SM, all resident), so it lets
-  // the NEXT launch in the stream start as soon as SMs free up: that kernel's CTAs run their set-up (barriers) while
-  // this grid's tail is still running.  Everything that touches activations (producers: x; consumers: res / out / split-K
-  // partials) first executes griddepcontrol.wait, which returns once the preceding grid has completed and its writes are
-  // visible.  PDLM == 1 (only the convolutions launch this way, so the launch before a convolution's predecessor has fully
-  // completed): the weight loader, which reads only weights and p.lens, does not wait and the first weight stages
-  // are prefetched under the predecessor's tail.  PDLM == 2 (every kernel launches this way): p.lens may come from a grid that
-  // is still running TWO launches upstream (validate_inputs_kernel writes the int32 lengths, LayerNorm starts early and waits,
-  // this kernel starts early too) -- a role that decoded tiles from stale lengths would walk a different tile sequence than
-  // the others and the pipeline would deadlock.  Every role waits.
-  if (PDLM) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // Programmatic dependent launch (ev_common.cuh).  The grid is persistent (<= one CTA per SM, all resident), so it lets the NEXT
+  // launch in the stream start as soon as SMs free up: that kernel's CTAs run their set-up (barriers) while this grid's tail is
+  // still running.  Every role, the weight loader included, executes griddepcontrol.wait before it reads p.lens or activations:
+  // p.lens may come from a grid that is still running TWO launches upstream (validate_inputs_kernel writes the int32 lengths,
+  // LayerNorm starts early and waits, this kernel starts early too), and a role that decoded tiles from stale lengths would walk
+  // a different tile sequence than the others and the pipeline would deadlock.
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   const int n_cb = (p.Cin + KB - 1) / KB;
   const int halo = ((p.K - 1) / 2) * p.dil;
@@ -193,7 +187,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
 
   if (warp < NCW) {
     // ============================ consumers: MMA issue + epilogue ==================================
-    if (PDLM) asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     const int wg = warp >> 2, wl = warp & 3;
     const bool split = pl.ksplit > 1;           // K-split: raw partial sums, the fused epilogue runs in the reduce kernel
     const bool has_res = p.res != nullptr && !split;
@@ -289,7 +283,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
     }
   } else if (warp < W_WLOAD) {
     // ============================ A producers ===================================================
-    if (PDLM) asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     const int pwarp = warp - NCW;
     const int wpg = NPWARPS / pl.ngroups;          // warps per group
     const int grp = pwarp / wpg;
@@ -378,7 +372,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
   } else {
     // ============================ weight loader ==================================================
     if (lane == 0) {
-      if (PDLM == 2) asm volatile("griddepcontrol.wait;" ::: "memory");      // p.lens (see the note after the set-up)
+      asm volatile("griddepcontrol.wait;" ::: "memory");      // p.lens (see the note after the set-up)
       // w_tc layout: [plane (hi, lo)][N tile of BNp = min(Cout,128)][tap][Cin/CPG granules][BNp][16 bytes]
       // (4 fp32 or 8 bf16 per granule; granule-major inside a tile)
       const int cin4 = p.Cin / CPG;
@@ -421,9 +415,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
 // Second half of a K-split convolution: out = epi( sum_z partial[z] ) with the slices added in the
 // fixed order z = 0..S-1 (deterministic, batch invariant), then bias / activation / residual /
 // accumulate exactly like the fused epilogue.  One float4 per thread.
-template <bool PDL>
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(ConvParams p, int S) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const size_t per = (size_t)p.B * p.L * p.Cout;
   const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 * 4 >= per) return;
@@ -437,50 +430,33 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(ConvParams p, int S)
 
 }  // namespace tc
 
-template <int MODE, int MT, int KBG, int PDLM>
-static int launch_tc_pdl(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
+template <int MODE, int MT, int KBG>
+static int launch_tc_variant(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
   static std::atomic<uint64_t> attr_devs{0};   // per instantiation; function attributes are per device
   if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, MT, KBG, PDLM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   const int grid = pl.total_tiles < sm_count() ? pl.total_tiles : sm_count();
-  if (PDLM) {
-    const cudaError_t e = launch_with_pdl(tc::conv1d_tc_kernel<MODE, MT, KBG, PDLM>, dim3((unsigned)grid), dim3(tc::NTHREADS),
-                                          (size_t)pl.smem_total, st, p, pl);
-    if (e != cudaSuccess) { set_error("conv1d_tc_kernel (PDL launch): %s", cudaGetErrorString(e)); return EV_ECUDA; }
-    count_launch();
-    return EV_OK;
-  }
-  tc::conv1d_tc_kernel<MODE, MT, KBG, PDLM><<<grid, tc::NTHREADS, pl.smem_total, st>>>(p, pl);
-  EV_CUDA_LAUNCH_CHECK("conv1d_tc_kernel");
-  return EV_OK;
-}
-
-// pdl: 0 for the default path, else pdl_mode()
-template <int MODE, int MT, int KBG>
-static int launch_tc_variant(const ConvParams& p, const tc::Plan& pl, cudaStream_t st, int pdl) {
-  if (pdl >= 2) return launch_tc_pdl<MODE, MT, KBG, 2>(p, pl, st);
-  if (pdl == 1) return launch_tc_pdl<MODE, MT, KBG, 1>(p, pl, st);
-  return launch_tc_pdl<MODE, MT, KBG, 0>(p, pl, st);
+  return launch("conv1d_tc_kernel", tc::conv1d_tc_kernel<MODE, MT, KBG>, (unsigned)grid, tc::NTHREADS, pl.smem_total, st, p, pl);
 }
 
 template <int MODE, int KBG>
-static int launch_tc_mt(const ConvParams& p, const tc::Plan& pl, cudaStream_t st, int pdl) {
-  if (pl.mt == 4) return launch_tc_variant<MODE, 4, KBG>(p, pl, st, pdl);
-  if (pl.mt == 2) return launch_tc_variant<MODE, 2, KBG>(p, pl, st, pdl);
-  return launch_tc_variant<MODE, 1, KBG>(p, pl, st, pdl);
+static int launch_tc_mt(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
+  if (pl.mt == 4) return launch_tc_variant<MODE, 4, KBG>(p, pl, st);
+  if (pl.mt == 2) return launch_tc_variant<MODE, 2, KBG>(p, pl, st);
+  return launch_tc_variant<MODE, 1, KBG>(p, pl, st);
 }
 
 template <int MODE, int KBG>
 static void preload_tc_mode() {
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 1, KBG, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 2, KBG, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 4, KBG, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 1, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 2, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 4, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
 }
-void preload_conv1d_tc() {      // see conv1d_gp.cu: preload_conv1d_gp (the default, non-PDL instantiations)
+void preload_conv1d_tc() {      // see conv1d_gp.cu: preload_conv1d_gp
   preload_tc_mode<0, 4>(); preload_tc_mode<0, 8>(); preload_tc_mode<1, 4>(); preload_tc_mode<2, 4>(); preload_tc_mode<2, 8>();
   preload_tc_mode<3, 4>(); preload_tc_mode<3, 8>();
   cudaFuncAttributes fa;
-  cudaFuncGetAttributes(&fa, tc::splitk_reduce_kernel<false>);
+  cudaFuncGetAttributes(&fa, tc::splitk_reduce_kernel);
   cudaGetLastError();
 }
 
@@ -559,11 +535,11 @@ int debug_tc_plan(const ConvParams& p, int mode, int* v) {
   return EV_OK;
 }
 
-static int dispatch_tc(const ConvParams& p, int mode, const tc::Plan& pl, cudaStream_t st, int pdl = 0) {
-  if (mode == 1) return launch_tc_mt<1, 4>(p, pl, st, pdl);
-  if (mode == 3) return pl.kbg == 8 ? launch_tc_mt<3, 8>(p, pl, st, pdl) : launch_tc_mt<3, 4>(p, pl, st, pdl);
-  if (mode == 2) return pl.kbg == 8 ? launch_tc_mt<2, 8>(p, pl, st, pdl) : launch_tc_mt<2, 4>(p, pl, st, pdl);
-  return pl.kbg == 8 ? launch_tc_mt<0, 8>(p, pl, st, pdl) : launch_tc_mt<0, 4>(p, pl, st, pdl);
+static int dispatch_tc(const ConvParams& p, int mode, const tc::Plan& pl, cudaStream_t st) {
+  if (mode == 1) return launch_tc_mt<1, 4>(p, pl, st);
+  if (mode == 3) return pl.kbg == 8 ? launch_tc_mt<3, 8>(p, pl, st) : launch_tc_mt<3, 4>(p, pl, st);
+  if (mode == 2) return pl.kbg == 8 ? launch_tc_mt<2, 8>(p, pl, st) : launch_tc_mt<2, 4>(p, pl, st);
+  return pl.kbg == 8 ? launch_tc_mt<0, 8>(p, pl, st) : launch_tc_mt<0, 4>(p, pl, st);
 }
 
 // p.w must be in the tensor-core layout [plane][Cout/BNp][K][Cin/4][BNp][4] (packing.py: to_tc_layout);
@@ -572,12 +548,10 @@ int launch_conv1d_tc(const ConvParams& p, int mode, cudaStream_t st) {
   tc::Plan pl;
   EV_TRY(plan_conv1d_tc(p, mode, &pl));
   const size_t per = (size_t)p.B * p.L * p.Cout;
-  const int rc = dispatch_tc(p, mode, pl, st, pdl_mode());      // EV_PDL (default 2)
+  const int rc = dispatch_tc(p, mode, pl, st);
   if (rc != EV_OK || pl.ksplit == 1) return rc;
   const size_t n4 = per / 4;
-  launch_k(tc::splitk_reduce_kernel<true>, tc::splitk_reduce_kernel<false>, (unsigned)((n4 + 255) / 256), 256, 0, st, p, pl.ksplit);
-  EV_CUDA_LAUNCH_CHECK("splitk_reduce_kernel");
-  return EV_OK;
+  return launch("splitk_reduce_kernel", tc::splitk_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, p, pl.ksplit);
 }
 
 }  // namespace ev

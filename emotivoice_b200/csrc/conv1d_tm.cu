@@ -20,9 +20,9 @@ constexpr int NTHREADS = 256;
 
 // TXN: threads along N (8 or 16); NV: float4 column groups per thread (1 or 2); TM: rows per thread.
 //   BN = TXN*4*NV,  BM = (256/TXN)*TM.
-template <int TXN, int NV, int TM, bool PDL>
+template <int TXN, int NV, int TM>
 __global__ void __launch_bounds__(NTHREADS) conv1d_tm_kernel(ConvParams p, int a_ld) {
-  pdl_entry<PDL>();
+  pdl_entry();
   constexpr int TYN = NTHREADS / TXN;   // threads along M
   constexpr int BM = TYN * TM;
   constexpr int BN = TXN * 4 * NV;
@@ -221,15 +221,11 @@ static int launch_variant(const ConvParams& p, cudaStream_t st) {
   const int a_ld = ((rows_a + 7) / 8) * 8 + 2;   // == 2 (mod 8): conflict-free transposed stores
   const size_t smem = (size_t)(2 * KC * a_ld + 2 * KC * BN) * sizeof(float);
   static std::atomic<uint64_t> attr_devs{0};   // per instantiation
-  if (first_use_on_device(attr_devs)) {
-    cudaFuncSetAttribute(conv1d_tm_kernel<TXN, NV, TM, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-    cudaFuncSetAttribute(conv1d_tm_kernel<TXN, NV, TM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  }
+  if (first_use_on_device(attr_devs))
+    cudaFuncSetAttribute(conv1d_tm_kernel<TXN, NV, TM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   EV_CHECK_ARG(smem <= 96 * 1024, "conv1d: smem %zu too large", smem);
   dim3 grid((p.L + BM - 1) / BM, (p.Cout + BN - 1) / BN, p.B);
-  launch_k(conv1d_tm_kernel<TXN, NV, TM, true>, conv1d_tm_kernel<TXN, NV, TM, false>, grid, NTHREADS, smem, st, p, a_ld);
-  EV_CUDA_LAUNCH_CHECK("conv1d_tm_kernel");
-  return EV_OK;
+  return launch("conv1d_tm_kernel", conv1d_tm_kernel<TXN, NV, TM>, grid, NTHREADS, smem, st, p, a_ld);
 }
 
 int launch_conv1d(const ConvParams& p, cudaStream_t st) {

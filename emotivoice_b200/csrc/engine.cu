@@ -37,13 +37,6 @@ void set_error(const char* fmt, ...) {
   g_err = buf;
 }
 void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
-static thread_local cudaError_t g_parked_launch_error = cudaSuccess;
-void park_launch_error(cudaError_t e) { if (e != cudaSuccess) g_parked_launch_error = e; }
-cudaError_t take_launch_error() {
-  const cudaError_t e = g_parked_launch_error;
-  g_parked_launch_error = cudaSuccess;
-  return e;
-}
 int sm_count() {
   static std::atomic<int> cache[64];
   int dev = 0;
@@ -69,8 +62,8 @@ int use_device_of(const void* dev_ptr) {
   if (e != cudaSuccess) { set_error("selecting the device of %p: %s", dev_ptr, cudaGetErrorString(e)); cudaGetLastError(); return EV_ECUDA; }
   return EV_OK;
 }
-int pdl_mode() {
-  static const int v = [] { const char* e = getenv("EV_PDL"); return (e && *e) ? atoi(e) : 2; }();
+bool pdl_enabled() {
+  static const bool v = [] { const char* e = getenv("EV_PDL"); return !(e && strcmp(e, "0") == 0); }();
   return v;
 }
 

@@ -12,9 +12,6 @@ namespace ev {
 // thread-local error string behind ev_last_error()
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
-// an error returned by cudaLaunchKernelEx (opt-in launch modes) is parked here and picked up by EV_CUDA_LAUNCH_CHECK
-void park_launch_error(cudaError_t e);
-cudaError_t take_launch_error();
 
 // Per-device one-time set-up.  cudaFuncSetAttribute and the SM count are per device and an engine may live on any GPU of the
 // process, so "done once" is tracked per device (bit d of `mask`); a benign race sets an attribute twice.
@@ -42,17 +39,6 @@ int use_device_of(const void* dev_ptr);  // cudaSetDevice(the device that owns d
     }                                                \
   } while (0)
 
-#define EV_CUDA_LAUNCH_CHECK(what)                                                        \
-  do {                                                                                    \
-    cudaError_t e__ = cudaGetLastError();                                                 \
-    if (e__ == cudaSuccess) e__ = ev::take_launch_error();                                \
-    if (e__ != cudaSuccess) {                                                             \
-      ev::set_error("%s: %s", what, cudaGetErrorString(e__));                             \
-      return EV_ECUDA;                                                                    \
-    }                                                                                     \
-    ev::count_launch();                                                                   \
-  } while (0)
-
 #define EV_TRY(expr)                 \
   do {                               \
     int rc__ = (expr);               \
@@ -60,43 +46,42 @@ int use_device_of(const void* dev_ptr);  // cudaSetDevice(the device that owns d
   } while (0)
 
 // ---------------------------------------------------------------------------------
-// Programmatic dependent launch.  EV_PDL=2 (the default since it measured 9 % on the batch-1 step, bitwise-identical results):
-// every kernel of the engine; EV_PDL=1: the tensor-core kernels only; EV_PDL=0: plain launches.  A kernel compiled with PDL = true starts with
-// griddepcontrol.launch_dependents (the next launch in the stream may be scheduled as soon as every CTA of this grid
-// has started) followed by griddepcontrol.wait (returns once the preceding grid has completed and its writes are
+// Programmatic dependent launch (measured 9 % on the batch-1 step, bitwise-identical results).  Every kernel of the engine
+// starts with griddepcontrol.launch_dependents (the next launch in the stream may be scheduled as soon as every CTA of this
+// grid has started) followed by griddepcontrol.wait (returns once the preceding grid has completed and its writes are
 // visible) -- before its first memory access, so stream order semantics are unchanged; what is gained is the launch
-// latency and, for the convolutions, the set-up (barriers, first weight stages) that runs before the wait.
+// latency and, for the convolutions, the set-up (barriers, first weight stages) that runs before the wait.  Launched
+// without the attribute (EV_PDL=0), both instructions are no-ops.
 // Transitivity: every kernel has at least one thread that waits unconditionally, so "grid N complete" implies "grid N-1 complete".
 // ---------------------------------------------------------------------------------
-template <bool PDL>
 __device__ __forceinline__ void pdl_entry() {
-  if (PDL) asm volatile("griddepcontrol.launch_dependents;\n\tgriddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;\n\tgriddepcontrol.wait;" ::: "memory");
 }
-int pdl_mode();      // 0, 1, 2 (default): the value of EV_PDL, read once
+bool pdl_enabled();  // false iff EV_PDL=0 (read once)
 
+// The engine's one way to launch a kernel: with programmatic stream serialization unless EV_PDL=0.  Reports the launch's own
+// error, or else the one cudaGetLastError() holds (and clears it), as "what: <error>"; counts the launch on success.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_with_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+inline int launch(const char* what, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, args...);
-}
-// launches `plain` exactly like `plain<<<grid, block, smem, st>>>(args...)`, or `with_pdl` with the attribute when EV_PDL >= 2;
-// launch errors surface through cudaGetLastError (EV_CUDA_LAUNCH_CHECK follows every call)
-template <typename K, typename... Args>
-inline void launch_k(K with_pdl, K plain, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  if (pdl_mode() >= 2) {
-    park_launch_error(launch_with_pdl(with_pdl, grid, block, smem, st, args...));
-  } else {
-    plain<<<grid, block, smem, st>>>(args...);
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, args...);
+  const cudaError_t last = cudaGetLastError();
+  if (e == cudaSuccess) e = last;
+  if (e != cudaSuccess) {
+    set_error("%s: %s", what, cudaGetErrorString(e));
+    return EV_ECUDA;
   }
+  count_launch();
+  return EV_OK;
 }
 
 // ---------------------------------------------------------------------------------

@@ -514,15 +514,7 @@ static int launch_pair_variant(const GpPairParams& p, const gpp::PPlan& pl, cons
     cudaFuncSetAttribute(gpp::resblock_gp_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  if (pdl_mode()) {
-    const cudaError_t e = launch_with_pdl(gpp::resblock_gp_kernel<MODE, MT, KBG>, dim3((unsigned)grid), dim3(gpp::GPP_THREADS), (size_t)pl.smem_total, st, p, pl, gs);
-    if (e != cudaSuccess) { set_error("resblock_gp_kernel (PDL launch): %s", cudaGetErrorString(e)); return EV_ECUDA; }
-    count_launch();
-    return EV_OK;
-  }
-  gpp::resblock_gp_kernel<MODE, MT, KBG><<<grid, gpp::GPP_THREADS, pl.smem_total, st>>>(p, pl, gs);
-  EV_CUDA_LAUNCH_CHECK("resblock_gp_kernel");
-  return EV_OK;
+  return launch("resblock_gp_kernel", gpp::resblock_gp_kernel<MODE, MT, KBG>, (unsigned)grid, gpp::GPP_THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 template <int MODE, int KBG>

@@ -27,12 +27,12 @@ __device__ __forceinline__ float warp_sum_f(float v) {
 // BertEmbeddings: y[b,t,:] = LayerNorm( (word[ids[b,t]] + type[tt[b,t]]) + pos[t] ), eps 1e-12.
 // One warp per token, the row lives in registers (C = NV*128 <= 768).
 // ---------------------------------------------------------------------------------------------
-template <int NV, bool PDL>
+template <int NV>
 __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ tts,
                                                              const float* __restrict__ word, const float* __restrict__ type,
                                                              const float* __restrict__ pos, const float* __restrict__ w,
                                                              const float* __restrict__ b, float* __restrict__ y, int rows, int N) {
-  pdl_entry<PDL>();
+  pdl_entry();
   constexpr int C = NV * 128;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -79,16 +79,15 @@ static int launch_bert_embed_ln(const int64_t* ids, const int64_t* tts, const fl
                                 const float* w, const float* b, float* y, int rows, int N, int C, cudaStream_t st) {
   EV_CHECK_ARG(rows > 0 && C % 128 == 0 && C <= 768, "bert_embed_ln: rows=%d C=%d (C must be a multiple of 128, <= 768)", rows, C);
   dim3 grid((rows + 7) / 8);
+  auto k = bert_embed_ln_kernel<6>;
   switch (C / 128) {
-    case 1: launch_k(bert_embed_ln_kernel<1, true>, bert_embed_ln_kernel<1, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
-    case 2: launch_k(bert_embed_ln_kernel<2, true>, bert_embed_ln_kernel<2, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
-    case 3: launch_k(bert_embed_ln_kernel<3, true>, bert_embed_ln_kernel<3, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
-    case 4: launch_k(bert_embed_ln_kernel<4, true>, bert_embed_ln_kernel<4, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
-    case 5: launch_k(bert_embed_ln_kernel<5, true>, bert_embed_ln_kernel<5, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
-    default: launch_k(bert_embed_ln_kernel<6, true>, bert_embed_ln_kernel<6, false>, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N); break;
+    case 1: k = bert_embed_ln_kernel<1>; break;
+    case 2: k = bert_embed_ln_kernel<2>; break;
+    case 3: k = bert_embed_ln_kernel<3>; break;
+    case 4: k = bert_embed_ln_kernel<4>; break;
+    case 5: k = bert_embed_ln_kernel<5>; break;
   }
-  EV_CUDA_LAUNCH_CHECK("bert_embed_ln_kernel");
-  return EV_OK;
+  return launch("bert_embed_ln_kernel", k, grid, 256, 0, st, ids, tts, word, type, pos, w, b, y, rows, N);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -96,11 +95,10 @@ static int launch_bert_embed_ln(const int64_t* ids, const int64_t* tts, const fl
 // BertPooler (x = the [CLS] row of each item: stride N_tokens*H, tanh) and the classification heads (stride H, none).
 // One CTA per (8 output columns, batch item); K is split over the CTA's threads and reduced in a fixed order.
 // ---------------------------------------------------------------------------------------------
-template <bool PDL>
 __global__ void __launch_bounds__(256) row_gemv_kernel(const float* __restrict__ x, size_t x_stride, const float* __restrict__ w,
                                                        const float* __restrict__ bias, float* __restrict__ out, int K, int N,
                                                        int act) {
-  pdl_entry<PDL>();
+  pdl_entry();
   __shared__ float red[8][8][33];
   const int b = blockIdx.y, n0 = blockIdx.x * 8;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -133,9 +131,7 @@ static int launch_row_gemv(const float* x, size_t x_stride, const float* w, cons
                            int act, cudaStream_t st) {
   EV_CHECK_ARG(N % 8 == 0 && N > 0 && B > 0 && B <= 65535, "row_gemv: N=%d B=%d", N, B);
   dim3 grid(N / 8, B);
-  launch_k(row_gemv_kernel<true>, row_gemv_kernel<false>, grid, 256, 0, st, x, x_stride, w, bias, out, K, N, act);
-  EV_CUDA_LAUNCH_CHECK("row_gemv_kernel");
-  return EV_OK;
+  return launch("row_gemv_kernel", row_gemv_kernel, grid, 256, 0, st, x, x_stride, w, bias, out, K, N, act);
 }
 
 struct StyleLayerW {

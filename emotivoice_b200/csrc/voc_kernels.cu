@@ -6,9 +6,8 @@ namespace ev {
 
 // (B, C, L) channels-first (the reference's Generator.forward input, hifigan/models.py:115)
 // -> (B, L, C) time-major (the engine's internal layout).  32x32 smem tile transpose.
-template <bool PDL>
 __global__ void transpose_cf_to_tm_kernel(const float* __restrict__ in, float* __restrict__ out, int C, int L) {
-  pdl_entry<PDL>();
+  pdl_entry();
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int l0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -27,21 +26,18 @@ __global__ void transpose_cf_to_tm_kernel(const float* __restrict__ in, float* _
 int launch_transpose_cf_to_tm(const float* in, float* out, int B, int C, int L, cudaStream_t st) {
   EV_CHECK_ARG(B > 0 && C > 0 && L > 0 && B <= 65535, "transpose: bad shape");
   dim3 grid((L + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  launch_k(transpose_cf_to_tm_kernel<true>, transpose_cf_to_tm_kernel<false>, grid, block, 0, st, in, out, C, L);
-  EV_CUDA_LAUNCH_CHECK("transpose_cf_to_tm_kernel");
-  return EV_OK;
+  return launch("transpose_cf_to_tm_kernel", transpose_cf_to_tm_kernel, grid, block, 0, st, in, out, C, L);
 }
 
 // wav[b,t] = tanh( bias + sum_j sum_c w[j][c] * lrelu(x[b, t+j-(K-1)/2, c]) )
 // (hifigan/models.py:127-129: F.leaky_relu default slope 0.01, Conv1d(C,1,7,pad 3), tanh).
 // HBM-bound: each CTA stages (256 + K - 1) rows once; rows >= len read as zero padding.
 constexpr int CP_BT = 256;
-template <bool PDL>
 __global__ void __launch_bounds__(CP_BT) conv_post_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                           const float* __restrict__ bias, const int32_t* __restrict__ lens,
                                                           int lens_mul, int L, int C, int K, float slope,
                                                           float* __restrict__ wav) {
-  pdl_entry<PDL>();
+  pdl_entry();
   extern __shared__ __align__(16) float cp_smem[];
   const int ld = C + 1;
   float* xs = cp_smem;                          // [(CP_BT + K - 1)][C + 1]
@@ -80,21 +76,16 @@ int launch_conv_post(const float* x, const float* w, const float* bias, const in
   EV_CHECK_ARG(B > 0 && B <= 65535 && L > 0, "conv_post: bad shape");
   const size_t smem = (size_t)((CP_BT + K - 1) * (C + 1) + K * C) * sizeof(float);
   static std::atomic<uint64_t> attr_devs{0};
-  if (first_use_on_device(attr_devs)) {
-    cudaFuncSetAttribute(conv_post_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-    cudaFuncSetAttribute(conv_post_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-  }
+  if (first_use_on_device(attr_devs))
+    cudaFuncSetAttribute(conv_post_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   dim3 grid((L + CP_BT - 1) / CP_BT, B);
-  launch_k(conv_post_kernel<true>, conv_post_kernel<false>, grid, CP_BT, smem, st, x, w, bias, lens, lens_mul, L, C, K, slope, wav);
-  EV_CUDA_LAUNCH_CHECK("conv_post_kernel");
-  return EV_OK;
+  return launch("conv_post_kernel", conv_post_kernel, grid, CP_BT, smem, st, x, w, bias, lens, lens_mul, L, C, K, slope, wav);
 }
 
 // pcm = (int16) trunc(wav * 32768): numpy astype('int16') of a float array is a C cast
 // (inference_am_vocoder_joint.py:130-131).  Values are inside (-1, 1) after tanh.
-template <bool PDL>
 __global__ void pcm16_kernel(const float* __restrict__ wav, int16_t* __restrict__ pcm, size_t n) {
-  pdl_entry<PDL>();
+  pdl_entry();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
     float v = truncf(wav[i] * 32768.0f);
@@ -104,9 +95,7 @@ __global__ void pcm16_kernel(const float* __restrict__ wav, int16_t* __restrict_
 }
 int launch_pcm16(const float* wav, int16_t* pcm, size_t n, cudaStream_t st) {
   if (n == 0) return EV_OK;
-  launch_k(pcm16_kernel<true>, pcm16_kernel<false>, (unsigned)((n + 255) / 256), 256, 0, st, wav, pcm, n);
-  EV_CUDA_LAUNCH_CHECK("pcm16_kernel");
-  return EV_OK;
+  return launch("pcm16_kernel", pcm16_kernel, (unsigned)((n + 255) / 256), 256, 0, st, wav, pcm, n);
 }
 
 }  // namespace ev

@@ -8,10 +8,12 @@ and issue a whole chunk's residual and output loads before its first store (DESI
 between the last HGMMA and the first STG after it there must be at least two non-constant LDG (residual, output) per pair of
 the first chunk: 4 pairs in conv1d_gp (8 at MT = 4), 2 MT pairs (one column group) in resblock_gp.
 """
+import os
 import re
 
 import pytest
 
+from emotivoice_b200 import build
 from test_wgmma_pipeline_sass import _sass_text, _tools
 
 CHUNK_PAIRS = {"conv1d_gp_kernel": lambda mt: 8 if mt == 4 else 4, "resblock_gp_kernel": lambda mt: 2 * mt}
@@ -47,7 +49,7 @@ def functions():
     nvcc, cuobjdump = _tools()
     if not nvcc or not cuobjdump:
         pytest.skip("needs nvcc and cuobjdump")
-    return _instructions(_sass_text(nvcc, cuobjdump))
+    return _instructions(_sass_text(nvcc, cuobjdump, [os.path.join(build.CSRC, src) for src in ("conv1d_gp.cu", "resblock_gp.cu")]))
 
 
 @pytest.mark.parametrize("kernel", list(CHUNK_PAIRS))

@@ -33,15 +33,15 @@ def _tools():
     return nvcc, cuobjdump
 
 
-def _sass_text(nvcc, cuobjdump):
+def _sass_text(nvcc, cuobjdump, sources):
+    """SASS of the in-tree library when it is current, else of `sources` (paths of .cu files) compiled to cubins"""
     if build._up_to_date(build._digest()):
         return subprocess.run([cuobjdump, "-sass", build.LIB_PATH], capture_output=True, text=True, check=True).stdout
     with tempfile.TemporaryDirectory() as tmp:
         procs = []
-        for src in KERNELS.values():
-            out = os.path.join(tmp, src[:-3] + ".cubin")
-            cmd = [nvcc] + [f for f in build.NVCC_FLAGS if f not in ("-cudart", "static")] + ["-I", build.INCLUDE, "-cubin",
-                                                                                              os.path.join(build.CSRC, src), "-o", out]
+        for src in sources:
+            out = os.path.join(tmp, os.path.basename(src)[:-3] + ".cubin")
+            cmd = [nvcc] + [f for f in build.NVCC_FLAGS if f not in ("-cudart", "static")] + ["-I", build.INCLUDE, "-cubin", src, "-o", out]
             procs.append((out, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
         text = []
         for out, p in procs:
@@ -78,7 +78,7 @@ def functions():
     nvcc, cuobjdump = _tools()
     if not nvcc or not cuobjdump:
         pytest.skip("needs nvcc and cuobjdump")
-    return _per_function(_sass_text(nvcc, cuobjdump))
+    return _per_function(_sass_text(nvcc, cuobjdump, [os.path.join(build.CSRC, src) for src in KERNELS.values()]))
 
 
 @pytest.mark.parametrize("kernel", list(KERNELS))

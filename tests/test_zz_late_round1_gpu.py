@@ -176,8 +176,8 @@ np.savez(sys.argv[3], **res)
 
 
 def _check_knobs_bitwise(model, dev, tmp_path, knobs):
-    """EV_PDL=2 (the default) launches every kernel of the engine with programmatic stream serialization (set-up and weight
-    prefetch of launch n+1 overlap the tail of launch n), EV_PDL=1 the tensor-core kernels only, EV_PDL=0 none.
+    """By default every kernel of the engine is launched with programmatic stream serialization (set-up and weight prefetch of
+    launch n+1 overlap the tail of launch n); EV_PDL=0 launches the same kernels without it, their griddepcontrol instructions no-ops.
     EV_VOC_GROUP=0 launches the three parallel ResBlocks of a vocoder stage one convolution at a time, EV_FUSE_RES=0 each ResBlock
     layer as two launches.  None of them reorders any output element's reduction, so every output bit must equal the default mode's;
     a missing griddepcontrol.wait or a tile-shape-dependent result would show up here as a mismatch."""
@@ -201,8 +201,8 @@ def _check_knobs_bitwise(model, dev, tmp_path, knobs):
         model.precision = "fp32"
 
 
-@pytest.mark.parametrize("knobs", [{"EV_PDL": "0"}, {"EV_PDL": "1"}, {"EV_VOC_GROUP": "0"}, {"EV_VOC_GROUP": "0", "EV_FUSE_RES": "0"}],
-                         ids=["plain_launches", "pdl_tensor_core_only", "no_grouped_launches", "no_grouped_no_fused"])
+@pytest.mark.parametrize("knobs", [{"EV_PDL": "0"}, {"EV_VOC_GROUP": "0"}, {"EV_VOC_GROUP": "0", "EV_FUSE_RES": "0"}],
+                         ids=["plain_launches", "no_grouped_launches", "no_grouped_no_fused"])
 def test_launch_modes_are_bitwise_identical(model, dev, tmp_path, knobs):
     _check_knobs_bitwise(model, dev, tmp_path, knobs)
 

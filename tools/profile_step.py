@@ -7,8 +7,8 @@ Prints, per step: device time of every kernel (name with template arguments), it
 then the total of each stage.  The three engine calls (`ev:am_phase1`, `ev:am_phase2`, `ev:vocoder`, the engine's NVTX range names)
 are wrapped in profiler ranges on the host, and a kernel belongs to the range its launch was issued in.  The vocoder's stages
 (`voc:stage1..4`) are NVTX ranges inside one engine call; torch.profiler does not record NVTX ranges, so they are not split out here.
-With programmatic dependent launch (EV_PDL=2, the default) a kernel's span starts while its predecessor still runs and includes its
-wait for it, so spans overlap and their sum exceeds the step time; run with EV_PDL=0 for spans that do not overlap.
+With programmatic dependent launch (the default) a kernel's span starts while its predecessor still runs and includes its wait for
+it, so spans overlap and their sum exceeds the step time; run with EV_PDL=0 for spans that do not overlap.
 The card's name and power limit are read in the same run.  With --out DIR the table is also written as DIR/profile_step.json; the
 raw trace goes to a temporary directory and is deleted.
 """
