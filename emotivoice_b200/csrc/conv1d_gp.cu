@@ -97,8 +97,8 @@ __device__ __forceinline__ float lrelu_f(float v, float slope) { return fmaxf(v,
 // MODE 0: one tf32 MMA per K step; 1: 3xTF32 fp32 emulation (hi/lo planes, three MMAs per K step); 2: bf16 operands,
 // bf16 activations in HBM (8 channels per granule); 3: "bf16x3": fp32 activations in HBM, every operand split
 // into bf16 hi + lo (16 significant bits), three bf16 MMAs per K = 16 step -- an fp32-class result (~1e-5 relative) at
-// half the tensor-core and shared-memory cost of 3xTF32.  Accumulation is fp32 in every mode.
-template <int MODE, int MT, int KBG>
+// half the tensor-core and shared-memory cost of 3xTF32.  Accumulation is fp32 in every mode.  BN = pl.BN, the N tile.
+template <int MODE, int MT, int KBG, int BN>
 __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_constant__ GpConvParams p, const __grid_constant__ GPlan pl,
                                                                   const __grid_constant__ GpGroups gs) {
   constexpr bool SPLIT3 = (MODE == 1);     // 3xTF32: hi / lo tf32 planes
@@ -110,12 +110,13 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   constexpr int WCPG = OP16 ? 8 : 4;       // channels per 16-byte granule of the weights
   constexpr int KB = CPG * KBG;
   constexpr int NA = ACC_REGS / MT;
+  constexpr int NK8 = KB / (2 * WCPG);     // MMA K steps of a full channel block
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules (16 channels) per MMA K step");
+  static_assert(MT * BN <= 2 * ACC_REGS, "accumulators of the tile exceed the register budget");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int lane = tid & 31;
-  const int BN = pl.BN;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* a_tiles = smem_raw + SMEM_HEAD;
@@ -199,8 +200,7 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
           mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
           const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
           const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
-          wgmma_fence();
-          for (int k8 = 0; k8 < nk8; ++k8) {
+          auto k_step = [&](int k8) {
             const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
             const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
             const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
@@ -208,8 +208,16 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
 #pragma unroll
             for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
               const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-              mma_step<MODE, NA>(BN, acc[mt], a_hi, desc_advance(a_hi, a_lo_off), b_hi, b_lo, first);
+              mma_step_fixed<MODE, BN>(acc[mt], a_hi, desc_advance(a_hi, a_lo_off), b_hi, b_lo, first);
             }
+          };
+          wgmma_fence();
+          if (nk8 == NK8) {                        // a full channel block: its NK8 * MT * m MMAs as one chain
+#pragma unroll
+            for (int k8 = 0; k8 < NK8; ++k8) k_step(k8);
+          } else {                                 // the short last block of a C_in that is not a multiple of KB (conv_pre's 80)
+#pragma unroll 1
+            for (int k8 = 0; k8 < nk8; ++k8) k_step(k8);
           }
           wgmma_commit();
           wgmma_wait<1>();          // the previous step's MMAs have completed: its stages may be refilled
@@ -717,28 +725,35 @@ int debug_gp_plan(const GpConvParams& p, int mode, int* v) {
   return EV_OK;
 }
 
-template <int MODE, int MT, int KBG>
-static int launch_gp_variant(const GpConvParams& p, const gp::GPlan& pl, const GpGroups& gs, cudaStream_t st) {
-  static std::atomic<uint64_t> attr_devs{0};
-  if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(gp::conv1d_gp_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  const int nsm = sm_count();
-  const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  return launch("conv1d_gp_kernel", gp::conv1d_gp_kernel<MODE, MT, KBG>, (unsigned)grid, gp::GP_THREADS, pl.smem_total, st, p, pl, gs);
-}
-
+// The instantiations: every (MODE, KBG) the shape rule gp_shape_kbg gives (KBG = 4 in 3xTF32) times every tile plan_gp can return,
+// BN = min(C_out, 128) in {32, 64, 96, 128} (validate_gp) with MT * BN <= 128.
+using GpKernel = void (*)(GpConvParams, gp::GPlan, GpGroups);
 template <int MODE, int KBG>
-static int launch_gp_mt(const GpConvParams& p, const gp::GPlan& pl, const GpGroups& gs, cudaStream_t st) {
-  if (pl.mt == 4) return launch_gp_variant<MODE, 4, KBG>(p, pl, gs, st);
-  if (pl.mt == 2) return launch_gp_variant<MODE, 2, KBG>(p, pl, gs, st);
-  return launch_gp_variant<MODE, 1, KBG>(p, pl, gs, st);
+static GpKernel gp_kernel_tile(int mt, int bn) {
+  switch (bn) {
+    case 128: return mt == 1 ? gp::conv1d_gp_kernel<MODE, 1, KBG, 128> : nullptr;
+    case 96: return mt == 1 ? gp::conv1d_gp_kernel<MODE, 1, KBG, 96> : nullptr;
+    case 64: return mt == 2 ? gp::conv1d_gp_kernel<MODE, 2, KBG, 64> : mt == 1 ? gp::conv1d_gp_kernel<MODE, 1, KBG, 64> : nullptr;
+    case 32: return mt == 4 ? gp::conv1d_gp_kernel<MODE, 4, KBG, 32> : mt == 2 ? gp::conv1d_gp_kernel<MODE, 2, KBG, 32>
+                  : mt == 1 ? gp::conv1d_gp_kernel<MODE, 1, KBG, 32> : nullptr;
+    default: return nullptr;
+  }
+}
+static GpKernel gp_kernel(int mode, int kbg, int mt, int bn) {
+  if (mode == 1) return kbg == 4 ? gp_kernel_tile<1, 4>(mt, bn) : nullptr;
+  if (mode == 3) return kbg == 8 ? gp_kernel_tile<3, 8>(mt, bn) : gp_kernel_tile<3, 4>(mt, bn);
+  if (mode == 2) return kbg == 8 ? gp_kernel_tile<2, 8>(mt, bn) : gp_kernel_tile<2, 4>(mt, bn);
+  return kbg == 8 ? gp_kernel_tile<0, 8>(mt, bn) : gp_kernel_tile<0, 4>(mt, bn);
 }
 
 static int dispatch_gp(const GpConvParams& p, const gp::GPlan& pl, const GpGroups& gs, int mode, cudaStream_t st) {
-  if (mode == 1) return launch_gp_mt<1, 4>(p, pl, gs, st);
-  if (mode == 3) return pl.kbg == 8 ? launch_gp_mt<3, 8>(p, pl, gs, st) : launch_gp_mt<3, 4>(p, pl, gs, st);
-  if (mode == 2) return pl.kbg == 8 ? launch_gp_mt<2, 8>(p, pl, gs, st) : launch_gp_mt<2, 4>(p, pl, gs, st);
-  return pl.kbg == 8 ? launch_gp_mt<0, 8>(p, pl, gs, st) : launch_gp_mt<0, 4>(p, pl, gs, st);
+  static std::atomic<uint64_t> attr_devs{0};
+  if (first_use_on_device(attr_devs)) preload_conv1d_gp();
+  const GpKernel k = gp_kernel(mode, pl.kbg, pl.mt, pl.BN);
+  EV_CHECK_ARG(k, "conv1d_gp: no kernel for mode %d, KBG %d, MT %d, BN %d", mode, pl.kbg, pl.mt, pl.BN);
+  const int nsm = sm_count();
+  const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
+  return launch("conv1d_gp_kernel", k, (unsigned)grid, gp::GP_THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 int launch_conv1d_gp(const GpConvParams& p, int mode, cudaStream_t st) {
@@ -816,16 +831,14 @@ static int plan_group(const GpConvParams* ps, int n, int mode, GpGroups* gs_out,
 }
 
 // Load every instantiation's code now (CUDA loads kernels lazily, at their first launch: tens of milliseconds for a kernel of this
-// size, which would otherwise hit whichever utterance first needs a new tile shape) and set the shared-memory attribute.
-template <int MODE, int KBG>
-static void preload_gp_mode() {
-  cudaFuncSetAttribute(gp::conv1d_gp_kernel<MODE, 1, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(gp::conv1d_gp_kernel<MODE, 2, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(gp::conv1d_gp_kernel<MODE, 4, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-}
+// size, which would otherwise hit whichever utterance first needs a new tile shape) and set the shared-memory attribute -- on
+// exactly the instantiations dispatch_gp can launch.
 void preload_conv1d_gp() {
-  preload_gp_mode<0, 4>(); preload_gp_mode<0, 8>(); preload_gp_mode<1, 4>(); preload_gp_mode<2, 4>(); preload_gp_mode<2, 8>();
-  preload_gp_mode<3, 4>(); preload_gp_mode<3, 8>();
+  for (int mode = 0; mode < 4; ++mode)
+    for (int kbg = 4; kbg <= 8; kbg += 4)
+      for (int bn = 32; bn <= 128; bn += 32)
+        for (int mt = 1; mt * bn <= 128; mt *= 2)
+          if (const GpKernel k = gp_kernel(mode, kbg, mt, bn)) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   cudaFuncSetAttribute(gp::conv_post_gp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   cudaFuncSetAttribute(gp::conv_post_gp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   cudaFuncSetAttribute(gp::conv_post_gp4_kernel<false, 7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024);

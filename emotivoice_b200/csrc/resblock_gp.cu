@@ -81,8 +81,8 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
 // LeakyReLU for 0 <= slope <= 1 as max(v, v*slope): two instructions (FMUL + FMNMX) instead of compare / multiply / select; same bits
 __device__ __forceinline__ float lrelu_f(float v, float slope) { return fmaxf(v, v * slope); }
 
-// MODE as conv1d_gp.cu: 0 tf32, 1 3xTF32, 2 bf16 activations + operands, 3 bf16x3 on fp32 activations.
-template <int MODE, int MT, int KBG>
+// MODE as conv1d_gp.cu: 0 tf32, 1 3xTF32, 2 bf16 activations + operands, 3 bf16x3 on fp32 activations.  C = p.C, the channels.
+template <int MODE, int MT, int KBG, int C>
 __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __grid_constant__ GpPairParams p, const __grid_constant__ PPlan pl,
                                                                      const __grid_constant__ GpPairGroups gs) {
   constexpr bool SPLIT3 = (MODE == 1), BF16 = (MODE == 2), X3B = (MODE == 3);
@@ -93,11 +93,14 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
   constexpr int KB = CPG * KBG;
   constexpr int KBGW = KBG * CPG / OCPG;        // operand granules (weights, xt tile) per channel block
   constexpr int NA = ACC_REGS / MT;
+  // C and KB are powers of two: every channel block is full (or the only one), so its MMA K steps are a constant
+  constexpr int NK = (C < KB ? C : KB) / (2 * OCPG);
+  static_assert(C % KB == 0 || C < KB, "every channel block has NK K steps");
   static_assert(!X3B || KBG % 4 == 0, "bf16x3 consumes four fp32 granules per MMA K step");
+  static_assert(MT * C <= 2 * ACC_REGS, "accumulators of the tile exceed the register budget");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
-  const int C = p.C;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* a2_tile = smem_raw + SMEM_HEAD;
@@ -178,18 +181,22 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       // ---- c1 over the staged x tile
       {
         int prev_sb = -1, prev_sa = -1;
+        // Not unrolled, not peeled: with C and the K steps constants the compiler would otherwise copy the channel-block and tap
+        // loops, and every copy adds a wgmma.wait_group site (tests/test_wgmma_pipeline_sass.py counts them).
+#pragma unroll 1
         for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
           const int sa = a_cnt % pl.a_stages;
-          const int nk = min(KB, C - cb * KB) / (2 * OCPG);
           mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
           const uint64_t x0 = desc_advance(x_desc0, smem_u32(x_tiles + sa * pl.x_stage_bytes) + (uint32_t)(wg * 64) * 16u);
+#pragma unroll 1
           for (int j = 0; j < K; ++j, ++b_cnt) {
             const int sb = b_cnt % pl.b_stages;
             mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
             const uint64_t xj = desc_advance(x0, (uint32_t)(j * dil) * 16u);
             wgmma_fence();
-            for (int k = 0; k < nk; ++k) {
+#pragma unroll
+            for (int k = 0; k < NK; ++k) {          // the channel block's NK * MT * m MMAs: one chain
               const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
               const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
               const uint64_t a_k = desc_advance(xj, (uint32_t)k * x_k);
@@ -197,7 +204,7 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
 #pragma unroll
               for (int mt = 0; mt < MT; ++mt) {
                 const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma_step<MODE, NA>(C, acc[mt], a_hi, desc_advance(a_hi, x_lo_off), b_hi, b_lo, first);
+                mma_step_fixed<MODE, C>(acc[mt], a_hi, desc_advance(a_hi, x_lo_off), b_hi, b_lo, first);
               }
             }
             wgmma_commit();
@@ -303,16 +310,18 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       // ---- c2 over the xt tile
       {
         int prev_sb = -1;
+#pragma unroll 1                            // as in c1
         for (int cb = 0; cb < n_cb; ++cb) {
-          const int nk = min(KB, C - cb * KB) / (2 * OCPG);
           const uint64_t a0 = desc_advance(a2_desc0, (uint32_t)(cb * KBGW) * a2_lbo);
+#pragma unroll 1
           for (int j = 0; j < K; ++j, ++b_cnt) {
             const int sb = b_cnt % pl.b_stages;
             mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
             const uint64_t aj = desc_advance(a0, (uint32_t)j * 16u);
             wgmma_fence();
-            for (int k = 0; k < nk; ++k) {
+#pragma unroll
+            for (int k = 0; k < NK; ++k) {
               const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
               const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
               const uint64_t a_k = desc_advance(aj, (uint32_t)k * 2u * a2_lbo);
@@ -320,7 +329,7 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
 #pragma unroll
               for (int mt = 0; mt < MT; ++mt) {
                 const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma_step<MODE, NA>(C, acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a2_plane_bytes), b_hi, b_lo, first);
+                mma_step_fixed<MODE, C>(acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a2_plane_bytes), b_hi, b_lo, first);
               }
             }
             wgmma_commit();
@@ -507,38 +516,41 @@ int debug_gp_pair_plan(const GpPairParams& p, int mode, int* v) {
   return EV_OK;
 }
 
-template <int MODE, int MT, int KBG>
-static int launch_pair_variant(const GpPairParams& p, const gpp::PPlan& pl, const GpPairGroups& gs, cudaStream_t st) {
+// The instantiations: every (MODE, KBG) of pair_shape_kbg times every tile plan_pair can return, C in {32, 64, 128} with MT * C <= 128.
+using PairKernel = void (*)(GpPairParams, gpp::PPlan, GpPairGroups);
+template <int MODE, int KBG>
+static PairKernel pair_kernel_tile(int mt, int c) {
+  switch (c) {
+    case 128: return mt == 1 ? gpp::resblock_gp_kernel<MODE, 1, KBG, 128> : nullptr;
+    case 64: return mt == 2 ? gpp::resblock_gp_kernel<MODE, 2, KBG, 64> : mt == 1 ? gpp::resblock_gp_kernel<MODE, 1, KBG, 64> : nullptr;
+    case 32: return mt == 4 ? gpp::resblock_gp_kernel<MODE, 4, KBG, 32> : mt == 2 ? gpp::resblock_gp_kernel<MODE, 2, KBG, 32>
+                  : mt == 1 ? gpp::resblock_gp_kernel<MODE, 1, KBG, 32> : nullptr;
+    default: return nullptr;
+  }
+}
+static PairKernel pair_kernel(int mode, int kbg, int mt, int c) {
+  if (mode == 1) return kbg == 4 ? pair_kernel_tile<1, 4>(mt, c) : nullptr;
+  if (mode == 3) return kbg == 8 ? pair_kernel_tile<3, 8>(mt, c) : pair_kernel_tile<3, 4>(mt, c);
+  if (mode == 2) return kbg == 8 ? pair_kernel_tile<2, 8>(mt, c) : pair_kernel_tile<2, 4>(mt, c);
+  return kbg == 8 ? pair_kernel_tile<0, 8>(mt, c) : pair_kernel_tile<0, 4>(mt, c);
+}
+
+static int dispatch_pair(const GpPairParams& p, const gpp::PPlan& pl, const GpPairGroups& gs, int mode, cudaStream_t st) {
   static std::atomic<uint64_t> attr_devs{0};
-  if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(gpp::resblock_gp_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  if (first_use_on_device(attr_devs)) preload_resblock_gp();
+  const PairKernel k = pair_kernel(mode, pl.kbg, pl.mt, p.C);
+  EV_CHECK_ARG(k, "resblock_gp: no kernel for mode %d, KBG %d, MT %d, C %d", mode, pl.kbg, pl.mt, p.C);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  return launch("resblock_gp_kernel", gpp::resblock_gp_kernel<MODE, MT, KBG>, (unsigned)grid, gpp::GPP_THREADS, pl.smem_total, st, p, pl, gs);
+  return launch("resblock_gp_kernel", k, (unsigned)grid, gpp::GPP_THREADS, pl.smem_total, st, p, pl, gs);
 }
 
-template <int MODE, int KBG>
-static int launch_pair_mt(const GpPairParams& p, const gpp::PPlan& pl, const GpPairGroups& gs, cudaStream_t st) {
-  if (pl.mt == 4) return launch_pair_variant<MODE, 4, KBG>(p, pl, gs, st);
-  if (pl.mt == 2) return launch_pair_variant<MODE, 2, KBG>(p, pl, gs, st);
-  return launch_pair_variant<MODE, 1, KBG>(p, pl, gs, st);
-}
-static int dispatch_pair(const GpPairParams& p, const gpp::PPlan& pl, const GpPairGroups& gs, int mode, cudaStream_t st) {
-  if (mode == 1) return launch_pair_mt<1, 4>(p, pl, gs, st);
-  if (mode == 3) return pl.kbg == 8 ? launch_pair_mt<3, 8>(p, pl, gs, st) : launch_pair_mt<3, 4>(p, pl, gs, st);
-  if (mode == 2) return pl.kbg == 8 ? launch_pair_mt<2, 8>(p, pl, gs, st) : launch_pair_mt<2, 4>(p, pl, gs, st);
-  return pl.kbg == 8 ? launch_pair_mt<0, 8>(p, pl, gs, st) : launch_pair_mt<0, 4>(p, pl, gs, st);
-}
-
-template <int MODE, int KBG>
-static void preload_pair_mode() {
-  cudaFuncSetAttribute(gpp::resblock_gp_kernel<MODE, 1, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(gpp::resblock_gp_kernel<MODE, 2, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(gpp::resblock_gp_kernel<MODE, 4, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-}
 void preload_resblock_gp() {      // see preload_conv1d_gp
-  preload_pair_mode<0, 4>(); preload_pair_mode<0, 8>(); preload_pair_mode<1, 4>(); preload_pair_mode<2, 4>(); preload_pair_mode<2, 8>();
-  preload_pair_mode<3, 4>(); preload_pair_mode<3, 8>();
+  for (int mode = 0; mode < 4; ++mode)
+    for (int kbg = 4; kbg <= 8; kbg += 4)
+      for (int c = 32; c <= 128; c *= 2)
+        for (int mt = 1; mt * c <= 128; mt *= 2)
+          if (const PairKernel k = pair_kernel(mode, kbg, mt, c)) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   cudaGetLastError();
 }
 

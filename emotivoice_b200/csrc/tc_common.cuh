@@ -218,6 +218,16 @@ __device__ __forceinline__ void wgmma_n(int n, float (&d)[NA], uint64_t a, uint6
 #undef EV_WG_CASE
 }
 
+// D = A * B with the instruction's N fixed at compile time (a multiple of 32 up to 2 * NA).
+template <bool BF16, int N, int NA>
+__device__ __forceinline__ void wgmma_fixed(float (&d)[NA], uint64_t a, uint64_t b, uint32_t acc) {
+  static_assert(N % 32 == 0 && N <= 128 && N <= 2 * NA, "N tile must be 32 / 64 / 96 / 128 and fit the accumulator");
+  if constexpr (N == 32) { if constexpr (BF16) wgmma_bf16_n32(d, a, b, acc); else wgmma_tf32_n32(d, a, b, acc); }
+  else if constexpr (N == 64) { if constexpr (BF16) wgmma_bf16_n64(d, a, b, acc); else wgmma_tf32_n64(d, a, b, acc); }
+  else if constexpr (N == 96) { if constexpr (BF16) wgmma_bf16_n96(d, a, b, acc); else wgmma_tf32_n96(d, a, b, acc); }
+  else { if constexpr (BF16) wgmma_bf16_n128(d, a, b, acc); else wgmma_tf32_n128(d, a, b, acc); }
+}
+
 // One K step of the convolution kernels' modes into one accumulator.  MODE 0: one tf32 MMA; 2: one bf16 MMA; 1 ("3xTF32") / 3
 // ("bf16x3"): operands split into hi + lo, a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (small terms first, the dropped lo*lo term is
 // below fp32 rounding), three MMAs into the same fp32 accumulator.
@@ -230,6 +240,21 @@ __device__ __forceinline__ void mma_step(int n, float (&d)[NA], uint64_t a_hi, u
     wgmma_n<OP16, NA>(n, d, a_hi, b_hi, 1u);
   } else {
     wgmma_n<OP16, NA>(n, d, a_hi, b_hi, acc);
+  }
+}
+
+// mma_step with N fixed at compile time (the granule-planar kernels): every MMA is one wgmma, so the MMAs of a whole channel
+// block form one unbroken chain between a fence and a commit -- the run-time switch above splits them with a branch and a
+// warpgroup.arrive per K step.  Same MMAs in the same order.
+template <int MODE, int N, int NA>
+__device__ __forceinline__ void mma_step_fixed(float (&d)[NA], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t acc) {
+  constexpr bool OP16 = MODE >= 2;
+  if constexpr (MODE == 1 || MODE == 3) {
+    wgmma_fixed<OP16, N>(d, a_lo, b_hi, acc);
+    wgmma_fixed<OP16, N>(d, a_hi, b_lo, 1u);
+    wgmma_fixed<OP16, N>(d, a_hi, b_hi, 1u);
+  } else {
+    wgmma_fixed<OP16, N>(d, a_hi, b_hi, acc);
   }
 }
 
