@@ -12,35 +12,26 @@
 //     lanes of a quad together with the eight rows of a warp cover whole 128-byte granule runs.
 // What still has to touch the operand between the copy and the MMA -- LeakyReLU of the input, zeroing of rows outside
 // [0, len) (the convolution's zero padding and the batch-invariant contract), round-to-nearest tf32 and the hi/lo split of
-// the 3xTF32 fp32 emulation -- is an IN-PLACE pass over the staged tile by four "transform" warps: shared memory to shared
-// memory, conflict-free (consecutive lanes = consecutive 16 B).
+// the 3xTF32 fp32 emulation -- is an IN-PLACE pass over the staged tile by four "transform" warps.
 // HBM therefore holds plain activation values (fp32, or bf16 in the bf16 mode): residuals stay exact, one copy per tensor.
 //
-// Roles (448 threads): warps 0-7 two consumer warpgroups (wgmma issue for rows [64 w, 64 w + 64) of every 128-row accumulator,
-// fp32 accumulators in registers, epilogue), 8-11 transform, 12 A loader (one lane), 13 weight loader (one lane).  mbarrier
-// pipelines: a_full (copy landed) -> a_ready (transformed) -> a_empty (every consumer warp has seen the MMAs that read the stage
-// complete), b_full / b_empty.  Persistent CTAs, static round-robin tile order.
+// The roles, their mbarrier ring and their code (x loader, transform warps, weight loader, the consumers' per-tap wgmma chain and
+// one-behind release) are gp_pipeline.cuh, shared with resblock_gp.cu; this kernel adds the tile order and the epilogue (consumer
+// warps: rows [64 w, 64 w + 64) of every 128-row accumulator, fp32 accumulators in registers).  Persistent CTAs, static
+// round-robin tile order.
 //
 // out[b, m*rate + n / CoutR, n % CoutR] = epi( bias[n] + sum_j sum_ci w[j][ci][n] * act_in(x[b, m + (j-(K-1)/2)*dil, ci]) )
 // rate > 1 is the polyphase form of ConvTranspose1d (packing.polyphase_pack): the GEMM's N = rate * CoutR columns are the
 // `rate` output phases of each input row.  Replaces hifigan/models.py:50-57 (ResBlock1 convs), :116 (conv_pre), :118-119 (ups).
 #include "ev_common.cuh"
-#include "tc_common.cuh"
+#include "gp_pipeline.cuh"
 
 namespace ev {
 namespace gp {
 
-using namespace tc;
+using namespace gpl;
 
-constexpr int NCW = 8;                       // consumer warps (two warpgroups)
-constexpr int NTW = 4;                       // transform warps
-constexpr int W_XFORM = NCW;                 // warps 8..11
-constexpr int W_ALOAD = W_XFORM + NTW;       // 12
-constexpr int W_BLOAD = W_ALOAD + 1;         // 13
-constexpr int GP_THREADS = (W_BLOAD + 1) * 32; // 448
-constexpr int MAX_A = 8, MAX_B = 8;
-constexpr int SMEM_HEAD = 1024;              // barriers
-constexpr int XF_UNROLL = 4;
+constexpr int MAX_A = 8;                     // x stages
 
 struct GPlan {
   int BN, mt, kbg, planes;
@@ -73,16 +64,7 @@ __host__ __device__ inline bool make_gplan(const GpConvParams& p, int mode, int 
   const int budget = 227 * 1024 - SMEM_HEAD;
   const int n_cb = (p.Cin + cpg * kbg - 1) / (cpg * kbg);
   const int b_max = n_cb * kmin < MAX_B ? n_cb * kmin : MAX_B;
-  q.a_stages = 2;
-  q.b_stages = b_max < 2 ? b_max : 2;
-  if (q.a_stages * q.a_stage_bytes + q.b_stages * q.b_stage_bytes > budget) return false;
-  auto fits = [&](int a, int b) { return a * q.a_stage_bytes + b * q.b_stage_bytes <= budget; };
-  // the weight ring turns over K times per activation stage: first 4 weight stages, then up to 4 activation stages (they
-  // prefetch ACROSS tiles: the ring is not bounded by the channel blocks of one tile), then whatever still fits
-  while (q.b_stages < b_max && q.b_stages < 4 && fits(q.a_stages, q.b_stages + 1)) ++q.b_stages;
-  while (q.a_stages < 4 && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
-  while (q.b_stages < b_max && fits(q.a_stages, q.b_stages + 1)) ++q.b_stages;
-  while (q.a_stages < MAX_A && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
+  if (!grow_stages(q.a_stage_bytes, q.b_stage_bytes, budget, MAX_A, b_max, &q.a_stages, &q.b_stages)) return false;
   q.tiles_m = (p.L + BM * mt - 1) / (BM * mt);
   q.tiles_n = (p.Cout + BN - 1) / BN;
   q.total_tiles = ng * p.B * q.tiles_m * q.tiles_n;
@@ -91,21 +73,16 @@ __host__ __device__ inline bool make_gplan(const GpConvParams& p, int mode, int 
   return true;
 }
 
-// LeakyReLU for 0 <= slope <= 1 as max(v, v*slope): two instructions (FMUL + FMNMX) instead of compare / multiply / select; same bits
-__device__ __forceinline__ float lrelu_f(float v, float slope) { return fmaxf(v, v * slope); }
-
 // MODE 0: one tf32 MMA per K step; 1: 3xTF32 fp32 emulation (hi/lo planes, three MMAs per K step); 2: bf16 operands,
 // bf16 activations in HBM (8 channels per granule); 3: "bf16x3": fp32 activations in HBM, every operand split
 // into bf16 hi + lo (16 significant bits), three bf16 MMAs per K = 16 step -- an fp32-class result (~1e-5 relative) at
 // half the tensor-core and shared-memory cost of 3xTF32.  Accumulation is fp32 in every mode.  BN = pl.BN, the N tile.
 template <int MODE, int MT, int KBG, int BN>
-__global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_constant__ GpConvParams p, const __grid_constant__ GPlan pl,
-                                                                  const __grid_constant__ GpGroups gs) {
-  constexpr bool SPLIT3 = (MODE == 1);     // 3xTF32: hi / lo tf32 planes
+__global__ void __launch_bounds__(THREADS, 1) conv1d_gp_kernel(const __grid_constant__ GpConvParams p, const __grid_constant__ GPlan pl,
+                                                               const __grid_constant__ GpGroups gs) {
   constexpr bool BF16 = (MODE == 2);       // bf16 activations in HBM, bf16 operands
   constexpr bool X3B = (MODE == 3);        // fp32 activations in HBM, operands split into bf16 hi + lo: three bf16 MMAs per K=16 step
   constexpr bool OP16 = BF16 || X3B;       // the MMA operands are bf16
-  constexpr int BPLANES = (SPLIT3 || X3B) ? 2 : 1;
   constexpr int CPG = BF16 ? 8 : 4;        // channels per 16-byte granule of the activations (HBM and the staged tile)
   constexpr int WCPG = OP16 ? 8 : 4;       // channels per 16-byte granule of the weights
   constexpr int KB = CPG * KBG;
@@ -118,21 +95,10 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int lane = tid & 31;
 
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* a_tiles = smem_raw + SMEM_HEAD;
   uint8_t* b_tiles = a_tiles + pl.a_stages * pl.a_stage_bytes;
-  const uint32_t bar_base = smem_u32(bars);
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_ready = [&](int s) { return bar_base + 8u * (MAX_A + s); };
-  auto a_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (3 * MAX_A + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (3 * MAX_A + MAX_B + s); };
-
-  if (tid == 0) {
-    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), NCW); }
-    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), NCW); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  const Ring<MAX_A> ring{smem_u32(smem_raw)};
+  if (tid == 0) ring.init(pl.a_stages, pl.b_stages);
   __syncthreads();
 
   // Programmatic dependent launch: harmless without the launch attribute.  With it, the next kernel in the stream may start
@@ -143,7 +109,7 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
   const int n_cb = (p.Cin + KB - 1) / KB;
   const int tiles_per_b = pl.tiles_m * pl.tiles_n;
   const int tiles_per_g = p.B * tiles_per_b;  // a launch may carry up to three convolutions of one shape (different taps, dilations,
-  const int gin = p.Cin / CPG;                // weights and tensors): tile -> (convolution, item, row tile, column tile)
+                                              // weights and tensors): tile -> (convolution, item, row tile, column tile)
 
   auto decode = [&](int tile, int& gi, int& b, int& t0, int& n0, int& len) {
     gi = tile / tiles_per_g;
@@ -167,20 +133,13 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
     const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
     // bf16x3: the two K granules of one MMA are two slots apart (hi in the even slots, lo in the odd ones), one K step = 4 slots
     const uint64_t a_desc0 = make_desc(0u, X3B ? 2u * a_lbo : a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
-    const uint32_t a_k8 = (X3B ? 4u : 2u) * a_lbo, b_k8 = 2u * b_lbo;   // bytes per K step
+    const uint32_t a_k8 = (X3B ? 4u : 2u) * a_lbo;   // bytes per K step
     const uint32_t a_lo_off = X3B ? a_lbo : (uint32_t)pl.a_plane_bytes;
     float acc[MT][NA];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
       for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
-    auto release = [&](int sb, int sa) {
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(b_empty(sb));
-        if (sa >= 0) mbar_arrive(a_empty(sa));
-      }
-    };
     int a_cnt = 0, b_cnt = 0;
     for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
       int gi, b, t0, n0, len;
@@ -189,41 +148,19 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
       const GpGroup& G = gs.g[gi];
       const int K = G.K;
       const uint32_t a_tap = (uint32_t)G.dil * 16u;          // bytes per tap shift
-      int prev_sb = -1, prev_sa = -1;
+      OneBehind<MAX_A> rel{ring, lane};
       for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
         const int sa = a_cnt % pl.a_stages;
         const int nk8 = min(KB, p.Cin - cb * KB) / (2 * WCPG);  // MMA K steps: two 16-byte operand granules each
-        mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
+        mbar_wait(ring.a_ready(sa), (a_cnt / pl.a_stages) & 1);
         const uint64_t a_hi0 = desc_advance(a_desc0, smem_u32(a_tiles + sa * pl.a_stage_bytes) + (uint32_t)(wg * 64) * 16u);
         for (int j = 0; j < K; ++j, ++b_cnt) {
           const int sb = b_cnt % pl.b_stages;
-          mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+          mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
           const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-          const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
-          auto k_step = [&](int k8) {
-            const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
-            const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-            const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
-            const uint32_t first = (cb | j | k8) != 0 ? 1u : 0u;
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
-              const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-              mma_step_fixed<MODE, BN>(acc[mt], a_hi, desc_advance(a_hi, a_lo_off), b_hi, b_lo, first);
-            }
-          };
-          wgmma_fence();
-          if (nk8 == NK8) {                        // a full channel block: its NK8 * MT * m MMAs as one chain
-#pragma unroll
-            for (int k8 = 0; k8 < NK8; ++k8) k_step(k8);
-          } else {                                 // the short last block of a C_in that is not a multiple of KB (conv_pre's 80)
-#pragma unroll 1
-            for (int k8 = 0; k8 < nk8; ++k8) k_step(k8);
-          }
-          wgmma_commit();
-          wgmma_wait<1>();          // the previous step's MMAs have completed: its stages may be refilled
-          if (prev_sb >= 0) release(prev_sb, prev_sa);
-          prev_sb = sb;
-          prev_sa = j == K - 1 ? sa : -1;
+          tap_chain<MODE, BN, NK8>(acc, desc_advance(a_hi0, (uint32_t)j * a_tap), a_k8, a_lo_off, b_hi0, (uint32_t)pl.b_plane_bytes, cb | j, nk8);
+          wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
+          rel.step(sb, j == K - 1 ? sa : -1);
         }
       }
 
@@ -292,7 +229,7 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
       };
       epi_load(0);
       wgmma_wait<0>();
-      release(prev_sb, prev_sa);
+      rel.drain();
 #pragma unroll
       for (int ch = 0; ch < NA / 4 / EQ; ++ch) {
         if (ch > 0) epi_load(ch);
@@ -300,94 +237,19 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
       }
     }
   } else if (warp < W_ALOAD) {
-    // ============================ transform warps: in-place pass over the landed A stage =======================
+    // ============================ transform warps ========================================================================
     const int xt = (warp - W_XFORM) * 32 + lane;      // 0..127
-    const bool lrelu = (p.in_act == EV_ACT_LRELU);
-    const float slope = p.in_slope;
     int a_cnt = 0;
     for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
       int gi, b, t0, n0, len;
       decode(tile, gi, b, t0, n0, len);
       if (t0 >= len) continue;
       const int span = (gs.g[gi].K - 1) * gs.g[gi].dil;
-      const int rows_a = BM * MT + span;
-      const int row0 = t0 - span / 2;
-      for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-        const int s = a_cnt % pl.a_stages;
-        const int ngran = min(KB, p.Cin - cb * KB) / CPG;
-        uint8_t* base = a_tiles + s * pl.a_stage_bytes;
-        mbar_wait(a_full(s), (a_cnt / pl.a_stages) & 1);
-        if (X3B) {
-          // fp32 -> bf16 hi + lo in place: the granule pair (2q, 2q+1) = 8 channels becomes [hi of the 8 | lo of the 8], so the hi
-          // plane is the even granule slots and the lo plane the odd ones (descriptor LBO = two slots)
-          for (int q = 0; q < ngran / 2; ++q) {
-            uint8_t* g0 = base + (size_t)(2 * q) * pl.rows_pad * 16;
-            uint8_t* g1 = g0 + (size_t)pl.rows_pad * 16;
-            for (int r = xt; r < rows_a; r += NTW * 32) {
-              const int row = row0 + r;
-              float4 u = make_float4(0.f, 0.f, 0.f, 0.f), w = u;
-              if (row >= 0 && row < len) { u = *reinterpret_cast<const float4*>(g0 + r * 16); w = *reinterpret_cast<const float4*>(g1 + r * 16); }
-              float f[8] = {u.x, u.y, u.z, u.w, w.x, w.y, w.z, w.w};
-              uint32_t hi[4], lo[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float a0 = f[2 * e], a1 = f[2 * e + 1];
-                if (lrelu) { a0 = lrelu_f(a0, slope); a1 = lrelu_f(a1, slope); }
-                hi[e] = pack_bf16(a0, a1);
-                lo[e] = pack_bf16(a0 - __uint_as_float(hi[e] << 16), a1 - __uint_as_float(hi[e] & 0xffff0000u));
-              }
-              *reinterpret_cast<uint4*>(g0 + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-              *reinterpret_cast<uint4*>(g1 + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            }
-          }
-        }
-        for (int g = 0; g < (X3B ? 0 : ngran); ++g) {
-          uint8_t* gb = base + (size_t)g * pl.rows_pad * 16;
-          for (int r0 = 0; r0 < rows_a; r0 += NTW * 32 * XF_UNROLL) {
-            uint4 v[XF_UNROLL];
-#pragma unroll
-            for (int u = 0; u < XF_UNROLL; ++u) {
-              const int r = r0 + u * (NTW * 32) + xt;
-              const int row = row0 + r;
-              v[u] = make_uint4(0u, 0u, 0u, 0u);
-              if (r < rows_a && row >= 0 && row < len) v[u] = *reinterpret_cast<const uint4*>(gb + r * 16);
-            }
-#pragma unroll
-            for (int u = 0; u < XF_UNROLL; ++u) {
-              const int r = r0 + u * (NTW * 32) + xt;
-              if (r >= rows_a) continue;
-              if (BF16) {
-                if (lrelu) {
-                  uint32_t w4[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float lo = lrelu_f(__uint_as_float(w4[e] << 16), slope);
-                    const float hi = lrelu_f(__uint_as_float(w4[e] & 0xffff0000u), slope);
-                    w4[e] = pack_bf16(lo, hi);
-                  }
-                  v[u] = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-                }
-                *reinterpret_cast<uint4*>(gb + r * 16) = v[u];
-              } else {
-                float4 t = make_float4(__uint_as_float(v[u].x), __uint_as_float(v[u].y), __uint_as_float(v[u].z), __uint_as_float(v[u].w));
-                if (lrelu) { t.x = lrelu_f(t.x, slope); t.y = lrelu_f(t.y, slope); t.z = lrelu_f(t.z, slope); t.w = lrelu_f(t.w, slope); }
-                // round to nearest tf32 (the MMA would otherwise truncate the low 13 mantissa bits)
-                const float4 h = make_float4(to_tf32(t.x), to_tf32(t.y), to_tf32(t.z), to_tf32(t.w));
-                *reinterpret_cast<float4*>(gb + r * 16) = h;
-                if (SPLIT3) {
-                  const float4 l = make_float4(to_tf32(t.x - h.x), to_tf32(t.y - h.y), to_tf32(t.z - h.z), to_tf32(t.w - h.w));
-                  *reinterpret_cast<float4*>(gb + pl.a_plane_bytes + r * 16) = l;
-                }
-              }
-            }
-          }
-        }
-        fence_proxy_async();      // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        mbar_arrive(a_ready(s));
-      }
+      transform_tile<MODE, KBG>(ring, a_cnt, pl.a_stages, a_tiles, pl.a_stage_bytes, pl.a_plane_bytes, pl.rows_pad, p.Cin, t0 - span / 2,
+                                           BM * MT + span, len, p.in_act == EV_ACT_LRELU, p.in_slope, xt);
     }
   } else if (warp == W_ALOAD) {
-    // ============================ A loader: one thread, KBG bulk copies per stage ================================
+    // ============================ x loader ===============================================================================
     if (lane == 0) {
       asm volatile("griddepcontrol.wait;" ::: "memory");
       int a_cnt = 0;
@@ -396,60 +258,25 @@ __global__ void __launch_bounds__(GP_THREADS, 1) conv1d_gp_kernel(const __grid_c
         decode(tile, gi, b, t0, n0, len);
         if (t0 >= len) continue;
         const int span = (gs.g[gi].K - 1) * gs.g[gi].dil;
-        const int halo = span / 2, rows_a = BM * MT + span;
-        const int r_lo = max(t0 - halo, 0);
-        const int r_hi = min(t0 - halo + rows_a, len);      // len <= L: never past the plane
-        const uint32_t nbytes = (uint32_t)(r_hi - r_lo) * 16u;
-        const uint32_t roff = (uint32_t)(r_lo - (t0 - halo)) * 16u;
-        const uint8_t* xb = reinterpret_cast<const uint8_t*>(gs.g[gi].x) + ((size_t)b * gin * p.L + r_lo) * 16;
-        for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-          const int s = a_cnt % pl.a_stages;
-          const int ngran = min(KB, p.Cin - cb * KB) / CPG;
-          mbar_wait(a_empty(s), ((a_cnt / pl.a_stages) & 1) ^ 1);
-          mbar_expect_tx(a_full(s), (uint32_t)ngran * nbytes);
-          const uint32_t dst = smem_u32(a_tiles + s * pl.a_stage_bytes) + roff;
-          const uint8_t* src = xb + (size_t)(cb * KBG) * p.L * 16;
-          for (int g = 0; g < ngran; ++g)
-            bulk_g2s(dst + (uint32_t)(g * pl.rows_pad * 16), src + (size_t)g * p.L * 16, nbytes, a_full(s));
-        }
+        load_x_tile<CPG, KBG>(ring, a_cnt, pl.a_stages, a_tiles, pl.a_stage_bytes, pl.rows_pad, gs.g[gi].x, b, p.Cin, p.L, t0 - span / 2,
+                              BM * MT + span, len);
       }
     }
     __syncwarp();
   } else {
     // ============================ weight loader (weights are constants: no dependency wait) ========================
     if (lane == 0) {
-      // w layout: [plane (hi, lo)][N tile of BNp = min(Cout,128)][tap][Cin/WCPG granules][BNp][16 bytes] (fp32 or bf16 granules)
-      const int bnp = p.Cout < 128 ? p.Cout : 128;
-      const int win = p.Cin / WCPG;                                  // weight granules along C_in
-      constexpr int KBGW = KBG * CPG / WCPG;                         // weight granules per pipeline stage
+      const int bnp = p.Cout < 128 ? p.Cout : 128;                   // the packing tile
+      const int win = p.Cin / WCPG;
       int b_cnt = 0;
       for (int tile = blockIdx.x; tile < pl.total_tiles; tile += gridDim.x) {
         int gi, b, t0, n0, len;
         decode(tile, gi, b, t0, n0, len);
         if (t0 >= len) continue;
         const int K = gs.g[gi].K;
-        const size_t plane = (size_t)K * win * p.Cout * 4;          // 4-byte words per plane
         const size_t tile_stride = (size_t)K * win * bnp * 4;       // 4-byte words per packed N tile
         const float* wt = gs.g[gi].w + (size_t)(n0 / bnp) * tile_stride + (size_t)(n0 % bnp) * 4;
-        for (int cb = 0; cb < n_cb; ++cb) {
-          const int ngran = min(KB, p.Cin - cb * KB) / WCPG;          // weight granules of this stage
-          for (int j = 0; j < K; ++j, ++b_cnt) {
-            const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_empty(sb), ((b_cnt / pl.b_stages) & 1) ^ 1);
-            mbar_expect_tx(b_full(sb), (uint32_t)(BPLANES * ngran * BN * 16));
-            const uint32_t dst = smem_u32(b_tiles + sb * pl.b_stage_bytes);
-            const float* src = wt + ((size_t)j * win + (size_t)cb * KBGW) * bnp * 4;
-            if (BN == bnp) {
-              bulk_g2s(dst, src, (uint32_t)(ngran * BN * 16), b_full(sb));
-              if (BPLANES == 2) bulk_g2s(dst + (uint32_t)pl.b_plane_bytes, src + plane, (uint32_t)(ngran * BN * 16), b_full(sb));
-            } else {
-              for (int g = 0; g < ngran; ++g) {
-                bulk_g2s(dst + (uint32_t)(g * BN * 16), src + (size_t)g * bnp * 4, (uint32_t)(BN * 16), b_full(sb));
-                if (BPLANES == 2) bulk_g2s(dst + (uint32_t)(pl.b_plane_bytes + g * BN * 16), src + plane + (size_t)g * bnp * 4, (uint32_t)(BN * 16), b_full(sb));
-              }
-            }
-          }
-        }
+        load_w_tile<MODE, KBG, BN>(ring, b_cnt, pl.b_stages, b_tiles, pl.b_stage_bytes, pl.b_plane_bytes, wt, K, p.Cin, p.Cout, bnp);
       }
     }
     __syncwarp();
@@ -640,7 +467,7 @@ static int validate_gp(const GpConvParams& p, int mode) {
 
 // K granules per stage decide the order of the (channel block, tap, k-step) reduction, so they are a function of the layer
 // shape alone (never of batch or length): 8 outside the 3xTF32 mode if a one-accumulator tile fits with them, else 4.
-static int gp_shape_kbg(const GpConvParams& p, int mode) {
+int gp_shape_kbg(const GpConvParams& p, int mode) {
   gp::GPlan pl;
   const int bn_max = p.Cout <= 128 ? p.Cout : 128;
   return (mode != 1 && gp::make_gplan(p, mode, bn_max, 1, 8, &pl)) ? 8 : 4;
@@ -753,7 +580,7 @@ static int dispatch_gp(const GpConvParams& p, const gp::GPlan& pl, const GpGroup
   EV_CHECK_ARG(k, "conv1d_gp: no kernel for mode %d, KBG %d, MT %d, BN %d", mode, pl.kbg, pl.mt, pl.BN);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  return launch("conv1d_gp_kernel", k, (unsigned)grid, gp::GP_THREADS, pl.smem_total, st, p, pl, gs);
+  return launch("conv1d_gp_kernel", k, (unsigned)grid, gpl::THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 int launch_conv1d_gp(const GpConvParams& p, int mode, cudaStream_t st) {
@@ -810,11 +637,8 @@ static int plan_group(const GpConvParams* ps, int n, int mode, GpGroups* gs_out,
   gp::GPlan& pl = *pl_out;
   int kbg = 0;
   EV_CHECK_ARG(ps && group_shapes_match(ps, n, mode, &kbg), "conv1d_gp group: the %d convolutions do not share a launch shape", n);
-  // heaviest member first: with static round-robin tiles the CTAs that take a second (third) tile then take a light one
-  int order[3] = {0, 1, 2};
-  for (int i = 0; i < n; ++i)
-    for (int j = i + 1; j < n; ++j)
-      if (ps[order[j]].K > ps[order[i]].K) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
+  int order[3];
+  gpl::heaviest_first(ps, n, order);
   gs = GpGroups{};
   gs.ng = n;
   int ksum = 0, span = 0, kmin = 1 << 30;

@@ -158,6 +158,7 @@ bool gp_group_supported(const GpConvParams* ps, int n, int mode);
 int debug_gp_group_plan(const GpConvParams* ps, int n, int mode, int* v11);
 int gp_solo_tiles(const GpConvParams& p, int mode);       // tiles of the convolution's own launch (0 if it cannot be planned)
 int debug_gp_plan(const GpConvParams& p, int mode, int* v11);
+int gp_shape_kbg(const GpConvParams& p, int mode);     // K granules per stage: a function of the layer shape, it fixes the reduction order
 // fp32 in[b*sb + t*st + c*sc] -> GP (fp32, or bf16 when bf16 != 0)
 int launch_to_gp(const float* in, long long sb, long long st_, long long sc, void* out, int B, int L, int C, int bf16, cudaStream_t st);
 // One ResBlock1 layer  out = [acc]( x + c2(lrelu(c1(lrelu(x), dil)), 1) )  as one kernel on granule-planar activations

@@ -7,27 +7,24 @@
 // re-read hits L2) and the launches halve.  Same reduction orders and roundings as two conv1d_gp launches: BITWISE equal to them.
 //
 // Tile = R = 128*MT - (K-1) output rows.  c1 computes MT accumulators for the 128*MT xt rows [t0 - (K-1)/2, ...) from a staged x
-// tile of 128*MT + (K-1)*d rows (bulk copies + transform warps, as in conv1d_gp.cu); c2 computes MT accumulators from the xt
+// tile of 128*MT + (K-1)*d rows (the x loader and transform warps of gp_pipeline.cuh); c2 computes MT accumulators from the xt
 // tile (its last K-1 rows per tile are surplus and discarded).  xt rows outside [0, len) are written as zeros: the reference
 // pads c2's input with zeros, it does not convolve c1 over the padding.
 //
-// Roles (448 threads): warps 0-7 two consumer warpgroups -- per tile: c1 (wgmma, accumulators in registers), epi1 into the xt tile,
-// a named barrier over both warpgroups, c2 over the xt tile, epi2 (+ b2 + x, accumulate modes) to HBM; warps 8-11 transform the
-// landed x stages in place; warp 12 x loader; warp 13 weight loader (w1 then w2 of every tile, the order the consumers read them).
-// The x ring and the weight ring prefetch across tiles, so the loads of tile i+1 run under c2 and the epilogues of tile i.
+// The roles and their code are gp_pipeline.cuh's, shared with conv1d_gp.cu: the consumer warpgroups run, per tile, c1 (one wgmma
+// chain per tap, accumulators in registers), epi1 into the xt tile, a named barrier over both warpgroups, c2 over the xt tile
+// (the same chains and one-behind release, with no x stage to hand back), epi2 (+ b2 + x, accumulate modes) to HBM; the weight
+// loader streams w1 then w2 of every tile, the order the consumers read them.  The x ring and the weight ring prefetch across
+// tiles, so the loads of tile i+1 run under c2 and the epilogues of tile i.
 #include "ev_common.cuh"
-#include "tc_common.cuh"
+#include "gp_pipeline.cuh"
 
 namespace ev {
 namespace gpp {
 
-using namespace tc;
+using namespace gpl;
 
-constexpr int NCW = 8, NTW = 4;
-constexpr int W_XFORM = 8, W_ALOAD = 12, W_BLOAD = 13;
-constexpr int GPP_THREADS = 14 * 32;
-constexpr int MAX_A = 6, MAX_B = 8;
-constexpr int SMEM_HEAD = 1024;
+constexpr int MAX_A = 6;                     // x stages
 
 struct PPlan {
   int mt, kbg;
@@ -63,13 +60,7 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
   q.b_plane_bytes = (kbg * cpg / ocpg) * C * 16;
   q.b_stage_bytes = splitp * q.b_plane_bytes;
   const int budget = 227 * 1024 - SMEM_HEAD - q.a2_bytes;
-  q.a_stages = 2; q.b_stages = 2;
-  auto fits = [&](int a, int b) { return a * q.x_stage_bytes + b * q.b_stage_bytes <= budget; };
-  if (!fits(2, 2)) return false;
-  while (q.b_stages < 4 && fits(q.a_stages, q.b_stages + 1)) ++q.b_stages;
-  while (q.a_stages < 4 && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
-  while (q.b_stages < MAX_B && fits(q.a_stages, q.b_stages + 1)) ++q.b_stages;
-  while (q.a_stages < MAX_A && fits(q.a_stages + 1, q.b_stages)) ++q.a_stages;
+  if (!grow_stages(q.x_stage_bytes, q.b_stage_bytes, budget, MAX_A, MAX_B, &q.a_stages, &q.b_stages)) return false;
   q.acc_cols = mt * C;
   q.tiles_m = (p.L + q.R - 1) / q.R;
   q.total_tiles = p.B * q.tiles_m;
@@ -78,16 +69,12 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
   return true;
 }
 
-// LeakyReLU for 0 <= slope <= 1 as max(v, v*slope): two instructions (FMUL + FMNMX) instead of compare / multiply / select; same bits
-__device__ __forceinline__ float lrelu_f(float v, float slope) { return fmaxf(v, v * slope); }
-
 // MODE as conv1d_gp.cu: 0 tf32, 1 3xTF32, 2 bf16 activations + operands, 3 bf16x3 on fp32 activations.  C = p.C, the channels.
 template <int MODE, int MT, int KBG, int C>
-__global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __grid_constant__ GpPairParams p, const __grid_constant__ PPlan pl,
+__global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_constant__ GpPairParams p, const __grid_constant__ PPlan pl,
                                                                      const __grid_constant__ GpPairGroups gs) {
   constexpr bool SPLIT3 = (MODE == 1), BF16 = (MODE == 2), X3B = (MODE == 3);
   constexpr bool OP16 = BF16 || X3B;
-  constexpr int SPL = (SPLIT3 || X3B) ? 2 : 1;
   constexpr int CPG = BF16 ? 8 : 4;
   constexpr int OCPG = OP16 ? 8 : 4;
   constexpr int KB = CPG * KBG;
@@ -102,22 +89,11 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
 
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* a2_tile = smem_raw + SMEM_HEAD;
   uint8_t* x_tiles = a2_tile + pl.a2_bytes;
   uint8_t* b_tiles = x_tiles + pl.a_stages * pl.x_stage_bytes;
-  const uint32_t bar_base = smem_u32(bars);
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_ready = [&](int s) { return bar_base + 8u * (MAX_A + s); };
-  auto a_empty = [&](int s) { return bar_base + 8u * (2 * MAX_A + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (3 * MAX_A + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (3 * MAX_A + MAX_B + s); };
-
-  if (tid == 0) {
-    for (int s = 0; s < pl.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_ready(s), NTW * 32); mbar_init(a_empty(s), NCW); }
-    for (int s = 0; s < pl.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), NCW); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  const Ring<MAX_A> ring{smem_u32(smem_raw)};
+  if (tid == 0) ring.init(pl.a_stages, pl.b_stages);
   __syncthreads();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
@@ -153,13 +129,6 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
       for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
-    auto release = [&](int sb, int sa) {
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(b_empty(sb));
-        if (sa >= 0) mbar_arrive(a_empty(sa));
-      }
-    };
     int a_cnt = 0, b_cnt = 0;
     for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
       int gi, b, t0;
@@ -180,43 +149,27 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       };
       // ---- c1 over the staged x tile
       {
-        int prev_sb = -1, prev_sa = -1;
+        OneBehind<MAX_A> rel{ring, lane};
         // Not unrolled, not peeled: with C and the K steps constants the compiler would otherwise copy the channel-block and tap
         // loops, and every copy adds a wgmma.wait_group site (tests/test_wgmma_pipeline_sass.py counts them).
 #pragma unroll 1
         for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
           const int sa = a_cnt % pl.a_stages;
-          mbar_wait(a_ready(sa), (a_cnt / pl.a_stages) & 1);
+          mbar_wait(ring.a_ready(sa), (a_cnt / pl.a_stages) & 1);
           const uint64_t x0 = desc_advance(x_desc0, smem_u32(x_tiles + sa * pl.x_stage_bytes) + (uint32_t)(wg * 64) * 16u);
 #pragma unroll 1
           for (int j = 0; j < K; ++j, ++b_cnt) {
             const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+            mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            const uint64_t xj = desc_advance(x0, (uint32_t)(j * dil) * 16u);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < NK; ++k) {          // the channel block's NK * MT * m MMAs: one chain
-              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-              const uint64_t a_k = desc_advance(xj, (uint32_t)k * x_k);
-              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
-#pragma unroll
-              for (int mt = 0; mt < MT; ++mt) {
-                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma_step_fixed<MODE, C>(acc[mt], a_hi, desc_advance(a_hi, x_lo_off), b_hi, b_lo, first);
-              }
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (prev_sb >= 0) release(prev_sb, prev_sa);
-            prev_sb = sb;
-            prev_sa = j == K - 1 ? sa : -1;
+            tap_chain<MODE, C, NK>(acc, desc_advance(x0, (uint32_t)(j * dil) * 16u), x_k, x_lo_off, b0, (uint32_t)pl.b_plane_bytes, cb | j);
+            wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
+            rel.step(sb, j == K - 1 ? sa : -1);
           }
         }
         load_b1(0);
         wgmma_wait<0>();
-        release(prev_sb, prev_sa);
+        rel.drain();
       }
       // ---- epi1: acc1 + b1 -> lrelu -> operand format -> xt tile.  Both warpgroups' c2 of the previous tile read the whole
       // ---- xt tile (their taps overlap the other's rows), so the tile is only rewritten once both have finished it.
@@ -309,38 +262,23 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       };
       // ---- c2 over the xt tile
       {
-        int prev_sb = -1;
+        OneBehind<MAX_A> rel{ring, lane};
 #pragma unroll 1                            // as in c1
         for (int cb = 0; cb < n_cb; ++cb) {
           const uint64_t a0 = desc_advance(a2_desc0, (uint32_t)(cb * KBGW) * a2_lbo);
 #pragma unroll 1
           for (int j = 0; j < K; ++j, ++b_cnt) {
             const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
+            mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            const uint64_t aj = desc_advance(a0, (uint32_t)j * 16u);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < NK; ++k) {
-              const uint64_t b_hi = desc_advance(b0, (uint32_t)k * 2u * b_lbo);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-              const uint64_t a_k = desc_advance(aj, (uint32_t)k * 2u * a2_lbo);
-              const uint32_t first = (cb | j | k) != 0 ? 1u : 0u;
-#pragma unroll
-              for (int mt = 0; mt < MT; ++mt) {
-                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma_step_fixed<MODE, C>(acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a2_plane_bytes), b_hi, b_lo, first);
-              }
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (prev_sb >= 0) release(prev_sb, -1);
-            prev_sb = sb;
+            tap_chain<MODE, C, NK>(acc, desc_advance(a0, (uint32_t)j * 16u), 2u * a2_lbo, (uint32_t)pl.a2_plane_bytes, b0, (uint32_t)pl.b_plane_bytes, cb | j);
+            wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
+            rel.step(sb, -1);
           }
         }
         epi_load(0);
         wgmma_wait<0>();
-        release(prev_sb, -1);
+        rel.drain();
       }
 #pragma unroll
       for (int q = 0; q < NA / 4; ++q) {
@@ -349,73 +287,18 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
       }
     }
   } else if (warp < W_ALOAD) {
-    // ============================ transform warps: in-place pass over the landed x stage =======================
+    // ============================ transform warps ========================================================================
     const int xt = (warp - W_XFORM) * 32 + lane;
-    const float slope = p.slope;
     int a_cnt = 0;
     for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
       int gi, b, t0;
       const int len = tile_len(tile, gi, b, t0);
       const int span = (gs.g[gi].K - 1) * gs.g[gi].dil;
-      const int rows1 = BM * MT + span;
-      const int row0 = t0 - (gs.g[gi].K - 1) / 2 - span / 2;
-      for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-        const int s = a_cnt % pl.a_stages;
-        const int ngran = min(KB, C - cb * KB) / CPG;
-        uint8_t* base = x_tiles + s * pl.x_stage_bytes;
-        mbar_wait(a_full(s), (a_cnt / pl.a_stages) & 1);
-        if (X3B) {
-          for (int q = 0; q < ngran / 2; ++q) {
-            uint8_t* g0 = base + (size_t)(2 * q) * pl.rows1_pad * 16;
-            uint8_t* g1 = g0 + (size_t)pl.rows1_pad * 16;
-            for (int r = xt; r < rows1; r += NTW * 32) {
-              const int row = row0 + r;
-              float4 u = make_float4(0.f, 0.f, 0.f, 0.f), w = u;
-              if (row >= 0 && row < len) { u = *reinterpret_cast<const float4*>(g0 + r * 16); w = *reinterpret_cast<const float4*>(g1 + r * 16); }
-              const float f[8] = {u.x, u.y, u.z, u.w, w.x, w.y, w.z, w.w};
-              uint32_t hi[4], lo[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float a0 = lrelu_f(f[2 * e], slope), a1 = lrelu_f(f[2 * e + 1], slope);
-                hi[e] = pack_bf16(a0, a1);
-                lo[e] = pack_bf16(a0 - __uint_as_float(hi[e] << 16), a1 - __uint_as_float(hi[e] & 0xffff0000u));
-              }
-              *reinterpret_cast<uint4*>(g0 + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-              *reinterpret_cast<uint4*>(g1 + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            }
-          }
-        } else {
-          for (int g = 0; g < ngran; ++g) {
-            uint8_t* gb = base + (size_t)g * pl.rows1_pad * 16;
-            for (int r = xt; r < rows1; r += NTW * 32) {
-              const int row = row0 + r;
-              uint4 v = make_uint4(0u, 0u, 0u, 0u);
-              if (row >= 0 && row < len) v = *reinterpret_cast<const uint4*>(gb + r * 16);
-              if (BF16) {
-                uint32_t w4[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  w4[e] = pack_bf16(lrelu_f(__uint_as_float(w4[e] << 16), slope), lrelu_f(__uint_as_float(w4[e] & 0xffff0000u), slope));
-                *reinterpret_cast<uint4*>(gb + r * 16) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-              } else {
-                float4 t = make_float4(lrelu_f(__uint_as_float(v.x), slope), lrelu_f(__uint_as_float(v.y), slope), lrelu_f(__uint_as_float(v.z), slope),
-                                       lrelu_f(__uint_as_float(v.w), slope));
-                const float4 h = make_float4(to_tf32(t.x), to_tf32(t.y), to_tf32(t.z), to_tf32(t.w));
-                *reinterpret_cast<float4*>(gb + r * 16) = h;
-                if (SPLIT3) {
-                  const float4 l = make_float4(to_tf32(t.x - h.x), to_tf32(t.y - h.y), to_tf32(t.z - h.z), to_tf32(t.w - h.w));
-                  *reinterpret_cast<float4*>(gb + pl.x_plane_bytes + r * 16) = l;
-                }
-              }
-            }
-          }
-        }
-        fence_proxy_async();
-        mbar_arrive(a_ready(s));
-      }
+      transform_tile<MODE, KBG>(ring, a_cnt, pl.a_stages, x_tiles, pl.x_stage_bytes, pl.x_plane_bytes, pl.rows1_pad, C,
+                                t0 - (gs.g[gi].K - 1) / 2 - span / 2, BM * MT + span, len, true, p.slope, xt);
     }
   } else if (warp == W_ALOAD) {
-    // ============================ x loader ===========================================================================
+    // ============================ x loader ===============================================================================
     if (lane == 0) {
       asm volatile("griddepcontrol.wait;" ::: "memory");
       int a_cnt = 0;
@@ -423,47 +306,19 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
         int gi, b, t0;
         const int len = tile_len(tile, gi, b, t0);
         const int span = (gs.g[gi].K - 1) * gs.g[gi].dil;
-        const int rows1 = BM * MT + span;
-        const int row0 = t0 - (gs.g[gi].K - 1) / 2 - span / 2;
-        const int r_lo = max(row0, 0), r_hi = min(row0 + rows1, len);
-        const uint32_t nbytes = (uint32_t)(r_hi - r_lo) * 16u, roff = (uint32_t)(r_lo - row0) * 16u;
-        const uint8_t* xb = reinterpret_cast<const uint8_t*>(gs.g[gi].x) + ((size_t)b * gC * p.L + r_lo) * 16;
-        for (int cb = 0; cb < n_cb; ++cb, ++a_cnt) {
-          const int s = a_cnt % pl.a_stages;
-          const int ngran = min(KB, C - cb * KB) / CPG;
-          mbar_wait(a_empty(s), ((a_cnt / pl.a_stages) & 1) ^ 1);
-          mbar_expect_tx(a_full(s), (uint32_t)ngran * nbytes);
-          const uint32_t dst = smem_u32(x_tiles + s * pl.x_stage_bytes) + roff;
-          const uint8_t* src = xb + (size_t)(cb * KBG) * p.L * 16;
-          for (int g = 0; g < ngran; ++g) bulk_g2s(dst + (uint32_t)(g * pl.rows1_pad * 16), src + (size_t)g * p.L * 16, nbytes, a_full(s));
-        }
+        load_x_tile<CPG, KBG>(ring, a_cnt, pl.a_stages, x_tiles, pl.x_stage_bytes, pl.rows1_pad, gs.g[gi].x, b, C, p.L,
+                              t0 - (gs.g[gi].K - 1) / 2 - span / 2, BM * MT + span, len);
       }
     }
     __syncwarp();
   } else {
     // ============================ weight loader: the consumers' order  w1(i), w2(i), w1(i+1), ... ====================
     if (lane == 0) {
-      const int win = C / OCPG;
       int b_cnt = 0;
-      auto stream = [&](const float* w, int K) {
-        const size_t plane = (size_t)K * win * C * 4;        // 4-byte words per plane
-        for (int cb = 0; cb < n_cb; ++cb) {
-          const int ngran = min(KB, C - cb * KB) / OCPG;
-          for (int j = 0; j < K; ++j, ++b_cnt) {
-            const int sb = b_cnt % pl.b_stages;
-            mbar_wait(b_empty(sb), ((b_cnt / pl.b_stages) & 1) ^ 1);
-            mbar_expect_tx(b_full(sb), (uint32_t)(SPL * ngran * C * 16));
-            const uint32_t dst = smem_u32(b_tiles + sb * pl.b_stage_bytes);
-            const float* src = w + ((size_t)j * win + (size_t)cb * KBGW) * C * 4;
-            bulk_g2s(dst, src, (uint32_t)(ngran * C * 16), b_full(sb));
-            if (SPL == 2) bulk_g2s(dst + (uint32_t)pl.b_plane_bytes, src + plane, (uint32_t)(ngran * C * 16), b_full(sb));
-          }
-        }
-      };
       for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
         const GpPairGroup& G = gs.g[group_of(tile)];
-        stream(G.w1, G.K);
-        stream(G.w2, G.K);
+        load_w_tile<MODE, KBG, C>(ring, b_cnt, pl.b_stages, b_tiles, pl.b_stage_bytes, pl.b_plane_bytes, G.w1, G.K, C, C, C);
+        load_w_tile<MODE, KBG, C>(ring, b_cnt, pl.b_stages, b_tiles, pl.b_stage_bytes, pl.b_plane_bytes, G.w2, G.K, C, C, C);
       }
     }
     __syncwarp();
@@ -472,17 +327,16 @@ __global__ void __launch_bounds__(GPP_THREADS, 1) resblock_gp_kernel(const __gri
 
 }  // namespace gpp
 
-// K granules per stage: the same function of the layer shape as conv1d_gp.cu's (it fixes the reduction order, and the fused layer
-// must stay bitwise equal to the two launches it replaces).
+// K granules per stage: conv1d_gp.cu's function of the layer shape (it fixes the reduction order, and the fused layer must stay
+// bitwise equal to the two launches it replaces).
 static int pair_shape_kbg(const GpPairParams& p, int mode) {
   GpConvParams q{};
-  q.B = 1; q.L = 128; q.Cin = p.C; q.Cout = p.C; q.K = p.K; q.dil = p.dil; q.rate = 1;
-  int v[11];
-  return debug_gp_plan(q, mode, v) == EV_OK ? v[2] : 4;
+  q.Cin = p.C; q.Cout = p.C; q.K = p.K; q.dil = p.dil; q.rate = 1;
+  return gp_shape_kbg(q, mode);
 }
 
 static bool plan_pair(const GpPairParams& p, int mode, gpp::PPlan* out) {
-  if (p.B <= 0 || p.L <= 0 || (p.C != 32 && p.C != 64 && p.C != 128) || !(p.K & 1) || p.dil < 1) return false;
+  if (mode < 0 || mode > 3 || p.B <= 0 || p.L <= 0 || (p.C != 32 && p.C != 64 && p.C != 128) || !(p.K & 1) || p.dil < 1) return false;
   if (mode >= 2 && p.C % 16) return false;
   if (p.x == p.out) return false;
   const int kbg = pair_shape_kbg(p, mode);
@@ -542,7 +396,7 @@ static int dispatch_pair(const GpPairParams& p, const gpp::PPlan& pl, const GpPa
   EV_CHECK_ARG(k, "resblock_gp: no kernel for mode %d, KBG %d, MT %d, C %d", mode, pl.kbg, pl.mt, p.C);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  return launch("resblock_gp_kernel", k, (unsigned)grid, gpp::GPP_THREADS, pl.smem_total, st, p, pl, gs);
+  return launch("resblock_gp_kernel", k, (unsigned)grid, gpl::THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 void preload_resblock_gp() {      // see preload_conv1d_gp
@@ -587,10 +441,8 @@ static bool plan_pair_group(const GpPairParams* ps, int n, int mode, GpPairGroup
     span1 = (q.K - 1) * q.dil > span1 ? (q.K - 1) * q.dil : span1;
     kmax = q.K > kmax ? q.K : kmax;
   }
-  int order[3] = {0, 1, 2};
-  for (int i = 0; i < n; ++i)
-    for (int j = i + 1; j < n; ++j)
-      if (ps[order[j]].K > ps[order[i]].K) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
+  int order[3];
+  gpl::heaviest_first(ps, n, order);
   const int nsm = sm_count();
   for (int mt = 4; mt >= 2; mt >>= 1) {
     gpp::PPlan pl;

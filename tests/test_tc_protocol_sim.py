@@ -7,8 +7,9 @@ producers (in groups) or bulk-copy loader + transform warps, weight loader, the 
 barriers with the hardware's semantics (arrival count, phase bit, `try_wait.parity(P)` passes iff the current phase parity
 != P; a wgmma reads its shared-memory operands until `wgmma.wait_group` has seen it complete, which the consumers do one
 step after issuing it) under many random schedules, and checks: no deadlock, every slot holds the expected contents when it
-is read, no slot is overwritten before its last reader is done.  The role loops are transcribed from the kernels; the
-planner (ring depths, groups) is the real one.
+is read, no slot is overwritten before its last reader is done.  The role loops are transcribed from the kernels (for the two
+granule-planar kernels, from the roles they share in csrc/gp_pipeline.cuh: one model of the x loader and the transform warps,
+and `mma_steps` for the consumers' tap chains with their one-behind release); the planner (ring depths, groups) is the real one.
 """
 import ctypes
 import random
@@ -206,21 +207,19 @@ def test_conv_protocol_model_catches_the_round1_bugs():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# conv1d_gp.cu: A loader (bulk copies) -> a_full -> transform warps (in place) -> a_ready -> MMA -> a_empty -> A loader
+# gp_pipeline.cuh (conv1d_gp.cu, resblock_gp.cu): x loader (bulk copies) -> a_full -> transform warps (in place) -> a_ready ->
+# MMA -> a_empty -> x loader
 # ------------------------------------------------------------------------------------------------------------------
 NTW = 4
 
 
-def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, early_release=False):
-    """tiles: list of booleans (True = active tile, False = padding tile that every role skips); K: taps, or taps per tile (a
-    grouped launch)."""
-    sim = Sim(seed)
-    taps = (lambda ti: K[ti]) if isinstance(K, (list, tuple)) else (lambda ti: K)     # grouped launch: the taps differ from tile to tile
+def add_x_roles(sim, tiles, n_cb, a_stages):
+    """The x loader (load_x_tile) and the four transform warps (transform_tile) over `tiles` (booleans: False = a padding tile that
+    every role skips); returns the barriers the consumers wait on and release, a_ready and a_empty.  Slot ("A", s) holds
+    ("raw", tile, block) once the bulk copies land and ("op", tile, block) once transformed."""
     a_full = [Bar(1) for _ in range(a_stages)]
     a_ready = [Bar(NTW) for _ in range(a_stages)]           # one arrival per transform warp here (the kernel: per thread)
     a_empty = [Bar(NCONS_WARPS) for _ in range(a_stages)]
-    b_full = [Bar(1) for _ in range(b_stages)]
-    b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
 
     def aloader():
         a_cnt = 0
@@ -242,11 +241,29 @@ def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, early_release=False):
             for cb in range(n_cb):
                 s = a_cnt % a_stages
                 yield ("wait", a_full[s], (a_cnt // a_stages) & 1)
-                yield ("read", ("A", s), ("raw", ti, cb) if w == 0 else sim.slots.get(("A", s)))
                 if w == 0:
+                    yield ("read", ("A", s), ("raw", ti, cb))
                     yield ("write", ("A", s), ("op", ti, cb))
                 yield ("arrive", a_ready[s])
                 a_cnt += 1
+
+    sim.add("aloader", aloader())
+    for w in range(NTW):
+        sim.add("xform%d" % w, xform(w))
+    return a_ready, a_empty
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# conv1d_gp.cu: per tile, K taps per channel block
+# ------------------------------------------------------------------------------------------------------------------
+def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, early_release=False):
+    """tiles: list of booleans (True = active tile, False = padding tile that every role skips); K: taps, or taps per tile (a
+    grouped launch)."""
+    sim = Sim(seed)
+    taps = (lambda ti: K[ti]) if isinstance(K, (list, tuple)) else (lambda ti: K)     # grouped launch: the taps differ from tile to tile
+    a_ready, a_empty = add_x_roles(sim, tiles, n_cb, a_stages)
+    b_full = [Bar(1) for _ in range(b_stages)]
+    b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
 
     def bloader():
         b_cnt = 0
@@ -278,9 +295,6 @@ def sim_gp(seed, tiles, n_cb, K, a_stages, b_stages, early_release=False):
                 a_cnt += 1
             yield from mma_steps(steps, b_empty, early_release)
 
-    sim.add("aloader", aloader())
-    for w in range(NTW):
-        sim.add("xform%d" % w, xform(w))
     sim.add("bloader", bloader())
     for w in range(NCONS_WARPS):
         sim.add("consumer%d" % w, consumer())
@@ -455,34 +469,10 @@ def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages, early_release=False):
     over the xt tile; the weight loader streams w1 then w2 of every tile."""
     sim = Sim(seed)
     taps = (lambda ti: K[ti]) if isinstance(K, (list, tuple)) else (lambda ti: K)     # grouped launch: the taps differ from tile to tile
-    a_full = [Bar(1) for _ in range(a_stages)]
-    a_ready = [Bar(NTW) for _ in range(a_stages)]
-    a_empty = [Bar(NCONS_WARPS) for _ in range(a_stages)]
+    a_ready, a_empty = add_x_roles(sim, [True] * n_tiles, n_cb, a_stages)
     b_full = [Bar(1) for _ in range(b_stages)]
     b_empty = [Bar(NCONS_WARPS) for _ in range(b_stages)]
     named = Bar(NCONS_WARPS)                                # bar.sync 1, 256
-
-    def aloader():
-        a_cnt = 0
-        for ti in range(n_tiles):
-            for cb in range(n_cb):
-                s = a_cnt % a_stages
-                yield ("wait", a_empty[s], ((a_cnt // a_stages) & 1) ^ 1)
-                yield ("write", ("X", s), ("raw", ti, cb))
-                yield ("arrive", a_full[s])
-                a_cnt += 1
-
-    def xform(w):
-        a_cnt = 0
-        for ti in range(n_tiles):
-            for cb in range(n_cb):
-                s = a_cnt % a_stages
-                yield ("wait", a_full[s], (a_cnt // a_stages) & 1)
-                if w == 0:
-                    yield ("read", ("X", s), ("raw", ti, cb))
-                    yield ("write", ("X", s), ("op", ti, cb))
-                yield ("arrive", a_ready[s])
-                a_cnt += 1
 
     def bloader():
         b_cnt = 0
@@ -512,7 +502,7 @@ def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages, early_release=False):
                 for j in range(taps(ti)):
                     sb = b_cnt % b_stages
                     waits = ([(a_ready[sa], (a_cnt // a_stages) & 1)] if j == 0 else []) + [(b_full[sb], (b_cnt // b_stages) & 1)]
-                    steps.append((waits, [(("X", sa), ("op", ti, cb)), (("B", sb), (1, ti, cb, j))],
+                    steps.append((waits, [(("A", sa), ("op", ti, cb)), (("B", sb), (1, ti, cb, j))],
                                   [b_empty[sb]] + ([a_empty[sa]] if j == taps(ti) - 1 else [])))
                     b_cnt += 1
                 a_cnt += 1
@@ -529,9 +519,6 @@ def sim_pair(seed, n_tiles, n_cb, K, a_stages, b_stages, early_release=False):
                     b_cnt += 1
             yield from mma_steps(steps, b_empty, early_release)
 
-    sim.add("aloader", aloader())
-    for w in range(NTW):
-        sim.add("xform%d" % w, xform(w))
     sim.add("bloader", bloader())
     for w in range(NCONS_WARPS):
         sim.add("consumer%d" % w, consumer(w))
