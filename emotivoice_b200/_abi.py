@@ -60,6 +60,8 @@ SIGNATURES = {
     "ev_phase2_workspace_bytes": (_sz, [_vp, _i, _i]),
     "ev_am_phase1": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_am_phase1_prosody": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ev_am_phase1_controls": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   _sz, _vp]),
     "ev_am_phase2": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_vocoder": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_wav_to_pcm16": (_i, [_vp, _vp, _sz, _vp]),
@@ -85,6 +87,7 @@ SIGNATURES = {
     "ev_op_attention_tc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ev_op_gauss_upsample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ev_op_duration_scan": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "ev_op_duration_scan_controls": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "ev_op_gauss_upsample_centers": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "ev_op_layernorm_embed": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "ev_op_cond_bias": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),

@@ -425,28 +425,33 @@ int launch_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T
 // ---------------------------------------------------------------------------------------------
 // x += pitch_embed(p) + energy_embed(e): two Conv1d(1 -> C, k=K, pad=(K-1)/2) on the predicted
 // scalar tracks (model_open_source.py:131-134).  wp/we are tap-major (K, C).
-// prosody (B,5) or null: per-item {alpha, p_scale, p_shift, e_scale, e_shift}; the tracks enter the
-// convolutions as p*p_scale + p_shift and e*e_scale + e_shift (unfused, so 1 and 0 give p back).  With
-// prosody and lens (batch-invariant contract) the window ends at lens[b] like the item's own B=1 call,
-// where the conv's zero padding follows the last token; the shifted pads would otherwise leak in.
+// prosody or null: {alpha, p_scale, p_shift, e_scale, e_shift} rows, one per item (B,5) or, with
+// per_token, one per token (B,T,5); the tracks enter the convolutions as p*p_scale + p_shift and
+// e*e_scale + e_shift (unfused, so 1 and 0 give p back), each tap with its own token's row.  With
+// prosody and window (batch-invariant contract) the window ends at lens[b] like the item's own B=1
+// call, where the conv's zero padding follows the last token; the shifted pads would otherwise leak
+// in.  Per-token rows of pad tokens (t >= lens[b]) act as neutral.  zero_pads: the tracks are the
+// caller's, and their pad entries read as 0, what the predictors write there.
 // ---------------------------------------------------------------------------------------------
 __global__ void var_embed_add_kernel(float* __restrict__ x, const float* __restrict__ pitch,
                                      const float* __restrict__ energy, const float* __restrict__ wp,
                                      const float* __restrict__ bp, const float* __restrict__ we,
-                                     const float* __restrict__ be, const float* __restrict__ prosody,
-                                     const int32_t* __restrict__ lens, int T, int C, int K) {
+                                     const float* __restrict__ be, const float* __restrict__ prosody, int per_token,
+                                     const int32_t* __restrict__ lens, int window, int zero_pads, int T, int C, int K) {
   pdl_entry();
   const int row = blockIdx.x;   // b*T + t
   const int b = row / T, t = row % T;
   __shared__ float ps[16], es[16];
   if (threadIdx.x < K) {
-    const int tl = (prosody && lens) ? min(T, lens[b]) : T;
+    const int len = lens ? min(T, lens[b]) : T;
+    const int tl = (prosody && window) ? len : T;
     const int tt = t + threadIdx.x - (K - 1) / 2;
     const bool ok = tt >= 0 && tt < tl;
-    float p = ok ? pitch[(size_t)b * T + tt] : 0.f;
-    float e = ok ? energy[(size_t)b * T + tt] : 0.f;
-    if (prosody && ok) {
-      const float* pr = prosody + (size_t)b * 5;
+    const bool rd = ok && !(zero_pads && tt >= len);
+    float p = rd ? pitch[(size_t)b * T + tt] : 0.f;
+    float e = rd ? energy[(size_t)b * T + tt] : 0.f;
+    if (prosody && ok && !(per_token && tt >= len)) {
+      const float* pr = prosody + (per_token ? (size_t)b * T + tt : (size_t)b) * 5;
       p = __fadd_rn(__fmul_rn(p, pr[1]), pr[2]);
       e = __fadd_rn(__fmul_rn(e, pr[3]), pr[4]);
     }
@@ -465,63 +470,88 @@ __global__ void var_embed_add_kernel(float* __restrict__ x, const float* __restr
   }
 }
 int launch_var_embed_add(float* x, const float* pitch, const float* energy, const float* wp, const float* bp,
-                         const float* we, const float* be, const float* prosody, const int32_t* lens, int B, int T, int C,
-                         int K, cudaStream_t st) {
+                         const float* we, const float* be, const float* prosody, int per_token, const int32_t* lens, int window,
+                         int zero_pads, int B, int T, int C, int K, cudaStream_t st) {
   EV_CHECK_ARG(K <= 16, "var_embed: K=%d > 16", K);
-  return launch("var_embed_add_kernel", var_embed_add_kernel, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, prosody, lens, T, C, K);
+  EV_CHECK_ARG(lens || !(per_token || zero_pads), "var_embed: per-token rows and caller tracks need lens");
+  return launch("var_embed_add_kernel", var_embed_add_kernel, B * T, 128, 0, st, x, pitch, energy, wp, bp, we, be, prosody, per_token,
+                lens, window, zero_pads, T, C, K);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Duration bookkeeping of GaussianUpsampling.forward (alignment.py:183-199): ds = float(d) * alpha
-// (alpha[b * alpha_stride] per item, 1 when alpha is null); the "all durations are zero" guard
-// (:187-191, applied after the scaling and over the WHOLE batch, pads included; it writes 1, not
-// alpha); c = cumsum(ds) - ds/2; mel_lens[b] = trunc(fl32(sum_t ds)); mel_lens[B] = max_b.
-// The scan runs in fp64 and rounds each output to fp32, which is what ATen's CPU cumsum does.  Each
-// ds is an fp32 value whose ulp is at least alpha * 2^-23 and the sums stay below 2^24, so every fp64
-// partial sum is exact and the order of the parallel scan cannot change a bit.  The frame count rounds
-// the exact sum once; the reference's cascade fp32 sum can land one frame off when the exact sum lies
-// within a few fp32 ulps of an integer.
+// (alpha[b * alpha_stride + t * alpha_tstride]: per item when alpha_tstride is 0, per token
+// otherwise; 1 when alpha is null); the "all durations are zero" guard (:187-191, applied after the
+// scaling and over the WHOLE batch, pads included; it writes 1, not alpha); c = cumsum(ds) - ds/2;
+// mel_lens[b] = trunc(fl32(sum_t ds)); mel_lens[B] = max_b.
+// The scan runs in fp64 and rounds each output to fp32, which is what ATen's CPU cumsum does.  Every
+// fp64 partial sum is exact, so the order of the parallel scan cannot change a bit:
+//  * one alpha per item: each nonzero ds = fl32(d * alpha) >= alpha is a multiple of ulp(alpha), and
+//    an item's sum stays below 2 * alpha * D with D = sum_t d <= max_frames < 2^24, so the sum has
+//    fewer than 49 significant bits;
+//  * alphas per token: the host keeps them in [1/16, 16]; every fp32 value >= 1/16 is a multiple of
+//    2^-27, and a sum that passes the frame check is below 2^24, so it has fewer than 52 bits.
+// (d itself converts exactly: it is at most max_frames < 2^24.)  The frame count rounds the exact sum
+// once; the reference's cascade fp32 sum can land one frame off when the exact sum lies within a few
+// fp32 ulps of an integer.
+// caller != 0: dur holds caller durations: entries at t >= lens[b] are ignored (read as 0), negative
+// ones are clamped to 0 and entries above max_frames to max_frames + 1 before anything is summed, so the
+// u64 sums cannot overflow and both passes over the durations see the same values.
 // status (may be null) gets bit 8 when an output would have no frames: any item under the
-// batch-invariant contract (its own B=1 call fails in the decoder), or the whole batch otherwise.
+// batch-invariant contract (its own B=1 call fails in the decoder), or the whole batch otherwise; and
+// bit 16 when a caller duration is negative or an item's frame count, before or after scaling,
+// exceeds max_frames (the vocoder indexes samples with int32: F * prod(upsample_rates) < 2^31).
 // One CTA (B*T is tiny).
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __restrict__ dur,
+__device__ __forceinline__ long long scan_dur(const int64_t* __restrict__ dur, int caller, const int32_t* __restrict__ lens,
+                                              int b, int t, int T, int max_frames, int& bad) {
+  const long long v = dur[(size_t)b * T + t];
+  if (!caller) return v;
+  if (lens && t >= lens[b]) return 0;
+  if (v < 0) { bad = 1; return 0; }
+  if (v > max_frames) { bad = 1; return (long long)max_frames + 1; }
+  return v;
+}
+
+__global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __restrict__ dur, int caller,
                                                              const int32_t* __restrict__ lens,
                                                              const float* __restrict__ alpha, int alpha_stride,
-                                                             int invariant, int B, int T, float* __restrict__ centers,
-                                                             float* __restrict__ ds_f, int32_t* __restrict__ mel_lens,
-                                                             int32_t* __restrict__ status) {
+                                                             int alpha_tstride, int invariant, int B, int T,
+                                                             float* __restrict__ centers, float* __restrict__ ds_f,
+                                                             int32_t* __restrict__ mel_lens, int32_t* __restrict__ status,
+                                                             int max_frames) {
   pdl_entry();
   __shared__ unsigned long long s_total;
-  __shared__ int s_max, s_min;
+  __shared__ int s_max, s_min, s_bad;
   const int tid = threadIdx.x, nw = blockDim.x >> 5, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) { s_total = 0ull; s_max = 0; s_min = 0x7fffffff; }
+  if (tid == 0) { s_total = 0ull; s_max = 0; s_min = 0x7fffffff; s_bad = 0; }
   __syncthreads();
   unsigned long long part = 0;
-  for (int i = tid; i < B * T; i += blockDim.x) part += (unsigned long long)dur[i];
+  int bad = 0;
+  for (int i = tid; i < B * T; i += blockDim.x) part += (unsigned long long)scan_dur(dur, caller, lens, i / T, i % T, T, max_frames, bad);
   for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
   if (lane == 0 && part) atomicAdd(&s_total, part);
+  if (bad) s_bad = 1;
   __syncthreads();
   const bool batch_all_zero = (s_total == 0ull);
   // one warp per batch item: chunked inclusive scan
   for (int b = wid; b < B; b += nw) {
     // literal batch: the guard looks at the whole batch and rewrites whole rows (pads included);
     // batch-invariant contract: each item is its own B=1 call of length lens[b].
-    bool all_zero = batch_all_zero;
-    int tl = T;
-    if (invariant) {
-      tl = lens ? min(T, lens[b]) : T;
-      unsigned long long own = 0;
-      for (int t = lane; t < tl; t += 32) own += (unsigned long long)dur[(size_t)b * T + t];
-      for (int o = 16; o > 0; o >>= 1) own += __shfl_xor_sync(0xffffffffu, own, o);
-      all_zero = (own == 0ull);
-    }
-    const float a = alpha ? alpha[(size_t)b * alpha_stride] : 1.0f;
+    const int tl = invariant ? (lens ? min(T, lens[b]) : T) : T;
+    unsigned long long own = 0;
+    for (int t = lane; t < tl; t += 32) own += (unsigned long long)scan_dur(dur, caller, lens, b, t, T, max_frames, bad);
+    for (int o = 16; o > 0; o >>= 1) own += __shfl_xor_sync(0xffffffffu, own, o);
+    const bool all_zero = invariant ? (own == 0ull) : batch_all_zero;
+    if (own > (unsigned long long)max_frames) bad = 1;
     double run = 0.0;
     for (int t0 = 0; t0 < T; t0 += 32) {
       const int t = t0 + lane;
       float d = 0.f;
-      if (t < T) d = all_zero ? (t < tl ? 1.0f : 0.f) : __fmul_rn((float)dur[(size_t)b * T + t], a);
+      if (t < T) {
+        const float a = alpha ? alpha[(size_t)b * alpha_stride + (size_t)t * alpha_tstride] : 1.0f;
+        d = all_zero ? (t < tl ? 1.0f : 0.f) : __fmul_rn((float)scan_dur(dur, caller, lens, b, t, T, max_frames, bad), a);
+      }
       double incl = d;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -535,22 +565,27 @@ __global__ void __launch_bounds__(1024) duration_scan_kernel(const int64_t* __re
       run += __shfl_sync(0xffffffffu, incl, 31);
     }
     if (lane == 0) {
-      const int n = (int)__double2float_rn(run);
+      const int n = (int)__double2float_rn(run);       // the conversion saturates: an oversized sum cannot wrap
+      if (n > max_frames) bad = 1;
       mel_lens[b] = n;
       atomicMax(&s_max, n);
       atomicMin(&s_min, n);
     }
   }
+  if (bad) s_bad = 1;
   __syncthreads();
   if (tid == 0) {
     mel_lens[B] = s_max;
     if (status && (invariant ? s_min == 0 : s_max == 0)) atomicOr(status, 8);
+    if (status && s_bad) atomicOr(status, 16);
   }
 }
-int launch_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int alpha_stride, int invariant, int B,
-                         int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, cudaStream_t st) {
-  return launch("duration_scan_kernel", duration_scan_kernel, 1, 1024, 0, st, dur, lens, alpha, alpha_stride, invariant, B, T,
-                centers, ds_f, mel_lens, status);
+int launch_duration_scan(const int64_t* dur, int caller, const int32_t* lens, const float* alpha, int alpha_stride, int alpha_tstride,
+                         int invariant, int B, int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, int max_frames,
+                         cudaStream_t st) {
+  EV_CHECK_ARG(max_frames > 0 && max_frames < (1 << 24), "duration_scan: max_frames=%d", max_frames);
+  return launch("duration_scan_kernel", duration_scan_kernel, 1, 1024, 0, st, dur, caller, lens, alpha, alpha_stride, alpha_tstride,
+                invariant, B, T, centers, ds_f, mel_lens, status, max_frames);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -749,6 +749,25 @@ int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64
                          const float* content, int B, int T, int invariant, const float* prosody, int64_t* dur_out,
                          float* pitch_out, float* energy_out, int32_t* lens32_out, int32_t* mel_lens_out, void* workspace,
                          size_t workspace_bytes, void* stream) {
+  return ev_am_phase1_controls(ctx, ling, lens64, spk, style, content, B, T, invariant, prosody, 0, nullptr, nullptr, nullptr, dur_out,
+                               pitch_out, energy_out, lens32_out, mel_lens_out, workspace, workspace_bytes, stream);
+}
+
+// Largest frame count an item may have: the vocoder indexes an item's samples with int32 (F * prod(upsample_rates) < 2^31),
+// and the duration scan's exactness argument wants counts below 2^24.
+static const int kScanMaxFrames = (1 << 24) - 1;
+static int max_item_frames(const ev_config& g) {
+  long long up = 1;
+  for (int i = 0; i < g.n_ups; ++i) up *= g.up_rates[i] > 0 ? g.up_rates[i] : 1;
+  const long long m = 2147483647LL / up;
+  return (int)(m < kScanMaxFrames ? m : kScanMaxFrames);
+}
+
+int ev_am_phase1_controls(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64, const int64_t* spk, const float* style,
+                          const float* content, int B, int T, int invariant, const float* prosody, int prosody_per_token,
+                          const int64_t* durations, const float* pitch_in, const float* energy_in, int64_t* dur_out,
+                          float* pitch_out, float* energy_out, int32_t* lens32_out, int32_t* mel_lens_out, void* workspace,
+                          size_t workspace_bytes, void* stream) {
   EV_CHECK_ARG(ctx && ctx->bound && ctx->has_am, "ev_am_phase1: acoustic-model weights not bound");
   EV_CHECK_ARG(ling && lens64 && spk && style && content && dur_out && pitch_out && energy_out && lens32_out &&
                    mel_lens_out && workspace,
@@ -787,11 +806,16 @@ int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens64
   EV_TRY(run_predictor(ctx, ctx->pitch, pin, b.p1[0], b.p2[0], B, T, lens, conv_lens, 0, pitch_out, nullptr, ws, st));
   EV_TRY(run_predictor(ctx, ctx->energy, pin, b.p1[1], b.p2[1], B, T, lens, conv_lens, 0, energy_out, nullptr, ws, st));
   EV_TRY(run_predictor(ctx, ctx->dur, pin, b.p1[2], b.p2[2], B, T, lens, conv_lens, 1, nullptr, dur_out, ws, st));
-  // x = x + pitch_embed + energy_embed (model_open_source.py:131-134), the tracks shifted / scaled per item when prosody is given
-  EV_TRY(launch_var_embed_add(b.hs, pitch_out, energy_out, ctx->pemb_w, ctx->pemb_b, ctx->eemb_w, ctx->eemb_b, prosody, conv_lens,
+  // x = x + pitch_embed + energy_embed (model_open_source.py:131-134) on the predicted tracks or the caller's, shifted / scaled
+  // per item or per token when prosody is given
+  EV_TRY(launch_var_embed_add(b.hs, pitch_in ? pitch_in : pitch_out, energy_in ? energy_in : energy_out, ctx->pemb_w, ctx->pemb_b,
+                              ctx->eemb_w, ctx->eemb_b, prosody, prosody_per_token, lens, invariant, (pitch_in || energy_in) ? 1 : 0,
                               B, T, H, g.embed_kernel, st));
-  // duration bookkeeping for the length regulator (alignment.py:183-199), durations scaled by alpha = prosody[b*5]
-  EV_TRY(launch_duration_scan(dur_out, lens, prosody, 5, invariant, B, T, b.centers, b.ds_f, mel_lens_out, mel_lens_out + B + 1, st));
+  // duration bookkeeping for the length regulator (alignment.py:183-199) on the predicted durations or the caller's, scaled by
+  // alpha = prosody[(b*T + t)*5] per token or prosody[b*5] per item
+  EV_TRY(launch_duration_scan(durations ? durations : dur_out, durations ? 1 : 0, lens, prosody, prosody_per_token ? 5 * T : 5,
+                              prosody_per_token ? 5 : 0, invariant, B, T, b.centers, b.ds_f, mel_lens_out, mel_lens_out + B + 1,
+                              max_item_frames(g), st));
   return EV_OK;
 }
 
@@ -1093,8 +1117,8 @@ int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* len
   EV_TRY(use_device_of(hs));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // centers_tmp holds 2*B*T floats: centres then float durations
-  EV_TRY(launch_duration_scan(dur, lens, nullptr, 0, invariant, B, T, centers_tmp, centers_tmp + (size_t)B * T, mel_lens_tmp, nullptr,
-                              st));
+  EV_TRY(launch_duration_scan(dur, 0, lens, nullptr, 0, 0, invariant, B, T, centers_tmp, centers_tmp + (size_t)B * T, mel_lens_tmp,
+                              nullptr, kScanMaxFrames, st));
   return launch_gauss_upsample(hs, centers_tmp, lens, mel_lens_tmp, B, T, H, F, invariant, pe, alpha, out, st);
 }
 
@@ -1145,7 +1169,8 @@ int ev_op_var_embed_add(float* x, const float* pitch, const float* energy, const
   EV_CHECK_ARG(x && pitch && energy && wp && bp && we && be, "ev_op_var_embed_add: null argument");
   EV_CHECK_ARG(B > 0 && T > 0 && C > 0 && K > 0 && (K & 1), "ev_op_var_embed_add: B=%d T=%d C=%d K=%d", B, T, C, K);
   EV_TRY(use_device_of(x));
-  return launch_var_embed_add(x, pitch, energy, wp, bp, we, be, prosody, lens, B, T, C, K, reinterpret_cast<cudaStream_t>(stream));
+  return launch_var_embed_add(x, pitch, energy, wp, bp, we, be, prosody, 0, lens, lens ? 1 : 0, 0, B, T, C, K,
+                              reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int invariant, int B, int T, float* centers,
@@ -1153,8 +1178,19 @@ int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* al
   EV_CHECK_ARG(dur && centers && ds && mel_lens, "ev_op_duration_scan: null argument");
   EV_CHECK_ARG(B > 0 && T > 0, "ev_op_duration_scan: B=%d T=%d", B, T);
   EV_TRY(use_device_of(dur));
-  return launch_duration_scan(dur, lens, alpha, 1, invariant, B, T, centers, ds, mel_lens, nullptr,
+  return launch_duration_scan(dur, 0, lens, alpha, 1, 0, invariant, B, T, centers, ds, mel_lens, nullptr, kScanMaxFrames,
                               reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ev_op_duration_scan_controls(const int64_t* dur, int caller, const int32_t* lens, const float* alpha, int alpha_stride,
+                                 int alpha_tstride, int invariant, int B, int T, int max_frames, float* centers, float* ds,
+                                 int32_t* mel_lens, int32_t* status, void* stream) {
+  EV_CHECK_ARG(dur && centers && ds && mel_lens, "ev_op_duration_scan_controls: null argument");
+  EV_CHECK_ARG(B > 0 && T > 0 && alpha_stride >= 0 && alpha_tstride >= 0, "ev_op_duration_scan_controls: B=%d T=%d strides %d %d", B,
+               T, alpha_stride, alpha_tstride);
+  EV_TRY(use_device_of(dur));
+  return launch_duration_scan(dur, caller, lens, alpha, alpha_stride, alpha_tstride, invariant, B, T, centers, ds, mel_lens, status,
+                              max_frames, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

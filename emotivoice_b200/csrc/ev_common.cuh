@@ -225,13 +225,18 @@ int launch_validate_inputs(const int64_t* ling, const int64_t* lens, const int64
                            int T, int n_vocab, int n_spk, cudaStream_t st);
 // zero rows t >= lens[b] of x (B,T,C) into y (masked_fill of the predictors' input)
 int launch_mask_rows(const float* x, const int32_t* lens, float* y, int B, int T, int C, cudaStream_t st);
-// prosody (B,5) {alpha, p_scale, p_shift, e_scale, e_shift} or null (neutral); lens: the window's end per item, or null
+// prosody {alpha, p_scale, p_shift, e_scale, e_shift} rows or null (neutral): (B,5), or (B,T,5) when per_token (rows of pad
+// tokens t >= lens[b] act as neutral); lens: item lengths or null; window: with prosody the window ends at lens[b];
+// zero_pads: track entries at t >= lens[b] read as 0 (caller-given tracks)
 int launch_var_embed_add(float* x, const float* pitch, const float* energy, const float* wp, const float* bp,
-                         const float* we, const float* be, const float* prosody, const int32_t* lens, int B, int T, int C,
-                         int K, cudaStream_t st);
-// alpha[b * alpha_stride] scales item b's durations (null: 1); status (may be null) |= 8 when an output has no frames
-int launch_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int alpha_stride, int invariant, int B,
-                         int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, cudaStream_t st);
+                         const float* we, const float* be, const float* prosody, int per_token, const int32_t* lens, int window,
+                         int zero_pads, int B, int T, int C, int K, cudaStream_t st);
+// alpha[b * alpha_stride + t * alpha_tstride] scales duration (b,t) (null: 1); caller: dur holds caller durations (pads
+// t >= lens[b] ignored, negatives clamped to 0); status (may be null) |= 8 when an output has no frames, |= 16 when a caller
+// duration is negative or an item's frame count (before or after scaling) exceeds max_frames
+int launch_duration_scan(const int64_t* dur, int caller, const int32_t* lens, const float* alpha, int alpha_stride, int alpha_tstride,
+                         int invariant, int B, int T, float* centers, float* ds_f, int32_t* mel_lens, int32_t* status, int max_frames,
+                         cudaStream_t st);
 int launch_gauss_upsample(const float* hs, const float* centers, const int32_t* lens, const int32_t* mel_lens,
                           int B, int T, int H, int F, int invariant, const float* pe, const float* alpha,
                           float* out, cudaStream_t st);

@@ -70,14 +70,73 @@ def speech_controls(speed=1.0, pitch_shift=0.0, energy_scale=1.0):
     return (1.0 / speed, pitch_shift, energy_scale)
 
 
+TOKEN_SPEED_RANGE = (1.0 / 16.0, 16.0)        # per-phoneme duration scales 1 / speed must lie in [1/16, 16] (modules.prosody_table)
+
+
+def phoneme_controls(n, speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+    """``speech_controls`` where each control may also be a sequence of ``n`` values, one per phoneme.  Returns the
+    ``(duration_scale, pitch_shift, energy_scale)`` triple with a float or a float64 array of length n in each place (an array
+    only where one was given).  Per-phoneme speeds must lie in [1/16, 16].  Raises ValueError."""
+    vals = []
+    for name, v in (("speed", speed), ("pitch_shift", pitch_shift), ("energy_scale", energy_scale)):
+        a = np.asarray(v, dtype=np.float64)
+        if a.ndim > 1 or (a.ndim == 1 and a.shape[0] != n):
+            raise ValueError("%s must be a float or a sequence of %d values (one per phoneme), got shape %s" % (name, n, a.shape))
+        vals.append(a)
+    sp, ps, es = vals
+    if sp.ndim == ps.ndim == es.ndim == 0:
+        return speech_controls(float(sp), float(ps), float(es))
+    if not (np.all(np.isfinite(sp)) and np.all(sp > 0)):
+        raise ValueError("speed must be finite and > 0")
+    if sp.ndim == 1 and not (np.all(sp >= TOKEN_SPEED_RANGE[0]) and np.all(sp <= TOKEN_SPEED_RANGE[1])):
+        raise ValueError("a per-phoneme speed must lie in [1/16, 16]")
+    if not np.all(np.isfinite(ps)):
+        raise ValueError("pitch_shift must be finite")
+    if not (np.all(np.isfinite(es)) and np.all(es > 0)):
+        raise ValueError("energy_scale must be finite and > 0")
+    out = (1.0 / sp, ps, es)
+    return tuple(float(x) if x.ndim == 0 else x for x in out)
+
+
+GIVEN = ("durations", "pitch", "energy")
+
+
+def given_values(n, durations=None, pitch=None, energy=None):
+    """A request's caller-given ``durations`` (integer frames >= 0) / ``pitch`` / ``energy`` (finite) tracks, each None or a
+    sequence of ``n`` values -> {name: int64 / float32 array} for the ones given.  Raises ValueError."""
+    out = {}
+    for name, v in (("durations", durations), ("pitch", pitch), ("energy", energy)):
+        if v is None:
+            continue
+        if isinstance(v, torch.Tensor):
+            v = v.detach().cpu().numpy()
+        a = np.asarray(v)
+        if a.shape != (n,):
+            raise ValueError("%s must hold %d values (one per phoneme), got shape %s" % (name, n, a.shape))
+        if name == "durations":
+            if a.dtype.kind not in "iu" or (a.size and a.min() < 0):
+                raise ValueError("durations must be integers >= 0")
+            out[name] = a.astype(np.int64)
+        else:
+            if a.dtype.kind not in "fiu" or not np.all(np.isfinite(a)):
+                raise ValueError("%s must be finite numbers" % name)
+            out[name] = a.astype(np.float32)
+    return out
+
+
 def collate(items, device="cpu", pad_id=0):
     """items: list of (ids, speaker_id, style_vec, content_vec) -> the keyword arguments of
     ``JETSGenerator.forward`` (inference_am_vocoder_joint.py:113-128), padded with id 0 (the collate
     convention of the reference's dataset, prompt_dataset.py:183).
 
-    An item may carry a fifth field, its ``(duration_scale, pitch_shift, energy_scale)`` (see ``speech_controls``).
-    When some item's controls are not neutral the result also holds the three per-item lists; otherwise it holds the
-    five inputs only, so neutral traffic makes exactly the uncontrolled call."""
+    An item may carry a fifth field, its ``(duration_scale, pitch_shift, energy_scale)`` (see ``speech_controls`` /
+    ``phoneme_controls``).  When some item's controls are not neutral the result also holds the three controls: per-item
+    lists, or (B,T) float64 tables when some item has per-phoneme values (each item's row holds its own values, per-item ones
+    repeated along it; pads are neutral).  Otherwise it holds the five inputs only, so neutral traffic makes exactly the
+    uncontrolled call.
+
+    An item may carry a sixth field, the dict of ``given_values``.  Every item of the batch must then give the same tracks;
+    they are padded to (B,T) with zeros (the padded entries are ignored by the model)."""
     B, T = len(items), max(len(it[0]) for it in items)
     ling = np.full((B, T), pad_id, dtype=np.int64)
     for b, it in enumerate(items):
@@ -99,10 +158,29 @@ def collate(items, device="cpu", pad_id=0):
         inputs_content_embedding=vecs(3),
     )
     controls = [tuple(it[4]) if len(it) > 4 else NEUTRAL_CONTROLS for it in items]
-    if any(c != NEUTRAL_CONTROLS for c in controls):
+    per_token = any(isinstance(x, np.ndarray) for c in controls for x in c)
+    if per_token:
+        for j, name in enumerate(("duration_scale", "pitch_shift", "energy_scale")):
+            tab = np.full((B, T), NEUTRAL_CONTROLS[j], dtype=np.float64)
+            for b, (it, c) in enumerate(zip(items, controls)):
+                if isinstance(c[j], np.ndarray):
+                    tab[b, :len(it[0])] = c[j]
+                else:
+                    tab[b, :] = c[j]            # a per-item value fills its whole row: the row is then one per-item scale
+            out[name] = tab
+    elif any(c != NEUTRAL_CONTROLS for c in controls):
         out["duration_scale"] = [c[0] for c in controls]
         out["pitch_shift"] = [c[1] for c in controls]
         out["energy_scale"] = [c[2] for c in controls]
+    given = [it[5] if len(it) > 5 else {} for it in items]
+    names = set(given[0])
+    if any(set(g) != names for g in given):
+        raise ValueError("every item of a batch must give the same caller tracks (durations / pitch / energy)")
+    for name in sorted(names):
+        tab = np.zeros((B, T), dtype=np.int64 if name == "durations" else np.float32)
+        for b, (it, g) in enumerate(zip(items, given)):
+            tab[b, :len(it[0])] = g[name]
+        out[name] = to(tab)
     return out
 
 
@@ -114,7 +192,8 @@ class MicroBatcher:
     float32 waveform trimmed to its own length (``mel_lengths[b] * hop``).  A worker thread collects up to
     ``max_batch`` requests, waiting at most ``max_wait_s`` after the first one, and runs ONE forward.
     Errors of a batch are delivered to every future of that batch.  Requests with different prosody controls
-    (``speed``, ``pitch_shift``, ``energy_scale``) share one forward: the controls are per item.
+    (``speed``, ``pitch_shift``, ``energy_scale``, per item or per phoneme) share one forward.  Requests that give their
+    own ``durations`` / ``pitch`` / ``energy`` run in one forward with the requests that give the same set of tracks.
     """
 
     def __init__(self, forward, device="cpu", max_batch=32, max_wait_s=0.005, hop=256):
@@ -127,15 +206,22 @@ class MicroBatcher:
         self._thread = threading.Thread(target=self._loop, name="ev-microbatcher", daemon=True)
         self._thread.start()
 
-    def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+    def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0, durations=None,
+               pitch=None, energy=None):
         """``speed`` > 1 speaks faster (duration_scale = 1 / speed); ``pitch_shift`` in semitones; ``energy_scale``
-        multiplies frame energy.  Invalid controls raise ValueError here, so they cannot fail a batch of other requests."""
-        controls = speech_controls(speed, pitch_shift, energy_scale)
+        multiplies frame energy.  Each is a float or a sequence of ``len(ids)`` values, one per phoneme (a per-phoneme speed
+        must lie in [1/16, 16]).  ``durations`` (integer frames), ``pitch`` and ``energy`` (the predictors' normalised units):
+        None or ``len(ids)`` values that replace the model's predictions (see ``JETSGenerator.forward``).  Invalid values
+        raise ValueError here, so they cannot fail a batch of other requests."""
+        ids = np.asarray(ids, dtype=np.int64)
+        controls = phoneme_controls(len(ids), speed, pitch_shift, energy_scale)
+        given = given_values(len(ids), durations, pitch, energy)
+        item = (ids, int(speaker_id), style_vec, content_vec, controls) + ((given,) if given else ())
         fut = Future()
         with self._lock:
             if self._closed:
                 raise RuntimeError("MicroBatcher is closed")
-            self._queue.append(((np.asarray(ids, dtype=np.int64), int(speaker_id), style_vec, content_vec, controls), fut))
+            self._queue.append((item, fut))
             self._lock.notify()
         return fut
 
@@ -171,20 +257,27 @@ class MicroBatcher:
             batch = self._take()
             if batch is None:
                 return
-            futs = [f for _, f in batch]
-            try:
-                out = self._forward(**collate([it for it, _ in batch], self._device))
-                wav = out["wav_predictions"]
-                lens = out.get("mel_lengths")
-                lens = [int(wav.shape[-1]) // self._hop] * len(batch) if lens is None else [int(v) for v in lens.tolist()]
-                wav = wav.detach().cpu()
-                self.batches_run += 1
-                for b, f in enumerate(futs):
-                    f.set_result(wav[b, 0, :lens[b] * self._hop].clone())
-            except BaseException as e:       # deliver, keep serving
-                for f in futs:
-                    if not f.done():
-                        f.set_exception(e)
+            groups = {}                      # one forward per set of caller-given tracks (the common case: one group)
+            for it, f in batch:
+                groups.setdefault(tuple(sorted(it[5])) if len(it) > 5 else (), []).append((it, f))
+            for group in groups.values():
+                self._run(group)
+
+    def _run(self, batch):
+        futs = [f for _, f in batch]
+        try:
+            out = self._forward(**collate([it for it, _ in batch], self._device))
+            wav = out["wav_predictions"]
+            lens = out.get("mel_lengths")
+            lens = [int(wav.shape[-1]) // self._hop] * len(batch) if lens is None else [int(v) for v in lens.tolist()]
+            wav = wav.detach().cpu()
+            self.batches_run += 1
+            for b, f in enumerate(futs):
+                f.set_result(wav[b, 0, :lens[b] * self._hop].clone())
+        except BaseException as e:       # deliver, keep serving
+            for f in futs:
+                if not f.done():
+                    f.set_exception(e)
 
 
 # ---- output side (SURVEY.md s8f rank 2): the on-wire format every front-end emits -----------------------------------

@@ -42,8 +42,9 @@ PITCH_STATS = (225.089, 53.78)
 ENERGY_STATS = (30.610, 21.78)
 
 
-def _per_item(name, v, B, neutral):
-    """None / float / length-B sequence / CPU tensor -> float64 numpy (B,).  Raises ValueError before anything is enqueued."""
+def _per_item(name, v, B, neutral, T=None):
+    """None / float / length-B sequence / CPU tensor -> float64 numpy (B,); with T given also a (B,T) nested sequence or CPU
+    tensor -> (B,T).  Raises ValueError before anything is enqueued."""
     if v is None:
         return np.full(B, neutral, dtype=np.float64)
     if isinstance(v, torch.Tensor):
@@ -57,37 +58,98 @@ def _per_item(name, v, B, neutral):
         raise ValueError("%s must be a float, a length-%d sequence or a CPU tensor" % (name, B)) from None
     if a.ndim == 0:
         return np.full(B, float(a), dtype=np.float64)
-    if a.shape != (B,):
-        raise ValueError("%s has shape %s, expected a float or length %d" % (name, a.shape, B))
+    if a.shape != (B,) and (T is None or a.shape != (B, T)):
+        raise ValueError("%s has shape %s, expected a float, length %d%s" % (name, a.shape, B, "" if T is None else " or (%d, %d)" % (B, T)))
     return a
 
 
-def prosody_table(B, duration_scale=None, pitch_shift=None, energy_scale=None, config=None):
-    """Host side of the prosody controls: -> None when every item is neutral, else a (B,5) float32 CPU tensor, row b =
-    {alpha, p_scale, p_shift, e_scale, e_shift}.  alpha = fl32(duration_scale) (GaussianUpsampling's alpha, alignment.py:183);
-    with r = 2^(semitones/12): p_scale = fl32(r), p_shift = fl32(mean (r-1) / std) in the normalised units of the pitch
-    predictor, so that the shifted track is the normalised pitch of r * f0; energy likewise with r = energy_scale."""
-    a = _per_item("duration_scale", duration_scale, B, 1.0)
-    s = _per_item("pitch_shift", pitch_shift, B, 0.0)
-    e = _per_item("energy_scale", energy_scale, B, 1.0)
+# Per-token duration scales are kept in this range: every fp32 value >= 1/16 is a multiple of 2^-27, which keeps the duration scan's
+# fp64 sums exact whatever the mix of scales in an utterance (see duration_scan_kernel).  Per-item scales, and rows of a (B,T) table
+# that hold one value throughout, only need to be > 0.
+TOKEN_SCALE_RANGE = (1.0 / 16.0, 16.0)
+
+
+def prosody_table(B, duration_scale=None, pitch_shift=None, energy_scale=None, config=None, T=None):
+    """Host side of the prosody controls: -> None when every item is neutral, else a float32 CPU tensor of rows
+    {alpha, p_scale, p_shift, e_scale, e_shift}: (B,5) with one row per item, or (B,T,5) with one row per token when T is given
+    and some control is a (B,T) table (the per-item ones are then repeated along T).  alpha = fl32(duration_scale)
+    (GaussianUpsampling's alpha, alignment.py:183); with r = 2^(semitones/12): p_scale = fl32(r), p_shift = fl32(mean (r-1) / std)
+    in the normalised units of the pitch predictor, so that the shifted track is the normalised pitch of r * f0; energy likewise
+    with r = energy_scale.  A (B,T) duration_scale must lie in [1/16, 16], except in rows that hold one value throughout."""
+    a = _per_item("duration_scale", duration_scale, B, 1.0, T)
+    s = _per_item("pitch_shift", pitch_shift, B, 0.0, T)
+    e = _per_item("energy_scale", energy_scale, B, 1.0, T)
     if not (np.all(np.isfinite(a)) and np.all(a > 0)):
         raise ValueError("duration_scale must be finite and > 0, got %s" % a.tolist())
     if not np.all(np.isfinite(s)):
         raise ValueError("pitch_shift must be finite, got %s" % s.tolist())
     if not (np.all(np.isfinite(e)) and np.all(e > 0)):
         raise ValueError("energy_scale must be finite and > 0, got %s" % e.tolist())
+    if a.ndim == 2:                 # a row with one value throughout is a per-item scale and keeps the per-item range
+        a32 = a.astype(np.float32)
+        lo, hi = TOKEN_SCALE_RANGE
+        varies = np.any(a32 != a32[:, :1], axis=1, keepdims=True)
+        if np.any(varies & ((a32 < lo) | (a32 > hi))):
+            raise ValueError("a per-token duration_scale must lie in [1/16, 16] (a row with one value throughout may hold any "
+                             "scale > 0), got values in [%g, %g]" % (a.min(), a.max()))
     if np.all(a == 1.0) and np.all(s == 0.0) and np.all(e == 1.0):
         return None
+    if max(a.ndim, s.ndim, e.ndim) == 2:
+        a, s, e = (np.broadcast_to(x if x.ndim == 2 else x[:, None], (B, T)) for x in (a, s, e))
     mp, sp = getattr(config, "pitch_stats", None) or PITCH_STATS
     me, se = getattr(config, "energy_stats", None) or ENERGY_STATS
     with np.errstate(over="ignore", invalid="ignore"):
         rp = np.exp2(s / 12.0)
-        tab = np.stack([a, rp, float(mp) * (rp - 1.0) / float(sp), e, float(me) * (e - 1.0) / float(se)], axis=1)
-        tab32 = tab.astype(np.float32)
-    if not (np.all(np.isfinite(tab32)) and np.all(tab32[:, 0] > 0) and np.all(tab32[:, 3] > 0)):
+        tab = np.stack([a, rp, float(mp) * (rp - 1.0) / float(sp), e, float(me) * (e - 1.0) / float(se)], axis=-1)
+        tab32 = np.ascontiguousarray(tab.astype(np.float32))
+    if not (np.all(np.isfinite(tab32)) and np.all(tab32[..., 0] > 0) and np.all(tab32[..., 3] > 0)):
         raise ValueError("prosody controls outside the fp32 range: duration_scale %s, pitch_shift %s, energy_scale %s"
                          % (a.tolist(), s.tolist(), e.tolist()))
     return torch.from_numpy(tab32)
+
+
+def caller_values(name, v, B, T, device, integer):
+    """A caller-given ``durations`` (integer) or ``pitch`` / ``energy`` (float) track -> None, a (B,T) int64 / float32 CPU tensor
+    (validated here: durations >= 0, tracks finite), or a (B,T) tensor on ``device`` (taken as it is: int64 / float32 exactly,
+    since converting it would enqueue work).  (T,) is accepted when B == 1, so that the squeezed predictions of a forward can
+    be passed straight back.  Raises ValueError before anything is enqueued."""
+    if v is None:
+        return None
+    want = torch.int64 if integer else torch.float32
+    kind = "an integer" if integer else "a floating-point"
+    if isinstance(v, torch.Tensor) and v.device.type != "cpu":
+        if v.device != torch.device(device):
+            raise ValueError("%s is on %s but the module is on %s" % (name, v.device, device))
+        if v.dtype != want:
+            raise ValueError("%s on the device must be %s, got %s" % (name, want, v.dtype))
+        t = v.detach()
+    else:
+        a = v.detach().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        if a.dtype.kind not in (("i", "u") if integer else ("f",)) and not (a.dtype == object and a.size == 0):
+            raise ValueError("%s must hold %s type, got %s" % (name, kind, a.dtype))
+        if integer:
+            if a.size and (a.min() < 0):
+                raise ValueError("%s must be >= 0 (frames per phoneme), got a minimum of %d" % (name, int(a.min())))
+            if a.size and a.max() > np.iinfo(np.int64).max:
+                raise ValueError("%s holds values beyond the int64 range" % name)
+        elif not np.all(np.isfinite(a)):
+            raise ValueError("%s must be finite" % name)
+        t = torch.from_numpy(np.ascontiguousarray(a.astype(np.int64 if integer else np.float32)))
+    if tuple(t.shape) != (B, T) and not (B == 1 and t.numel() == T and t.dim() <= 1):
+        raise ValueError("%s has shape %s, expected (%d, %d)%s" % (name, tuple(t.shape), B, T, " or (%d,)" % T if B == 1 else ""))
+    return t.reshape(B, T).contiguous()
+
+
+def controls_for(module, inputs_ling, duration_scale, pitch_shift, energy_scale, durations, pitch, energy):
+    """Every host-side check of the controls of ``forward``, before anything is packed or enqueued -> (prosody table or None,
+    {"durations": .., "pitch": .., "energy": ..} with None for an absent one)."""
+    B, T = int(inputs_ling.shape[0]), int(inputs_ling.shape[1])
+    prosody = prosody_table(B, duration_scale, pitch_shift, energy_scale, module.config, T=T)
+    dev = next(module.parameters()).device
+    given = dict(durations=caller_values("durations", durations, B, T, dev, True),
+                 pitch=caller_values("pitch", pitch, B, T, dev, False),
+                 energy=caller_values("energy", energy, B, T, dev, False))
+    return prosody, given
 
 
 def _bucket(nbytes):
@@ -227,14 +289,22 @@ class _Engine:
             pass
         return tl.pin[:n].clone()
 
-    def acoustic(self, ling, lens, spk, style, content, invariant, prosody=None):
-        """``prosody``: None (neutral: the plain ev_am_phase1 call) or the (B,5) CPU table of ``prosody_table``."""
+    def acoustic(self, ling, lens, spk, style, content, invariant, prosody=None, given=None):
+        """``prosody``: None (neutral: the plain ev_am_phase1 call) or the (B,5) / (B,T,5) CPU table of ``prosody_table``;
+        ``given``: None or the caller's {"durations", "pitch", "energy"} of ``controls_for`` (each None, a CPU or a device tensor)."""
         lib, dev = self.lib, self.device
         B, T = ling.shape
         self.ensure_pe(T)
-        if prosody is not None:       # uploaded with the inputs; the pinned source lives until the read-back below
-            prosody_host = prosody.pin_memory()
-            prosody = prosody_host.to(dev, non_blocking=True)
+        pinned = []                   # CPU sources are uploaded with the inputs; the pinned copies live until the read-back below
+
+        def upload(t):
+            if t is None or t.device == dev:
+                return t
+            pinned.append(t.pin_memory())
+            return pinned[-1].to(dev, non_blocking=True)
+        prosody = upload(prosody)
+        given = {k: upload(v) for k, v in (given or {}).items()}
+        caller = {k: v for k, v in given.items() if v is not None}
         dur = torch.empty((B, T), dtype=torch.int64, device=dev)
         pitch = torch.empty((B, T), dtype=torch.float32, device=dev)
         energy = torch.empty((B, T), dtype=torch.float32, device=dev)
@@ -244,7 +314,14 @@ class _Engine:
         st = self._stream()
         lens32_ptr = meta.data_ptr()
         mel_lens_ptr = meta.data_ptr() + 4 * B
-        if prosody is None:
+        ptr = lambda t: None if t is None else t.data_ptr()
+        if caller or (prosody is not None and prosody.dim() == 3):
+            _abi.check(lib.ev_am_phase1_controls(self.handle, ling.data_ptr(), lens.data_ptr(), spk.data_ptr(), style.data_ptr(),
+                                                 content.data_ptr(), B, T, int(invariant), ptr(prosody),
+                                                 int(prosody is not None and prosody.dim() == 3), ptr(given.get("durations")),
+                                                 ptr(given.get("pitch")), ptr(given.get("energy")), dur.data_ptr(), pitch.data_ptr(),
+                                                 energy.data_ptr(), lens32_ptr, mel_lens_ptr, ws1.data_ptr(), n1, st))
+        elif prosody is None:
             _abi.check(lib.ev_am_phase1(self.handle, ling.data_ptr(), lens.data_ptr(), spk.data_ptr(), style.data_ptr(),
                                         content.data_ptr(), B, T, int(invariant), dur.data_ptr(), pitch.data_ptr(),
                                         energy.data_ptr(), lens32_ptr, mel_lens_ptr, ws1.data_ptr(), n1, st))
@@ -265,6 +342,10 @@ class _Engine:
                 raise IndexError("inputs_speaker holds ids outside [0, %d)" % int(self.cfg.n_speaker))
             if status & 4:
                 raise RuntimeError("input_lengths must lie in [1, %d] (the padded width of inputs_ling)" % T)
+            if status & 16:
+                raise ValueError("durations hold a negative value, or an utterance would have more frames than the vocoder can "
+                                 "index (frames * %d must stay below 2^31); mel lengths %s"
+                                 % (self.total_up, mel_lens_host[:B].tolist()))
             # the reference's decoder fails on a zero-length input (Conv1d raises); nothing of phase 2 has been enqueued
             raise RuntimeError("duration_scale leaves an utterance with no frames (mel lengths %s); use a larger duration_scale"
                                % mel_lens_host[:B].tolist())
@@ -440,18 +521,19 @@ class PromptTTS(_EngineOwner):
     @torch.no_grad()
     def forward(self, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
                 mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0,
-                duration_scale=None, pitch_shift=None, energy_scale=None):
-        """``duration_scale`` / ``pitch_shift`` / ``energy_scale``: prosody controls, see ``JETSGenerator.forward``."""
+                duration_scale=None, pitch_shift=None, energy_scale=None, durations=None, pitch=None, energy=None):
+        """``duration_scale`` / ``pitch_shift`` / ``energy_scale`` and ``durations`` / ``pitch`` / ``energy``: prosody
+        controls, see ``JETSGenerator.forward``."""
         if mel_targets is not None:
             raise NotImplementedError("training-mode forward (teacher forcing) is out of scope for this engine")
-        prosody = prosody_table(inputs_ling.shape[0], duration_scale, pitch_shift, energy_scale, self.config)
+        prosody, given = controls_for(self, inputs_ling, duration_scale, pitch_shift, energy_scale, durations, pitch, energy)
         eng = self._engine()
         with eng.call_lock:
             return _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                               inputs_content_embedding, not self.compat_padded_batch, prosody)[0]
+                               inputs_content_embedding, not self.compat_padded_batch, prosody, given)[0]
 
 
-def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant, prosody=None):
+def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant, prosody=None, given=None):
     dev = eng.device
     ling = _prep(inputs_ling, torch.int64, dev)
     lens = _prep(input_lengths, torch.int64, dev)
@@ -465,7 +547,7 @@ def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content,
     if tuple(style.shape) != want or tuple(content.shape) != want:
         raise RuntimeError("inputs_style_embedding %s / inputs_content_embedding %s must both be %s"
                            % (tuple(style.shape), tuple(content.shape), want))
-    r = eng.acoustic(ling, lens, spk, style, content, invariant, prosody)
+    r = eng.acoustic(ling, lens, spk, style, content, invariant, prosody, given)
     out = {
         "mel_targets": None,
         "dec_outputs": r["mel"],
@@ -495,8 +577,9 @@ class JETSGenerator(_EngineOwner):
     reference's B=1 call for that item (what every reference caller runs); set the attribute
     to True to reproduce the literal padded-batch forward instead.  For B=1 both agree.
 
-    Prosody controls (keyword arguments of ``forward``; each None, one float for every item, or a length-B
-    sequence / CPU tensor with one value per item):
+    Prosody controls (keyword arguments of ``forward``; each None, one float for every item, a length-B sequence / CPU
+    tensor with one value per item, or a (B,T) nested sequence / CPU tensor with one value per phoneme, T =
+    ``inputs_ling.shape[1]``):
 
     * ``duration_scale`` (1.0): multiplies the predicted durations before the length regulator -- the ``alpha`` of
       the reference's GaussianUpsampling (alignment.py:180-183).  Above 1 is slower speech; a server's ``speed``
@@ -505,9 +588,26 @@ class JETSGenerator(_EngineOwner):
       2^(s/12) * f0, with the statistics of ``config.pitch_stats`` (default 225.089, 53.78).
     * ``energy_scale`` (1.0): multiplies frame energy the same way (``config.energy_stats``, default 30.610, 21.78).
 
-    The returned predictions stay the model's raw ones; ``mel_lengths`` counts the scaled frames.  Neutral values
-    give bitwise the uncontrolled output.  ``alpha=`` is accepted and ignored, as in the reference's inference
-    branch.  An utterance scaled to zero frames raises RuntimeError (the reference's decoder raises too).
+    A per-phoneme value acts exactly where the per-item one acts, on its own token: token t's duration is
+    fl32(fl32(d_t) * a_t), its pitch enters ``pitch_embed`` as p_t * r_t + shift_t.  Entries at t >= input_lengths[b]
+    are ignored.  A per-phoneme ``duration_scale`` must lie in [1/16, 16] (a row holding one value throughout may hold
+    any scale, as a per-item value may).  A table whose rows are constant gives
+    bitwise the per-item result (under ``compat_padded_batch`` a per-phoneme table leaves the pad positions
+    unshifted, where a per-item value shifts them too).
+
+    Caller-given values (keyword arguments ``durations`` (integer frames), ``pitch``, ``energy`` (the predictors'
+    normalised units)): each (B,T), or (T,) when B == 1, on the CPU or on the module's device.  They replace the
+    predictions where those are used -- the durations in the length regulator, the tracks in ``pitch_embed`` /
+    ``energy_embed`` -- and the controls above apply on top.  Values at t >= input_lengths[b] are ignored.  So the
+    returned ``log_duration_predictions``, ``pitch_predictions`` and ``energy_predictions`` can be edited and passed
+    back.  The all-zero guard of the length regulator applies to caller durations too.  Device durations are checked
+    on the device: a negative one, or an utterance with more frames than the vocoder can index, raises ValueError
+    before anything of the decoder is enqueued.
+
+    The returned predictions stay the model's raw ones; ``mel_lengths`` counts the frames actually used.  Neutral
+    values give bitwise the uncontrolled output.  Wrong shapes, dtypes or values raise ValueError before anything is
+    enqueued.  ``alpha=`` is accepted and ignored, as in the reference's inference branch.  An utterance scaled to
+    zero frames raises RuntimeError (the reference's decoder raises too).
     """
 
     def __init__(self, config):
@@ -527,15 +627,15 @@ class JETSGenerator(_EngineOwner):
     @torch.no_grad()
     def forward(self, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
                 mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0,
-                cut_flag=True, duration_scale=None, pitch_shift=None, energy_scale=None):
+                cut_flag=True, duration_scale=None, pitch_shift=None, energy_scale=None, durations=None, pitch=None, energy=None):
         if mel_targets is not None:
             raise NotImplementedError("training-mode forward (teacher forcing / random segments) is out of scope")
-        prosody = prosody_table(inputs_ling.shape[0], duration_scale, pitch_shift, energy_scale, self.config)
+        prosody, given = controls_for(self, inputs_ling, duration_scale, pitch_shift, energy_scale, durations, pitch, energy)
         eng = self._engine()
         invariant = not self.compat_padded_batch
         with eng.call_lock:
             return self._forward_locked(eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                                        inputs_content_embedding, prosody)
+                                        inputs_content_embedding, prosody, given)
 
     def reserve(self, batch=1, phonemes=256, frames=2048):
         """Serving set-up: pre-size the engine's workspace arena (current CUDA stream) for requests up to this shape, so that no
@@ -544,9 +644,9 @@ class JETSGenerator(_EngineOwner):
         self._engine().reserve(batch, phonemes, frames)
 
     def _forward_locked(self, eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
-                        prosody=None):
+                        prosody=None, given=None):
         outputs, r = _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                                 inputs_content_embedding, invariant, prosody)
+                                 inputs_content_embedding, invariant, prosody, given)
         B = r["mel"].shape[0]
         mel_lens_ptr = (r["meta"].data_ptr() + 4 * B) if invariant else None
         # jets.py:62-66: z = dec_outputs.transpose(1, 2); wav = generator(z).  dec_outputs is already the

@@ -138,7 +138,8 @@ EV_API size_t ev_phase2_workspace_bytes(const ev_ctx* ctx, int B, int F);
  *     [0, n_vocab), bit 1 = a speaker id outside [0, n_speaker), bit 2 = a length outside [1, T],
  *     bit 3 = an output with no frames (set only by ev_am_phase1_prosody with duration scales below 1:
  *     under the batch-invariant contract any item, otherwise the whole batch; the reference's decoder raises
- *     RuntimeError on a zero-length input).  Do not run phase 2 when it is set.
+ *     RuntimeError on a zero-length input), bit 4 = invalid caller durations or an item with more frames than
+ *     the vocoder can index (see ev_am_phase1_controls).  Do not run phase 2 when bit 3 or 4 is set.
  *   invariant != 0: batch-invariant contract (each item == the reference's B=1 call);
  *   invariant == 0: literal padded-batch forward of the reference. */
 EV_API int ev_am_phase1(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, const int64_t* spk,
@@ -155,12 +156,37 @@ EV_API int ev_am_phase1(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, c
  *     exact sum lies within a few fp32 ulps of an integer.
  *   pitch / energy enter pitch_embed / energy_embed (model_open_source.py:131-134) as p*p_scale + p_shift and
  *     e*e_scale + e_shift (two fp32 roundings each; 1 and 0 give the unscaled track back bit for bit).
- *   dur_out, pitch_out and energy_out stay the model's raw predictions. */
+ *   dur_out, pitch_out and energy_out stay the model's raw predictions.
+ * Equivalent to ev_am_phase1_controls(..., prosody, 0, NULL, NULL, NULL, ...). */
 EV_API int ev_am_phase1_prosody(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, const int64_t* spk,
                                 const float* style, const float* content, int B, int T, int invariant,
                                 const float* prosody, int64_t* dur_out, float* pitch_out, float* energy_out,
                                 int32_t* lens32_out, int32_t* mel_lens_out, void* workspace, size_t workspace_bytes,
                                 void* stream);
+
+/* ev_am_phase1_prosody with phoneme-level controls; it launches the same kernels.
+ *   prosody: NULL, (B,5) f32 per item (prosody_per_token == 0, as ev_am_phase1_prosody), or (B,T,5) f32 per token
+ *     (prosody_per_token != 0): row (b,t) = {alpha, p_scale, p_shift, e_scale, e_shift} of token t, acting exactly where
+ *     the per-item row acts (token t's duration is fl32(fl32(d_t) * alpha_t); token t's pitch enters pitch_embed as
+ *     p_t * p_scale_t + p_shift_t, each tap of the k-wide window with its own token's row).  Rows of tokens
+ *     t >= lens[b] are ignored (neutral).  Per-token alphas must lie in [1/16, 16] (the exactness of the scan rests on it;
+ *     the library does not check it); per-item alphas only need to be > 0.
+ *   durations: NULL, or (B,T) i64 caller durations that replace the predictions in the length regulator; entries at
+ *     t >= lens[b] are ignored.  The all-zero guard applies to them as to predicted ones.  They are checked on the device:
+ *     a negative entry, or an item whose frame count before or after scaling reaches 2^31 / prod(upsample_rates)
+ *     (the vocoder indexes samples with int32; at most 2^24 - 1 frames in any case), sets bit 4 (value 16) of the status
+ *     word.  That bit can also be set by predicted durations scaled past the limit.  Do not run phase 2 when it is set.
+ *   pitch_in / energy_in: NULL, or (B,T) f32 caller tracks that replace the predictions where they enter
+ *     pitch_embed / energy_embed (entries at t >= lens[b] are ignored, i.e. read as the 0 the predictors write there);
+ *     the prosody rows apply on top.  Not checked, as in the reference.
+ *   dur_out, pitch_out and energy_out stay the model's raw predictions; mel_lens_out counts the frames actually used.
+ *   All caller arrays are device memory, read in stream order. */
+EV_API int ev_am_phase1_controls(ev_ctx* ctx, const int64_t* ling, const int64_t* lens, const int64_t* spk,
+                                 const float* style, const float* content, int B, int T, int invariant,
+                                 const float* prosody, int prosody_per_token, const int64_t* durations,
+                                 const float* pitch_in, const float* energy_in, int64_t* dur_out, float* pitch_out,
+                                 float* energy_out, int32_t* lens32_out, int32_t* mel_lens_out, void* workspace,
+                                 size_t workspace_bytes, void* stream);
 
 /* Replaces: GaussianUpsampling.forward matmul (alignment.py:201-211), the decoder
  * (model_open_source.py:146) and to_mel (:147).  Must follow ev_am_phase1 on the same stream;
@@ -292,6 +318,13 @@ EV_API int ev_op_attention_tc(const float* qkv, const int32_t* key_lens, float* 
  * mel_lens (B+1) i32: trunc(fl32(sum ds)) per item, max in slot B. */
 EV_API int ev_op_duration_scan(const int64_t* dur, const int32_t* lens, const float* alpha, int invariant, int B, int T,
                                float* centers, float* ds, int32_t* mel_lens, void* stream);
+/* The duration bookkeeping of ev_am_phase1_controls alone: as ev_op_duration_scan, with alpha[b * alpha_stride +
+ * t * alpha_tstride] (alpha_tstride 0: per item); caller != 0: dur holds caller durations (entries t >= lens[b] ignored,
+ * negative ones clamped to 0); status (may be NULL) |= 8 when an output has no frames, |= 16 when a caller duration is
+ * negative or an item's frame count before or after scaling exceeds max_frames (in [1, 2^24 - 1]). */
+EV_API int ev_op_duration_scan_controls(const int64_t* dur, int caller, const int32_t* lens, const float* alpha, int alpha_stride,
+                                        int alpha_tstride, int invariant, int B, int T, int max_frames, float* centers, float* ds,
+                                        int32_t* mel_lens, int32_t* status, void* stream);
 EV_API int ev_op_gauss_upsample(const float* hs, const int64_t* dur, const int32_t* lens, int B, int T, int H,
                                 int F, int invariant, const float* pe, const float* alpha, float* centers_tmp,
                                 int32_t* mel_lens_tmp, float* out, void* stream);
