@@ -158,8 +158,15 @@ __global__ void __launch_bounds__(THREADS, 1) conv1d_gp_kernel(const __grid_cons
           const int sb = b_cnt % pl.b_stages;
           mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
           const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-          tap_chain<MODE, BN, NK8>(acc, desc_advance(a_hi0, (uint32_t)j * a_tap), a_k8, a_lo_off, b_hi0, (uint32_t)pl.b_plane_bytes, cb | j, nk8);
-          wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
+          const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
+          // the wait inside each branch: joined before it, the paths would leave the tap as two commit groups (tc::tap_chain)
+          if (nk8 == NK8) {
+            tap_chain<MODE, BN, NK8>(acc, a_j, a_k8, a_lo_off, b_hi0, (uint32_t)pl.b_plane_bytes, cb | j);
+            wgmma_wait<1>();        // the previous tap's chain has completed: its stages may be refilled
+          } else {
+            tap_chain_short<MODE, BN>(acc, a_j, a_k8, a_lo_off, b_hi0, (uint32_t)pl.b_plane_bytes, cb | j, nk8);
+            wgmma_wait<1>();
+          }
           rel.step(sb, j == K - 1 ? sa : -1);
         }
       }

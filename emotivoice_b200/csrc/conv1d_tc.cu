@@ -125,7 +125,8 @@ __device__ __forceinline__ void splitk_reduce_store(const ConvParams& p, int S, 
 // MODE 1: "3xTF32" fp32 emulation: x = hi + lo with hi = tf32(x), lo = tf32(x - hi), three MMAs per K step into the same fp32
 //                 accumulator.  Weights arrive pre-split (two planes, packing.to_tc_layout); activations are split by the producer warps.
 // MT: 128-row accumulator tiles per CTA tile.  KBG: 16-byte K granules (4 tf32 or 8 bf16 channels each) per pipeline stage.
-template <int MODE, int MT, int KBG>
+// BN = pl.BN, the N tile: fixed at compile time, so a tap of a full channel block is one unbroken wgmma chain (tc::tap_chain).
+template <int MODE, int MT, int KBG, int BN>
 __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Plan pl) {
   constexpr bool SPLIT3 = (MODE == 1);
   constexpr bool X3B = (MODE == 3);       // "bf16x3": fp32 operands split into bf16 hi + lo planes, three bf16 MMAs per K = 16 step
@@ -133,14 +134,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
   constexpr int PLANES = (SPLIT3 || X3B) ? 2 : 1;
   constexpr int CPG = BF16 ? 8 : 4;       // channels per 16-byte granule
   constexpr int KB = CPG * KBG;
+  constexpr int NK8 = KBG / 2;            // MMA K steps of a full channel block: two 16-byte granules each
   constexpr int GSH = (KBG == 8 ? 3 : 2);
-  constexpr int NA = ACC_REGS / MT;       // accumulator registers per 128-row tile
+  constexpr int NA = BN / 2;              // accumulator registers per 128-row tile: BN columns x 64 rows over 128 threads
   constexpr int NCW = NCONS / 32;         // consumer warps: every one of them releases each stage
+  static_assert(BN % 16 == 0 && MT * BN <= 2 * ACC_REGS, "accumulators of the tile exceed the register budget");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: ptxas serialises every wgmma on a path it cannot prove uniform
   const int lane = tid & 31;
-  const int BN = pl.BN;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* a_tiles = smem_raw + 1024;
@@ -194,7 +196,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
     const int oact = split ? EV_ACT_NONE : p.out_act, accm = split ? EV_ACC_STORE : p.acc;
     const uint32_t a_lbo = (uint32_t)pl.rows_pad * 16u, b_lbo = (uint32_t)BN * 16u;
     const uint64_t a_desc0 = make_desc(0u, a_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
-    const uint32_t a_tap = (uint32_t)p.dil * 16u, a_k8 = 2u * a_lbo, b_k8 = 2u * b_lbo;
+    const uint32_t a_tap = (uint32_t)p.dil * 16u, a_k8 = 2u * a_lbo;
     float acc[MT][NA];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
@@ -226,21 +228,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv1d_tc_kernel(ConvParams p, Pl
             const int sb = b_cnt % pl.b_stages;
             mbar_wait(b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b_hi0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
+            // the tap's nk8 K steps x MT accumulators as one chain; the K-split slice's first tap overwrites the accumulators.  The
+            // wait inside each branch: joined before it, the paths would leave the tap as two commit groups (tc::tap_chain)
             const uint64_t a_j = desc_advance(a_hi0, (uint32_t)j * a_tap);
-            wgmma_fence();
-            for (int k8 = 0; k8 < nk8; ++k8) {
-              const uint64_t b_hi = desc_advance(b_hi0, (uint32_t)k8 * b_k8);
-              const uint64_t b_lo = desc_advance(b_hi, (uint32_t)pl.b_plane_bytes);
-              const uint64_t a_k = desc_advance(a_j, (uint32_t)k8 * a_k8);
-              const uint32_t first = ((cb - cb_lo) | j | k8) != 0 ? 1u : 0u;
-#pragma unroll
-              for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
-                const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-                mma_step<MODE, NA>(nt, acc[mt], a_hi, desc_advance(a_hi, (uint32_t)pl.a_plane_bytes), b_hi, b_lo, first);
-              }
+            if (nk8 == NK8) {
+              tap_chain<MODE, BN, NK8>(acc, a_j, a_k8, (uint32_t)pl.a_plane_bytes, b_hi0, (uint32_t)pl.b_plane_bytes, (cb - cb_lo) | j);
+              wgmma_wait<1>();        // the previous step's MMAs have completed: its stages may be refilled
+            } else {
+              tap_chain_short<MODE, BN>(acc, a_j, a_k8, (uint32_t)pl.a_plane_bytes, b_hi0, (uint32_t)pl.b_plane_bytes, (cb - cb_lo) | j, nk8);
+              wgmma_wait<1>();
             }
-            wgmma_commit();
-            wgmma_wait<1>();          // the previous step's MMAs have completed: its stages may be refilled
             if (prev_sb >= 0) release(prev_sb, prev_sa);
             prev_sb = sb;
             prev_sa = j == p.K - 1 ? sa : -1;
@@ -430,31 +427,42 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(ConvParams p, int S)
 
 }  // namespace tc
 
-template <int MODE, int MT, int KBG>
-static int launch_tc_variant(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
-  static std::atomic<uint64_t> attr_devs{0};   // per instantiation; function attributes are per device
-  if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, MT, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  const int grid = pl.total_tiles < sm_count() ? pl.total_tiles : sm_count();
-  return launch("conv1d_tc_kernel", tc::conv1d_tc_kernel<MODE, MT, KBG>, (unsigned)grid, tc::NTHREADS, pl.smem_total, st, p, pl);
+// The instantiations: every (MODE, KBG) the shape rule tc_shape_kbg gives (KBG = 4 in 3xTF32) times every tile plan_conv1d_tc can
+// return.  BN starts at min(C_out, 128) and halves while it stays a multiple of 16 (so any multiple of 16 up to 128), MT halves until
+// MT * BN <= 128: 14 tiles per (MODE, KBG), 98 kernels.
+using TcKernel = void (*)(ConvParams, tc::Plan);
+template <int MODE, int KBG>
+static TcKernel tc_kernel_tile(int mt, int bn) {
+  using namespace tc;
+  switch (bn) {
+    case 128: return mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 128> : nullptr;
+    case 112: return mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 112> : nullptr;
+    case 96: return mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 96> : nullptr;
+    case 80: return mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 80> : nullptr;
+    case 64: return mt == 2 ? conv1d_tc_kernel<MODE, 2, KBG, 64> : mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 64> : nullptr;
+    case 48: return mt == 2 ? conv1d_tc_kernel<MODE, 2, KBG, 48> : mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 48> : nullptr;
+    case 32: return mt == 4 ? conv1d_tc_kernel<MODE, 4, KBG, 32> : mt == 2 ? conv1d_tc_kernel<MODE, 2, KBG, 32>
+                  : mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 32> : nullptr;
+    case 16: return mt == 4 ? conv1d_tc_kernel<MODE, 4, KBG, 16> : mt == 2 ? conv1d_tc_kernel<MODE, 2, KBG, 16>
+                  : mt == 1 ? conv1d_tc_kernel<MODE, 1, KBG, 16> : nullptr;
+    default: return nullptr;
+  }
+}
+static TcKernel tc_kernel(int mode, int kbg, int mt, int bn) {
+  if (mode == 1) return kbg == 4 ? tc_kernel_tile<1, 4>(mt, bn) : nullptr;
+  if (mode == 3) return kbg == 8 ? tc_kernel_tile<3, 8>(mt, bn) : tc_kernel_tile<3, 4>(mt, bn);
+  if (mode == 2) return kbg == 8 ? tc_kernel_tile<2, 8>(mt, bn) : tc_kernel_tile<2, 4>(mt, bn);
+  return kbg == 8 ? tc_kernel_tile<0, 8>(mt, bn) : tc_kernel_tile<0, 4>(mt, bn);
 }
 
-template <int MODE, int KBG>
-static int launch_tc_mt(const ConvParams& p, const tc::Plan& pl, cudaStream_t st) {
-  if (pl.mt == 4) return launch_tc_variant<MODE, 4, KBG>(p, pl, st);
-  if (pl.mt == 2) return launch_tc_variant<MODE, 2, KBG>(p, pl, st);
-  return launch_tc_variant<MODE, 1, KBG>(p, pl, st);
-}
-
-template <int MODE, int KBG>
-static void preload_tc_mode() {
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 1, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 2, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(tc::conv1d_tc_kernel<MODE, 4, KBG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-}
-void preload_conv1d_tc() {      // see conv1d_gp.cu: preload_conv1d_gp
-  preload_tc_mode<0, 4>(); preload_tc_mode<0, 8>(); preload_tc_mode<1, 4>(); preload_tc_mode<2, 4>(); preload_tc_mode<2, 8>();
-  preload_tc_mode<3, 4>(); preload_tc_mode<3, 8>();
+// Load every instantiation's code now and set the shared-memory attribute (see conv1d_gp.cu: preload_conv1d_gp), on exactly the
+// instantiations dispatch_tc can launch.
+void preload_conv1d_tc() {
+  for (int mode = 0; mode < 4; ++mode)
+    for (int kbg = 4; kbg <= 8; kbg += 4)
+      for (int bn = 16; bn <= 128; bn += 16)
+        for (int mt = 1; mt <= 4 && mt * bn <= 128; mt *= 2)
+          if (const TcKernel k = tc_kernel(mode, kbg, mt, bn)) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   cudaFuncAttributes fa;
   cudaFuncGetAttributes(&fa, tc::splitk_reduce_kernel);
   cudaGetLastError();
@@ -536,10 +544,12 @@ int debug_tc_plan(const ConvParams& p, int mode, int* v) {
 }
 
 static int dispatch_tc(const ConvParams& p, int mode, const tc::Plan& pl, cudaStream_t st) {
-  if (mode == 1) return launch_tc_mt<1, 4>(p, pl, st);
-  if (mode == 3) return pl.kbg == 8 ? launch_tc_mt<3, 8>(p, pl, st) : launch_tc_mt<3, 4>(p, pl, st);
-  if (mode == 2) return pl.kbg == 8 ? launch_tc_mt<2, 8>(p, pl, st) : launch_tc_mt<2, 4>(p, pl, st);
-  return pl.kbg == 8 ? launch_tc_mt<0, 8>(p, pl, st) : launch_tc_mt<0, 4>(p, pl, st);
+  static std::atomic<uint64_t> attr_devs{0};   // function attributes are per device
+  if (first_use_on_device(attr_devs)) preload_conv1d_tc();
+  const TcKernel k = tc_kernel(mode, pl.kbg, pl.mt, pl.BN);
+  EV_CHECK_ARG(k, "conv1d_tc: no kernel for mode %d, KBG %d, MT %d, BN %d", mode, pl.kbg, pl.mt, pl.BN);
+  const int grid = pl.total_tiles < sm_count() ? pl.total_tiles : sm_count();
+  return launch("conv1d_tc_kernel", k, (unsigned)grid, tc::NTHREADS, pl.smem_total, st, p, pl);
 }
 
 // p.w must be in the tensor-core layout [plane][Cout/BNp][K][Cin/4][BNp][4] (packing.py: to_tc_layout);

@@ -6,7 +6,7 @@
 //   warps 8-11            transform: an in-place pass over the landed stage (LeakyReLU, zeros outside [0, len), the MODE's tf32
 //                         rounding or hi / lo split), fence.proxy.async -> a_ready
 //   warp 13, one lane     weight loader: one weight stage per (channel block, tap), in the order the consumers read them -> b_full
-//   warps 0-7             consumers: per tap one wgmma chain over a channel block, then -- one tap behind, once wgmma.wait_group 1 has
+//   warps 0-7             consumers: per tap one wgmma chain over a channel block (tc::tap_chain), then -- one tap behind, once wgmma.wait_group 1 has
 //                         seen the previous chain complete -- that chain's weight stage -> b_empty and, after a block's last tap, its
 //                         x stage -> a_empty
 // Every role walks the same tiles and channel blocks and counts stages the same way (slot = count % stages, parity = count /
@@ -217,38 +217,8 @@ __device__ __forceinline__ void load_w_tile(Ring<MAX_A> ring, int& b_cnt, int b_
   }
 }
 
-// Consumers, one tap over one channel block: NK K steps x MT accumulators of mma_step_fixed as one chain between a fence and a commit.
-// a: the A descriptor at this tap and warpgroup; a_step: A bytes per K step; a_lo: offset of the A lo operand; b: the weight stage's
-// descriptor (N columns, so 2 N granules per K step); b_lo: offset of its lo plane.  cbj = channel block | tap: 0 on a tile's first
-// tap, whose first MMAs overwrite the accumulators.  nk < NK: the short last block of a C_in that is not a multiple of the block
-// (conv_pre's 80), the same K step in a run-time loop.
-template <int MODE, int N, int NK, int MT, int NA>
-__device__ __forceinline__ void tap_chain(float (&acc)[MT][NA], uint64_t a, uint32_t a_step, uint32_t a_lo, uint64_t b, uint32_t b_lo, int cbj,
-                                          int nk = NK) {
-  auto k_step = [&](int k) {
-    const uint64_t b_hi = desc_advance(b, (uint32_t)k * (2u * N * 16u));
-    const uint64_t b_lo_k = desc_advance(b_hi, b_lo);
-    const uint64_t a_k = desc_advance(a, (uint32_t)k * a_step);
-    const uint32_t first = (cbj | k) != 0 ? 1u : 0u;
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {      // one weight tile feeds MT accumulators
-      const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
-      mma_step_fixed<MODE, N>(acc[mt], a_hi, desc_advance(a_hi, a_lo), b_hi, b_lo_k, first);
-    }
-  };
-  wgmma_fence();
-  if (nk == NK) {
-#pragma unroll
-    for (int k = 0; k < NK; ++k) k_step(k);
-  } else {
-#pragma unroll 1
-    for (int k = 0; k < nk; ++k) k_step(k);
-  }
-  wgmma_commit();
-}
-
-// Consumers: a tap's stages go back one tap behind its issue.  After a tap_chain that read weight stage sb (and x stage sa >= 0 on a
-// channel block's last tap) the kernel runs wgmma_wait<1>() -- the PREVIOUS chain has completed, so its operands are no longer read --
+// Consumers: each tap is one tc::tap_chain (tc_common.cuh), and a tap's stages go back one tap behind its issue.  After a tap_chain
+// that read weight stage sb (and x stage sa >= 0 on a channel block's last tap) the kernel runs wgmma_wait<1>() -- the PREVIOUS chain has completed, so its operands are no longer read --
 // then step(sb, sa), which hands the previous chain's stages back and remembers this one's.  After a tile's last chain: the
 // epilogue's first loads, wgmma_wait<0>(), then drain().  The waits stay in each kernel's own source, where its wgmma.wait_group
 // sites -- the bound tests/test_wgmma_pipeline_sass.py puts on its WARPGROUP.DEPBAR count -- can be read.

@@ -201,51 +201,25 @@ __device__ __forceinline__ void wgmma_bf16_n128(float* d, uint64_t a, uint64_t b
                : "l"(a), "l"(b), "r"(acc));
 }
 
-// D = A * B with the instruction's N chosen at run time (any multiple of 16 up to 2 * NA; warp-uniform branch).  NA: the
-// accumulator registers the caller holds for this tile, so accumulators of narrower tiles need no registers they never use.
-template <bool BF16, int NA>
-__device__ __forceinline__ void wgmma_n(int n, float (&d)[NA], uint64_t a, uint64_t b, uint32_t acc) {
-#define EV_WG_CASE(N)                                                    \
-  case N:                                                                \
-    if constexpr (2 * NA >= N) {                                         \
-      if (BF16) wgmma_bf16_n##N(d, a, b, acc); else wgmma_tf32_n##N(d, a, b, acc); \
-    }                                                                    \
-    break;
-  switch (n) {
-    EV_WG_CASE(16) EV_WG_CASE(32) EV_WG_CASE(48) EV_WG_CASE(64) EV_WG_CASE(80) EV_WG_CASE(96) EV_WG_CASE(112) EV_WG_CASE(128)
-    default: break;
-  }
-#undef EV_WG_CASE
-}
-
-// D = A * B with the instruction's N fixed at compile time (a multiple of 32 up to 2 * NA).
+// D = A * B with the instruction's N fixed at compile time (a multiple of 16 up to 2 * NA).  Every convolution kernel fixes N
+// this way: with N chosen at run time each MMA went through a jump table, and ptxas fenced it with its own warpgroup.arrive.
 template <bool BF16, int N, int NA>
 __device__ __forceinline__ void wgmma_fixed(float (&d)[NA], uint64_t a, uint64_t b, uint32_t acc) {
-  static_assert(N % 32 == 0 && N <= 128 && N <= 2 * NA, "N tile must be 32 / 64 / 96 / 128 and fit the accumulator");
-  if constexpr (N == 32) { if constexpr (BF16) wgmma_bf16_n32(d, a, b, acc); else wgmma_tf32_n32(d, a, b, acc); }
+  static_assert(N % 16 == 0 && N >= 16 && N <= 128 && N <= 2 * NA, "N tile must be a multiple of 16 up to 128 and fit the accumulator");
+  if constexpr (N == 16) { if constexpr (BF16) wgmma_bf16_n16(d, a, b, acc); else wgmma_tf32_n16(d, a, b, acc); }
+  else if constexpr (N == 32) { if constexpr (BF16) wgmma_bf16_n32(d, a, b, acc); else wgmma_tf32_n32(d, a, b, acc); }
+  else if constexpr (N == 48) { if constexpr (BF16) wgmma_bf16_n48(d, a, b, acc); else wgmma_tf32_n48(d, a, b, acc); }
   else if constexpr (N == 64) { if constexpr (BF16) wgmma_bf16_n64(d, a, b, acc); else wgmma_tf32_n64(d, a, b, acc); }
+  else if constexpr (N == 80) { if constexpr (BF16) wgmma_bf16_n80(d, a, b, acc); else wgmma_tf32_n80(d, a, b, acc); }
   else if constexpr (N == 96) { if constexpr (BF16) wgmma_bf16_n96(d, a, b, acc); else wgmma_tf32_n96(d, a, b, acc); }
+  else if constexpr (N == 112) { if constexpr (BF16) wgmma_bf16_n112(d, a, b, acc); else wgmma_tf32_n112(d, a, b, acc); }
   else { if constexpr (BF16) wgmma_bf16_n128(d, a, b, acc); else wgmma_tf32_n128(d, a, b, acc); }
 }
 
-// One K step of the convolution kernels' modes into one accumulator.  MODE 0: one tf32 MMA; 2: one bf16 MMA; 1 ("3xTF32") / 3
-// ("bf16x3"): operands split into hi + lo, a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (small terms first, the dropped lo*lo term is
-// below fp32 rounding), three MMAs into the same fp32 accumulator.
-template <int MODE, int NA>
-__device__ __forceinline__ void mma_step(int n, float (&d)[NA], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t acc) {
-  constexpr bool OP16 = MODE >= 2;
-  if (MODE == 1 || MODE == 3) {
-    wgmma_n<OP16, NA>(n, d, a_lo, b_hi, acc);
-    wgmma_n<OP16, NA>(n, d, a_hi, b_lo, 1u);
-    wgmma_n<OP16, NA>(n, d, a_hi, b_hi, 1u);
-  } else {
-    wgmma_n<OP16, NA>(n, d, a_hi, b_hi, acc);
-  }
-}
-
-// mma_step with N fixed at compile time (the granule-planar kernels): every MMA is one wgmma, so the MMAs of a whole channel
-// block form one unbroken chain between a fence and a commit -- the run-time switch above splits them with a branch and a
-// warpgroup.arrive per K step.  Same MMAs in the same order.
+// One K step of the convolution kernels' modes into one accumulator, N fixed at compile time.  MODE 0: one tf32 MMA; 2: one bf16
+// MMA; 1 ("3xTF32") / 3 ("bf16x3"): operands split into hi + lo, a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (small terms first, the
+// dropped lo*lo term is below fp32 rounding), three MMAs into the same fp32 accumulator.  Every MMA is one wgmma, so the MMAs of a
+// whole channel block form one unbroken chain between a fence and a commit.
 template <int MODE, int N, int NA>
 __device__ __forceinline__ void mma_step_fixed(float (&d)[NA], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t acc) {
   constexpr bool OP16 = MODE >= 2;
@@ -256,6 +230,54 @@ __device__ __forceinline__ void mma_step_fixed(float (&d)[NA], uint64_t a_hi, ui
   } else {
     wgmma_fixed<OP16, N>(d, a_hi, b_hi, acc);
   }
+}
+
+// One K step k of a tap into the MT accumulators (one weight tile feeds all of them).  a: the A descriptor at this tap and
+// warpgroup; a_step: A bytes per K step; a_lo: offset of the A lo operand; b: the weight stage's descriptor (N columns, so 2 N
+// granules per K step); b_lo: offset of its lo plane.  cbj = channel block | tap: 0 on a tile's first tap, whose first MMAs
+// overwrite the accumulators.
+template <int MODE, int N, int MT, int NA>
+__device__ __forceinline__ void tap_k_step(float (&acc)[MT][NA], uint64_t a, uint32_t a_step, uint32_t a_lo, uint64_t b, uint32_t b_lo,
+                                           int cbj, int k) {
+  const uint64_t b_hi = desc_advance(b, (uint32_t)k * (2u * N * 16u));
+  const uint64_t b_lo_k = desc_advance(b_hi, b_lo);
+  const uint64_t a_k = desc_advance(a, (uint32_t)k * a_step);
+  const uint32_t first = (cbj | k) != 0 ? 1u : 0u;
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt) {
+    const uint64_t a_hi = desc_advance(a_k, (uint32_t)(mt * BM) * 16u);
+    mma_step_fixed<MODE, N>(acc[mt], a_hi, desc_advance(a_hi, a_lo), b_hi, b_lo_k, first);
+  }
+}
+
+// Consumers of the convolution kernels (conv1d_tc.cu, conv1d_gp.cu, resblock_gp.cu), one tap over a full channel block: NK K steps
+// x MT accumulators of mma_step_fixed as one chain between a fence and a commit (arguments: tap_k_step).
+//
+// A C_in that is not a multiple of the block (conv_pre's 80 channels, any such C_in at the conv1d_tc C ABI) ends in a short block:
+// tap_chain_short.  The kernel picks one of the two per channel block and runs its wgmma_wait<1>() inside the same branch.  Where
+// the two paths join before the commit instead, the commit opens a second commit group at the join, which ptxas closes with an
+// empty no-op HGMMA (gsb0): each tap is then two groups, and `wgmma.wait_group 1` after it waits for the tap's real MMAs, so every
+// tap drained the tensor core before the next one was queued.  Where they join between commit and wait, the compiler copies the
+// wait into both paths anyway; writing it there keeps the source's wait sites equal to the WARPGROUP.DEPBAR in the SASS.
+template <int MODE, int N, int NK, int MT, int NA>
+__device__ __forceinline__ void tap_chain(float (&acc)[MT][NA], uint64_t a, uint32_t a_step, uint32_t a_lo, uint64_t b, uint32_t b_lo, int cbj) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < NK; ++k) tap_k_step<MODE, N>(acc, a, a_step, a_lo, b, b_lo, cbj, k);
+  wgmma_commit();
+}
+
+// The short last block: nk K steps (1 <= nk < NK) in a run-time loop, a fence on every trip (a wgmma after a loop head with no fence
+// of its own gets a warpgroup.arrive injected by ptxas, warning C7519), one commit.
+template <int MODE, int N, int MT, int NA>
+__device__ __forceinline__ void tap_chain_short(float (&acc)[MT][NA], uint64_t a, uint32_t a_step, uint32_t a_lo, uint64_t b, uint32_t b_lo,
+                                                int cbj, int nk) {
+#pragma unroll 1
+  for (int k = 0; k < nk; ++k) {
+    wgmma_fence();
+    tap_k_step<MODE, N>(acc, a, a_step, a_lo, b, b_lo, cbj, k);
+  }
+  wgmma_commit();
 }
 
 }  // namespace tc
