@@ -64,6 +64,7 @@ SIGNATURES = {
                                    _sz, _vp]),
     "ev_am_phase2": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_vocoder": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
+    "ev_join_mel": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "ev_wav_to_pcm16": (_i, [_vp, _vp, _sz, _vp]),
     "ev_launch_count": (_u64, []),
     "ev_op_conv1d": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp]),

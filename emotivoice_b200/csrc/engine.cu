@@ -669,7 +669,9 @@ int ev_create(ev_ctx** out, int device, const ev_config* cfg) {
     int prev = -1;
     cudaGetDevice(&prev);
     if (prev != device) cudaSetDevice(device);
-    if (first_use_on_device(loaded)) { preload_conv1d_gp(); preload_resblock_gp(); preload_attention_tc(); preload_conv1d_tc(); }
+    if (first_use_on_device(loaded)) {
+      preload_conv1d_gp(); preload_resblock_gp(); preload_attention_tc(); preload_conv1d_tc(); preload_voc_kernels();
+    }
     if (prev >= 0 && prev != device) cudaSetDevice(prev);
     cudaGetLastError();
   }
@@ -925,6 +927,13 @@ int ev_vocoder(ev_ctx* ctx, const float* mel, int mel_time_major, const int32_t*
   EV_CHECK_ARG(mul == ctx->total_up, "ev_vocoder: internal rate mismatch");
   // x = leaky_relu(x) [slope 0.01]; conv_post; tanh (:127-129)
   return launch_conv_post_gp(v.ACC, bf, ctx->post_w, ctx->post_b, mel_lens, mul, B, L, ctx->ups.back().cout, ctx->post_k, 0.01f, wav_out, st);
+}
+
+int ev_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* group, int B, int F, int n_mels, int G, int Fg, float* joined,
+                int32_t* group_lens, void* stream) {
+  EV_CHECK_ARG(mel && mel_lens && group && joined && group_lens, "ev_join_mel: null argument");
+  EV_TRY(use_device_of(mel));
+  return launch_join_mel(mel, mel_lens, group, B, F, n_mels, G, Fg, joined, group_lens, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ev_wav_to_pcm16(const float* wav, int16_t* pcm, size_t n, void* stream) {

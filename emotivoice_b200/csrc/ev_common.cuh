@@ -249,6 +249,11 @@ int launch_transpose_cf_to_tm(const float* in, float* out, int B, int C, int L, 
 int launch_conv_post(const float* x, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B,
                      int L, int C, int K, float slope, float* wav, cudaStream_t st);
 int launch_pcm16(const float* wav, int16_t* pcm, size_t n, cudaStream_t st);
+// valid rows of mel (B,F,C) of consecutive items with one group id, concatenated -> joined (G,Fg,C), zero past each group's
+// length; group_lens[g] = min(group frames, Fg).  B <= 4096.
+int launch_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* group, int B, int F, int C, int G, int Fg, float* joined,
+                    int32_t* group_lens, cudaStream_t st);
+void preload_voc_kernels();
 
 __device__ __forceinline__ float act_apply(float v, int act, float slope) {
   switch (act) {

@@ -82,6 +82,82 @@ int launch_conv_post(const float* x, const float* w, const float* bias, const in
   return launch("conv_post_kernel", conv_post_kernel, grid, CP_BT, smem, st, x, w, bias, lens, lens_mul, L, C, K, slope, wav);
 }
 
+// Joined mel of long-text synthesis: the valid rows mel[b, :mel_lens[b]] of consecutive items with one group id, concatenated in
+// item order, -> joined (G, Fg, C) time-major, rows past a group's length zero; group_lens[g] = min(frames of group g, Fg).
+// Every CTA scans the B lengths into item offsets in shared memory (B <= JM_MAX_ITEMS), then copies JM_ROWS output rows, each
+// from the item a binary search over the offsets finds.  `group` must be non-decreasing from 0 in steps of 0 or 1 up to G - 1;
+// other ids give an unspecified result but no out-of-bounds access.
+constexpr int JM_THREADS = 256, JM_ROWS = 64, JM_MAX_ITEMS = 4096;
+__global__ void __launch_bounds__(JM_THREADS) join_mel_kernel(const float* __restrict__ mel, const int32_t* __restrict__ mel_lens,
+                                                              const int32_t* __restrict__ group, int B, int F, int C, int G, int Fg,
+                                                              float* __restrict__ joined, int32_t* __restrict__ group_lens) {
+  pdl_entry();
+  extern __shared__ int jm_smem[];
+  int* off = jm_smem;              // [B + 1]: first joined row of item b, counted over all items
+  int* first = off + B + 1;        // [G + 1]: first item of group g; first[G] = B
+  __shared__ int part[JM_THREADS];
+  const int per = (B + JM_THREADS - 1) / JM_THREADS;
+  const int b0 = min(B, (int)threadIdx.x * per), b1 = min(B, b0 + per);
+  int s = 0;
+  for (int b = b0; b < b1; ++b) s += min(max(mel_lens[b], 0), F);
+  part[threadIdx.x] = s;
+  for (int g = threadIdx.x; g <= G; g += JM_THREADS) first[g] = B;
+  __syncthreads();
+  for (int d = 1; d < JM_THREADS; d <<= 1) {       // inclusive scan of the per-thread sums
+    const int v = (int)threadIdx.x >= d ? part[threadIdx.x - d] : 0;
+    __syncthreads();
+    part[threadIdx.x] += v;
+    __syncthreads();
+  }
+  int o = threadIdx.x ? part[threadIdx.x - 1] : 0;
+  for (int b = b0; b < b1; ++b) {
+    off[b] = o;
+    o += min(max(mel_lens[b], 0), F);
+  }
+  if (threadIdx.x == JM_THREADS - 1) off[B] = part[JM_THREADS - 1];
+  for (int b = threadIdx.x; b < B; b += JM_THREADS) {
+    const int g = group[b];
+    if (g >= 0 && g < G && (b == 0 || group[b - 1] != g)) first[g] = b;
+  }
+  __syncthreads();
+  if (blockIdx.x == 0)
+    for (int g = threadIdx.x; g < G; g += JM_THREADS) group_lens[g] = min(max(off[max(first[g + 1], first[g])] - off[first[g]], 0), Fg);
+  const int c4n = C / 4;
+  const long long rows = (long long)G * Fg;
+  for (int i = threadIdx.x; i < JM_ROWS * c4n; i += JM_THREADS) {
+    const long long r = (long long)blockIdx.x * JM_ROWS + i / c4n;
+    if (r >= rows) break;
+    const int g = (int)(r / Fg), f = (int)(r % Fg), c4 = i % c4n;
+    const int s0 = first[g], e = max(first[g + 1], s0);
+    const int pos = off[s0] + f;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (s0 < e && pos < off[e]) {
+      int lo = s0, hi = e - 1;                       // the last item of the group whose offset is <= pos
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= pos) lo = mid; else hi = mid - 1;
+      }
+      v = __ldg(reinterpret_cast<const float4*>(mel + ((size_t)lo * F + (pos - off[lo])) * C) + c4);
+    }
+    reinterpret_cast<float4*>(joined + (size_t)r * C)[c4] = v;
+  }
+}
+int launch_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* group, int B, int F, int C, int G, int Fg, float* joined,
+                    int32_t* group_lens, cudaStream_t st) {
+  EV_CHECK_ARG(B > 0 && B <= JM_MAX_ITEMS, "join_mel: B=%d must lie in [1, %d]", B, JM_MAX_ITEMS);
+  EV_CHECK_ARG(G > 0 && G <= B && F > 0 && Fg > 0 && C > 0 && C % 4 == 0, "join_mel: B=%d G=%d F=%d Fg=%d n_mels=%d", B, G, F, Fg, C);
+  EV_CHECK_ARG((long long)B * F < (1ll << 31) && (long long)G * Fg < (1ll << 31), "join_mel: B*F or G*Fg reaches 2^31");
+  const long long blocks = ((long long)G * Fg + JM_ROWS - 1) / JM_ROWS;
+  const size_t smem = (size_t)(B + 1 + G + 1) * sizeof(int);
+  return launch("join_mel_kernel", join_mel_kernel, (unsigned)blocks, JM_THREADS, smem, st, mel, mel_lens, group, B, F, C, G, Fg, joined,
+                group_lens);
+}
+void preload_voc_kernels() {      // see preload_conv1d_gp
+  cudaFuncAttributes fa;
+  cudaFuncGetAttributes(&fa, join_mel_kernel);
+  cudaGetLastError();
+}
+
 // pcm = (int16) trunc(wav * 32768): numpy astype('int16') of a float array is a C cast
 // (inference_am_vocoder_joint.py:130-131).  Values are inside (-1, 1) after tanh.
 __global__ void pcm16_kernel(const float* __restrict__ wav, int16_t* __restrict__ pcm, size_t n) {

@@ -53,6 +53,64 @@ def encode(req, token2id, speaker2id):
     return ids, int(speaker2id[req.speaker])
 
 
+# ---- long text: phoneme lines cut into segments that are each an utterance of their own -----------------------------------
+
+SOS_EOS = "<sos/eos>"           # the edge token every frontend line starts and ends with (frontend.py:28,57, frontend_cn.py:103,120)
+# Break tokens the reference frontends emit.  Punctuation: frontend_cn.py:110-112 turns every punctuation mark into sp3,
+# frontend_en.py:69-71 emits engsp4; sp4 and the English marks close sentences too.  Word and language boundaries: the rest.
+PUNCTUATION_BREAKS = frozenset({"sp3", "sp4", "engsp4", ".", "?", "!"})
+WORD_BREAKS = frozenset({"sp1", "sp2", "engsp1", "engsp2", "cn_eng_sp", "eng_cn_sp"})
+
+
+def split_phonemes(phonemes, max_phonemes=256):
+    """Cut a phoneme line (token strings, as ``parse_line`` yields them) into segments of at most ``max_phonemes`` tokens,
+    each wrapped as ``<sos/eos> ... <sos/eos>`` like a frontend line, for ``JETSGenerator.forward(join=...)`` /
+    ``MicroBatcher.submit_joined``.
+
+    One leading and one trailing ``<sos/eos>`` are stripped; an inner ``<sos/eos>`` forces a cut and is dropped, so several
+    frontend lines put together fall apart at their edges.  Greedily, a window of at most ``max_phonemes - 2`` inner tokens is
+    cut after its last punctuation break (``PUNCTUATION_BREAKS``), else after its last word break (``WORD_BREAKS``), else at its
+    end; the break token stays at the end of the left segment.  Joining the segments' inner tokens gives back the input's
+    inner tokens (less the inner ``<sos/eos>``), and a wrapped line of at most ``max_phonemes`` tokens with no inner
+    ``<sos/eos>`` comes back whole.  The default keeps every line of the reference's inference text whole (the longest has 223
+    tokens).  Raises ValueError for ``max_phonemes < 3`` or an input with no inner token."""
+    max_phonemes = int(max_phonemes)
+    if max_phonemes < 3:
+        raise ValueError("max_phonemes must be >= 3 (two <sos/eos> edges and one token), got %d" % max_phonemes)
+    toks = list(phonemes)
+    if toks and toks[0] == SOS_EOS:
+        toks = toks[1:]
+    if toks and toks[-1] == SOS_EOS:
+        toks = toks[:-1]
+    runs, cur = [], []
+    for t in toks:
+        if t != SOS_EOS:
+            cur.append(t)
+        elif cur:
+            runs.append(cur)
+            cur = []
+    if cur:
+        runs.append(cur)
+    if not runs:
+        raise ValueError("the phoneme line holds no token between its <sos/eos> edges")
+    width = max_phonemes - 2
+    segments = []
+    for run in runs:
+        i = 0
+        while len(run) - i > width:
+            window = run[i:i + width]
+            cut = width                      # tokens the left segment keeps
+            for breaks in (PUNCTUATION_BREAKS, WORD_BREAKS):
+                at = [k for k, t in enumerate(window) if t in breaks]
+                if at:
+                    cut = at[-1] + 1
+                    break
+            segments.append(run[i:i + cut])
+            i += cut
+        segments.append(run[i:])
+    return [[SOS_EOS] + s + [SOS_EOS] for s in segments]
+
+
 NEUTRAL_CONTROLS = (1.0, 0.0, 1.0)      # (duration_scale, pitch_shift, energy_scale)
 
 
@@ -194,6 +252,11 @@ class MicroBatcher:
     Errors of a batch are delivered to every future of that batch.  Requests with different prosody controls
     (``speed``, ``pitch_shift``, ``energy_scale``, per item or per phoneme) share one forward.  Requests that give their
     own ``durations`` / ``pitch`` / ``energy`` run in one forward with the requests that give the same set of tracks.
+
+    ``submit_joined`` takes a long text as segments (``split_phonemes``): they enter a forward as consecutive items of one
+    ``join`` group, so the text comes back as one waveform; plain requests of that forward each get a group of their own.
+    ``max_batch`` counts items.  A joined request is never split across forwards; one with more segments than ``max_batch``
+    runs alone.  A forward without a joined request is called exactly as before, with no ``join`` keyword.
     """
 
     def __init__(self, forward, device="cpu", max_batch=32, max_wait_s=0.005, hop=256):
@@ -217,11 +280,29 @@ class MicroBatcher:
         controls = phoneme_controls(len(ids), speed, pitch_shift, energy_scale)
         given = given_values(len(ids), durations, pitch, energy)
         item = (ids, int(speaker_id), style_vec, content_vec, controls) + ((given,) if given else ())
+        return self._enqueue([item], False)
+
+    def submit_joined(self, segments, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+        """One long text as ``segments``: a list of phoneme id arrays, e.g. ``split_phonemes`` output put through ``encode``.
+        ``style_vec`` / ``content_vec``: one vector for every segment, or a list (or a 2-D array) with one vector per segment,
+        for a different prompt per sentence.  ``speed`` / ``pitch_shift`` / ``energy_scale``: one float each, checked as in
+        ``submit``.  The future's result is the text's float32 waveform, the segments' mel joined and vocoded as one,
+        trimmed to ``joined_lengths[g] * hop``.  Raises ValueError here for invalid arguments."""
+        segs = [np.asarray(s, dtype=np.int64) for s in segments]
+        if not segs or any(s.ndim != 1 or s.size == 0 for s in segs):
+            raise ValueError("segments must be a non-empty list of non-empty 1-D phoneme id arrays")
+        controls = speech_controls(speed, pitch_shift, energy_scale)
+        styles = _per_segment("style_vec", style_vec, len(segs))
+        contents = _per_segment("content_vec", content_vec, len(segs))
+        items = [(s, int(speaker_id), st, ct, controls) for s, st, ct in zip(segs, styles, contents)]
+        return self._enqueue(items, True)
+
+    def _enqueue(self, items, joined):
         fut = Future()
         with self._lock:
             if self._closed:
                 raise RuntimeError("MicroBatcher is closed")
-            self._queue.append((item, fut))
+            self._queue.append((items, fut, joined))
             self._lock.notify()
         return fut
 
@@ -244,12 +325,16 @@ class MicroBatcher:
             if not self._queue:
                 return None
             deadline = time.monotonic() + self._max_wait
-            while len(self._queue) < self._max_batch and not self._closed:
+            while sum(len(e[0]) for e in self._queue) < self._max_batch and not self._closed:
                 left = deadline - time.monotonic()
                 if left <= 0:
                     break
                 self._lock.wait(left)
-            batch, self._queue = self._queue[:self._max_batch], self._queue[self._max_batch:]
+            n = items = 0                    # whole requests in arrival order up to max_batch items; the first one always
+            while n < len(self._queue) and (n == 0 or items + len(self._queue[n][0]) <= self._max_batch):
+                items += len(self._queue[n][0])
+                n += 1
+            batch, self._queue = self._queue[:n], self._queue[n:]
             return batch
 
     def _loop(self):
@@ -258,17 +343,22 @@ class MicroBatcher:
             if batch is None:
                 return
             groups = {}                      # one forward per set of caller-given tracks (the common case: one group)
-            for it, f in batch:
-                groups.setdefault(tuple(sorted(it[5])) if len(it) > 5 else (), []).append((it, f))
+            for its, f, joined in batch:
+                it = its[0]
+                groups.setdefault(tuple(sorted(it[5])) if len(it) > 5 else (), []).append((its, f, joined))
             for group in groups.values():
                 self._run(group)
 
     def _run(self, batch):
-        futs = [f for _, f in batch]
+        futs = [f for _, f, _ in batch]
         try:
-            out = self._forward(**collate([it for it, _ in batch], self._device))
+            kw = collate([it for its, _, _ in batch for it in its], self._device)
+            joined = any(j for _, _, j in batch)
+            if joined:                       # one group per request: a joined request's segments share its id
+                kw["join"] = [g for g, (its, _, _) in enumerate(batch) for _ in its]
+            out = self._forward(**kw)
             wav = out["wav_predictions"]
-            lens = out.get("mel_lengths")
+            lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
             lens = [int(wav.shape[-1]) // self._hop] * len(batch) if lens is None else [int(v) for v in lens.tolist()]
             wav = wav.detach().cpu()
             self.batches_run += 1
@@ -278,6 +368,19 @@ class MicroBatcher:
             for f in futs:
                 if not f.done():
                     f.set_exception(e)
+
+
+def _per_segment(name, v, n):
+    """``submit_joined``'s style / content argument -> n vectors: one vector repeated, or a list / 2-D array of n vectors."""
+    if isinstance(v, (list, tuple)) and len(v) and (getattr(v[0], "ndim", 0) >= 1 or isinstance(v[0], (list, tuple))):
+        rows = list(v)
+    elif getattr(v, "ndim", 1) == 2:
+        rows = [v[i] for i in range(v.shape[0])]
+    else:
+        return [v] * n
+    if len(rows) != n:
+        raise ValueError("%s holds %d vectors for %d segments" % (name, len(rows), n))
+    return rows
 
 
 # ---- output side (SURVEY.md s8f rank 2): the on-wire format every front-end emits -----------------------------------
@@ -300,13 +403,14 @@ def pcm16_to_wav_bytes(pcm, sample_rate=16000):
 def fetch_pcm16(model, out, hop=256):
     """Finish one forward the way the callers do (inference_am_vocoder_joint.py:130-131), without the fp32 waveform
     ever crossing PCIe: ``wav * 32768 -> int16`` on the GPU (``model.to_pcm16``), ONE device->host copy of the int16
-    batch into pinned memory, then per-item trimming to ``mel_lengths[b] * hop`` on the host.
-    ``out`` is the dict ``model(...)`` returned.  Returns a list of 1-D int16 numpy arrays (one per batch item)."""
+    batch into pinned memory, then per-item trimming to ``mel_lengths[b] * hop`` on the host (``joined_lengths_host[g] * hop``
+    for the output of a joined forward).  ``out`` is the dict ``model(...)`` returned.  Returns a list of 1-D int16 numpy
+    arrays (one per batch item, or per group of a joined forward)."""
     wav = out["wav_predictions"]
     pcm = model.to_pcm16(wav)                                              # (B, 1, 256 F) int16, device (saturating, see to_pcm16)
     host = torch.empty(pcm.shape, dtype=torch.int16, pin_memory=True)
     host.copy_(pcm, non_blocking=True)
-    lens = out.get("mel_lengths")
+    lens = out.get("joined_lengths_host", out.get("mel_lengths"))
     lens = None if lens is None else [int(v) for v in lens.tolist()]      # tiny D2H; also orders after the copy above
     torch.cuda.current_stream(pcm.device).synchronize()
     B, n = pcm.shape[0], int(pcm.shape[-1])

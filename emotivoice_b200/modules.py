@@ -152,6 +152,40 @@ def controls_for(module, inputs_ling, duration_scale, pitch_shift, energy_scale,
     return prosody, given
 
 
+JOIN_MAX_ITEMS = 4096             # items of one joined forward: ev_join_mel keeps their offsets in shared memory
+
+
+def join_groups(join, B):
+    """The ``join`` of ``forward`` -> None, or the (B,) int32 numpy group ids: a sequence or CPU tensor of B integers, 0 first,
+    each next one equal to the previous one or one more.  Raises ValueError before anything is enqueued."""
+    if join is None:
+        return None
+    if isinstance(join, torch.Tensor):
+        if join.device.type != "cpu":
+            raise ValueError("join must be a sequence or a CPU tensor (reading a %s tensor would synchronise the device)"
+                             % join.device.type)
+        join = join.detach().numpy()
+    try:
+        a = np.asarray(join)
+    except (TypeError, ValueError):
+        raise ValueError("join must hold %d integer group ids" % B) from None
+    if a.shape != (B,) or a.dtype.kind not in "iu":
+        raise ValueError("join must hold %d integer group ids (one per batch item), got %s of shape %s" % (B, a.dtype, a.shape))
+    if B > JOIN_MAX_ITEMS:
+        raise ValueError("a joined forward takes at most %d items, got %d" % (JOIN_MAX_ITEMS, B))
+    steps = np.diff(a.astype(np.int64))
+    if a[0] != 0 or np.any((steps != 0) & (steps != 1)):
+        raise ValueError("join must start at 0 and each next id must equal the previous one or one more, got %s" % a.tolist())
+    return a.astype(np.int32)
+
+
+def group_frames(group, mel_lens_host):
+    """(B,) group ids and per-item frame counts -> (G,) int64 frames of each joined output."""
+    out = np.zeros(int(group[-1]) + 1, dtype=np.int64)
+    np.add.at(out, group, np.asarray(mel_lens_host, dtype=np.int64))
+    return out
+
+
 def _bucket(nbytes):
     """Workspace sizes are rounded up to a geometric series (x1.125 steps, 2 MiB granularity): utterances of similar length
     then request IDENTICAL sizes, so torch's caching allocator serves them from its pool instead of calling cudaMalloc
@@ -289,9 +323,11 @@ class _Engine:
             pass
         return tl.pin[:n].clone()
 
-    def acoustic(self, ling, lens, spk, style, content, invariant, prosody=None, given=None):
+    def acoustic(self, ling, lens, spk, style, content, invariant, prosody=None, given=None, group=None):
         """``prosody``: None (neutral: the plain ev_am_phase1 call) or the (B,5) / (B,T,5) CPU table of ``prosody_table``;
-        ``given``: None or the caller's {"durations", "pitch", "energy"} of ``controls_for`` (each None, a CPU or a device tensor)."""
+        ``given``: None or the caller's {"durations", "pitch", "energy"} of ``controls_for`` (each None, a CPU or a device tensor);
+        ``group``: None or the (B,) int32 group ids of ``join_groups`` (a joined forward: the result then also carries the group
+        ids on the device, the group lengths on the host and on the device, and a phase-2 workspace the joined vocoder pass fits)."""
         lib, dev = self.lib, self.device
         B, T = ling.shape
         self.ensure_pe(T)
@@ -304,6 +340,7 @@ class _Engine:
             return pinned[-1].to(dev, non_blocking=True)
         prosody = upload(prosody)
         given = {k: upload(v) for k, v in (given or {}).items()}
+        group_dev = None if group is None else upload(torch.from_numpy(group))
         caller = {k: v for k, v in given.items() if v is not None}
         dur = torch.empty((B, T), dtype=torch.int64, device=dev)
         pitch = torch.empty((B, T), dtype=torch.float32, device=dev)
@@ -350,14 +387,28 @@ class _Engine:
             raise RuntimeError("duration_scale leaves an utterance with no frames (mel lengths %s); use a larger duration_scale"
                                % mel_lens_host[:B].tolist())
         F = int(mel_lens_host[B])
+        joined = {}
+        need2 = lib.ev_phase2_workspace_bytes(self.handle, B, F)
+        if group is not None:
+            frames = group_frames(group, mel_lens_host[:B].numpy())
+            if int(frames.max()) * self.total_up >= 2 ** 31:
+                raise ValueError("a joined output would have more frames than the vocoder can index (frames * %d must stay below "
+                                 "2^31); group lengths %s" % (self.total_up, frames.tolist()))
+            lens_host = torch.from_numpy(frames.astype(np.int32))
+            G, Fg = len(frames), int(frames.max())
+            # The vocoder's kernels read their lengths before they wait for the kernel ahead of them (include/emotivoice_b200.h,
+            # ev_vocoder), so the joined pass cannot take ev_join_mel's freshly written group_lens: it takes this upload, enqueued
+            # before phase 2 and so complete before the vocoder's first kernel starts.
+            joined = dict(group=group_dev, G=G, Fg=Fg, lens_host=lens_host, voc_lens=upload(lens_host))
+            need2 = max(need2, lib.ev_phase2_workspace_bytes(self.handle, G, Fg))
         self.ensure_pe(F)
-        ws2 = self._ws("p2", lib.ev_phase2_workspace_bytes(self.handle, B, F))
+        ws2 = self._ws("p2", need2)
         n2 = ws2.numel()
         mel = torch.empty((B, F, int(self.cfg.n_mels)), dtype=torch.float32, device=dev)
         _abi.check(lib.ev_am_phase2(self.handle, ws1.data_ptr(), lens32_ptr, mel_lens_ptr, B, T, F, int(invariant),
                                     mel.data_ptr(), ws2.data_ptr(), n2, st))
         return dict(mel=mel, dur=dur, pitch=pitch, energy=energy, meta=meta, mel_lens=meta[B:2 * B],
-                    mel_lens_host=mel_lens_host[:B], F=F, ws2=ws2, n2=n2)
+                    mel_lens_host=mel_lens_host[:B], F=F, ws2=ws2, n2=n2, joined=joined)
 
     def vocode(self, mel, time_major, mel_lens_ptr, ws=None, n=0):
         lib, dev = self.lib, self.device
@@ -372,6 +423,15 @@ class _Engine:
         _abi.check(lib.ev_vocoder(self.handle, mel.data_ptr(), int(bool(time_major)), mel_lens_ptr, B, F,
                                   wav.data_ptr(), ws.data_ptr(), n, self._stream()))
         return wav
+
+    def join_mel(self, mel, mel_lens, group, G, Fg):
+        """ev_join_mel: (B,F,n_mels) mel + device (B,) frame counts and group ids -> joined (G,Fg,n_mels) mel, (G,) int32 lengths."""
+        B, F, C = mel.shape
+        joined = torch.empty((G, Fg, C), dtype=torch.float32, device=self.device)
+        lens = torch.empty((G,), dtype=torch.int32, device=self.device)
+        _abi.check(self.lib.ev_join_mel(mel.data_ptr(), mel_lens.data_ptr(), group.data_ptr(), B, F, C, G, Fg, joined.data_ptr(),
+                                        lens.data_ptr(), self._stream()))
+        return joined, lens
 
 
 class _EngineOwner(nn.Module):
@@ -533,7 +593,7 @@ class PromptTTS(_EngineOwner):
                                inputs_content_embedding, not self.compat_padded_batch, prosody, given)[0]
 
 
-def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant, prosody=None, given=None):
+def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content, invariant, prosody=None, given=None, group=None):
     dev = eng.device
     ling = _prep(inputs_ling, torch.int64, dev)
     lens = _prep(input_lengths, torch.int64, dev)
@@ -547,7 +607,7 @@ def _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, style, content,
     if tuple(style.shape) != want or tuple(content.shape) != want:
         raise RuntimeError("inputs_style_embedding %s / inputs_content_embedding %s must both be %s"
                            % (tuple(style.shape), tuple(content.shape), want))
-    r = eng.acoustic(ling, lens, spk, style, content, invariant, prosody, given)
+    r = eng.acoustic(ling, lens, spk, style, content, invariant, prosody, given, group)
     out = {
         "mel_targets": None,
         "dec_outputs": r["mel"],
@@ -608,6 +668,17 @@ class JETSGenerator(_EngineOwner):
     values give bitwise the uncontrolled output.  Wrong shapes, dtypes or values raise ValueError before anything is
     enqueued.  ``alpha=`` is accepted and ignored, as in the reference's inference branch.  An utterance scaled to
     zero frames raises RuntimeError (the reference's decoder raises too).
+
+    Long text (keyword argument ``join``): one group id per batch item, a sequence or CPU tensor of B integers, 0 first and
+    each next one equal to the previous one or one more.  Consecutive items with one id are the segments of one output, in
+    order (``frontdoor.split_phonemes`` cuts a long phoneme line into such segments).  The acoustic model runs over the B items
+    exactly as without ``join``, with every control above; ``dec_outputs``, the predictions and ``mel_lengths`` stay per item.
+    The vocoder then runs once per group over the items' valid mel rows concatenated, so its receptive field spans each seam
+    and a group comes out as one continuous waveform: ``wav_predictions`` is (G, 1, hop * Fg), Fg the longest group's frames,
+    and the result also holds ``joined_mel`` (G, Fg, n_mels, zeros past a group's length), ``joined_lengths`` ((G,) int32 on
+    the device) and ``joined_lengths_host`` (the same on the host).  A group's waveform is bitwise what it gives in a forward
+    of its own.  A malformed ``join``, or ``join`` with ``compat_padded_batch``, raises ValueError before anything is
+    enqueued; a group too long for the vocoder's sample index raises ValueError before the decoder is enqueued.
     """
 
     def __init__(self, config):
@@ -627,31 +698,43 @@ class JETSGenerator(_EngineOwner):
     @torch.no_grad()
     def forward(self, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
                 mel_targets=None, output_lengths=None, pitch_targets=None, energy_targets=None, alpha=1.0,
-                cut_flag=True, duration_scale=None, pitch_shift=None, energy_scale=None, durations=None, pitch=None, energy=None):
+                cut_flag=True, duration_scale=None, pitch_shift=None, energy_scale=None, durations=None, pitch=None, energy=None,
+                join=None):
         if mel_targets is not None:
             raise NotImplementedError("training-mode forward (teacher forcing / random segments) is out of scope")
         prosody, given = controls_for(self, inputs_ling, duration_scale, pitch_shift, energy_scale, durations, pitch, energy)
+        group = join_groups(join, int(inputs_ling.shape[0]))
+        if group is not None and self.compat_padded_batch:
+            raise ValueError("join needs per-item lengths: the literal padded forward (compat_padded_batch = True) has none")
         eng = self._engine()
         invariant = not self.compat_padded_batch
         with eng.call_lock:
             return self._forward_locked(eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                                        inputs_content_embedding, prosody, given)
+                                        inputs_content_embedding, prosody, given, group)
 
     def reserve(self, batch=1, phonemes=256, frames=2048):
         """Serving set-up: pre-size the engine's workspace arena (current CUDA stream) for requests up to this shape, so that no
         forward allocates device memory afterwards.  Without it the arena simply grows when a larger request arrives (one allocation
-        stall per new maximum)."""
+        stall per new maximum).  For joined traffic (``forward(join=...)``), ``frames`` counts a joined output's frames: the
+        longest group's, not the longest segment's."""
         self._engine().reserve(batch, phonemes, frames)
 
     def _forward_locked(self, eng, invariant, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding, inputs_content_embedding,
-                        prosody=None, given=None):
+                        prosody=None, given=None, group=None):
         outputs, r = _am_forward(eng, inputs_ling, input_lengths, inputs_speaker, inputs_style_embedding,
-                                 inputs_content_embedding, invariant, prosody, given)
+                                 inputs_content_embedding, invariant, prosody, given, group)
         B = r["mel"].shape[0]
         mel_lens_ptr = (r["meta"].data_ptr() + 4 * B) if invariant else None
-        # jets.py:62-66: z = dec_outputs.transpose(1, 2); wav = generator(z).  dec_outputs is already the
-        # vocoder's time-major input layout: no transpose, no copy.
-        wav = eng.vocode(r["mel"], time_major=True, mel_lens_ptr=mel_lens_ptr, ws=r["ws2"], n=r["n2"])
+        j = r["joined"]
+        if j:
+            # long text: the items' valid rows joined per group, then one vocoder pass over the G groups
+            mel, lens = eng.join_mel(r["mel"], r["mel_lens"], j["group"], j["G"], j["Fg"])
+            wav = eng.vocode(mel, time_major=True, mel_lens_ptr=j["voc_lens"].data_ptr(), ws=r["ws2"], n=r["n2"])
+            outputs.update(joined_mel=mel, joined_lengths=lens, joined_lengths_host=j["lens_host"])
+        else:
+            # jets.py:62-66: z = dec_outputs.transpose(1, 2); wav = generator(z).  dec_outputs is already the
+            # vocoder's time-major input layout: no transpose, no copy.
+            wav = eng.vocode(r["mel"], time_major=True, mel_lens_ptr=mel_lens_ptr, ws=r["ws2"], n=r["n2"])
         outputs["wav_predictions"] = wav
         outputs["z_start_idxs"] = None
         outputs["segment_size"] = self.segment_size

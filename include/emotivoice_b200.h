@@ -207,6 +207,19 @@ EV_API int ev_am_phase2(ev_ctx* ctx, const void* phase1_workspace, const int32_t
 EV_API int ev_vocoder(ev_ctx* ctx, const float* mel, int mel_time_major, const int32_t* mel_lens, int B, int F,
                       float* wav_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Long text: the mel of several items (the segments of one text, synthesised as one batch) joined into one vocoder input, so that
+ * ev_vocoder runs over each text's seams and returns one continuous waveform per text.
+ *   mel (B,F,n_mels) f32 time-major (ev_am_phase2's mel_out); mel_lens (B) i32 (its frame counts); group (B) i32: the output each
+ *   item belongs to, 0 for the first item, each next id equal to the previous one or one more, G - 1 for the last (1 <= B <= 4096).
+ *   joined (G,Fg,n_mels) f32 time-major: group g's rows are the valid rows mel[b, :mel_lens[b]] of its items in item order, zeros past
+ *   its length; group_lens (G) i32: min(that length, Fg).  Fg is at least the longest group (the host knows every length from the
+ *   mel_lens it read back).  No allocation, no sync.
+ *   group_lens is written by a kernel, so like any kernel output it is still pending when this returns: do not pass it as the
+ *   mel_lens of an ev_vocoder enqueued behind it (see ev_vocoder); give that call lengths that were complete before, e.g. copied from
+ *   the host. */
+EV_API int ev_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* group, int B, int F, int n_mels, int G, int Fg,
+                       float* joined, int32_t* group_lens, void* stream);
+
 /* Replaces the callers' post-processing (inference_am_vocoder_joint.py:130-131):
  * pcm[i] = (int16) trunc(wav[i] * 32768), n elements. */
 EV_API int ev_wav_to_pcm16(const float* wav, int16_t* pcm, size_t n, void* stream);
