@@ -1,0 +1,68 @@
+"""Host side of the output formats (``JETSGenerator.format_audio``, ``frontdoor.fetch_audio``): which rates and encodings are
+accepted, the resampling ratio, and the polyphase filter bank ``ev_format_audio`` runs.  Pure host code, no CUDA.
+
+Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the filter is
+``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
+item of n samples gives ``ceil(n * up / down)`` samples.
+"""
+import math
+
+import numpy as np
+
+ENCODINGS = {"float32": 0, "pcm16": 1, "mulaw": 2, "alaw": 3}        # EV_AUDIO_* (include/emotivoice_b200.h)
+NUMPY_DTYPES = {"float32": np.float32, "pcm16": np.int16, "mulaw": np.uint8, "alaw": np.uint8}
+RATE_RANGE = (4000, 192000)
+MAX_FACTOR = 1024               # largest up or down ev_format_audio takes (the bank of up = 1024 is ~86 KB of shared memory)
+
+
+def plan(sample_rate, encoding, source_rate):
+    """-> (rate, up, down): the output rate (``source_rate`` for None) and the coprime resampling factors.  Accepts an integer
+    rate in [4000, 192000] Hz whose ratio to ``source_rate`` reduces to up / down with both at most 1024, and an encoding of
+    ``ENCODINGS``.  Raises ValueError otherwise."""
+    if encoding not in ENCODINGS:
+        raise ValueError("encoding must be one of %s, got %r" % (sorted(ENCODINGS), encoding))
+    if sample_rate is None:
+        rate = int(source_rate)
+    else:
+        if isinstance(sample_rate, (bool, np.bool_)) or not isinstance(sample_rate, (int, float, np.integer, np.floating)):
+            raise ValueError("sample_rate must be an integer number of Hz, got %r" % (sample_rate,))
+        if not (math.isfinite(float(sample_rate)) and float(sample_rate) == int(sample_rate)):
+            raise ValueError("sample_rate must be an integer number of Hz, got %r" % (sample_rate,))
+        rate = int(sample_rate)
+    if not RATE_RANGE[0] <= rate <= RATE_RANGE[1]:
+        raise ValueError("sample_rate must lie in [%d, %d] Hz, got %d" % (RATE_RANGE + (rate,)))
+    g = math.gcd(rate, int(source_rate))
+    up, down = rate // g, int(source_rate) // g
+    if max(up, down) > MAX_FACTOR:
+        raise ValueError("%d Hz from %d Hz is the ratio %d/%d; rates whose ratio needs a factor above %d are not supported"
+                         % (rate, source_rate, up, down, MAX_FACTOR))
+    return rate, up, down
+
+
+def resample_filter(up, down):
+    """scipy.signal.resample_poly's default filter for up / down, float64, already multiplied by ``up``."""
+    from scipy.signal import firwin
+    max_rate = max(up, down)
+    h = firwin(2 * 10 * max_rate + 1, 1.0 / max_rate, window=("kaiser", 5.0))
+    h *= up
+    return h
+
+
+def polyphase_bank(up, down):
+    """-> (up, taps_per_phase) float32 C-contiguous: row p holds the filter taps p, p + up, p + 2 up, ... (zero past its end)."""
+    h = resample_filter(up, down)
+    taps = -(-len(h) // up)
+    padded = np.zeros(up * taps, dtype=np.float64)
+    padded[:len(h)] = h
+    return np.ascontiguousarray(padded.reshape(taps, up).T.astype(np.float32))
+
+
+def resampled_length(n, up, down):
+    """Samples ``resample_poly`` returns for n input samples: ceil(n * up / down)."""
+    return (int(n) * up + down - 1) // down
+
+
+def packed_offsets(n_in, items, up, down):
+    """Where each listed item's output starts in the packed buffer: (len(items) + 1,) int64, the last entry the total."""
+    counts = [resampled_length(n_in[b], up, down) for b in items]
+    return np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)

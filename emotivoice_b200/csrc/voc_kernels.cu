@@ -1,5 +1,6 @@
 // HiFi-GAN generator kernels that are not implicit GEMMs (sm_90a, fp32): the layout change at
-// the Generator.forward boundary, the final conv_post + tanh, and the callers' PCM16 conversion.
+// the Generator.forward boundary, the final conv_post + tanh, the joined mel of long text, the callers' PCM16 conversion and
+// the output formatting (resampling + PCM16 / G.711 encoding).
 #include "ev_common.cuh"
 
 namespace ev {
@@ -152,26 +153,149 @@ int launch_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* gr
   return launch("join_mel_kernel", join_mel_kernel, (unsigned)blocks, JM_THREADS, smem, st, mel, mel_lens, group, B, F, C, G, Fg, joined,
                 group_lens);
 }
-void preload_voc_kernels() {      // see preload_conv1d_gp
-  cudaFuncAttributes fa;
-  cudaFuncGetAttributes(&fa, join_mel_kernel);
-  cudaGetLastError();
-}
-
 // pcm = (int16) trunc(wav * 32768): numpy astype('int16') of a float array is a C cast
-// (inference_am_vocoder_joint.py:130-131).  Values are inside (-1, 1) after tanh.
+// (inference_am_vocoder_joint.py:130-131).  Values are inside (-1, 1) after tanh; outside it they saturate.
+__device__ __forceinline__ int16_t pcm16_of(float v) {
+  v = truncf(v * 32768.0f);
+  v = fminf(fmaxf(v, -32768.f), 32767.f);
+  return (int16_t)(int)v;
+}
 __global__ void pcm16_kernel(const float* __restrict__ wav, int16_t* __restrict__ pcm, size_t n) {
   pdl_entry();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    float v = truncf(wav[i] * 32768.0f);
-    v = fminf(fmaxf(v, -32768.f), 32767.f);
-    pcm[i] = (int16_t)(int)v;
-  }
+  if (i < n) pcm[i] = pcm16_of(wav[i]);
 }
 int launch_pcm16(const float* wav, int16_t* pcm, size_t n, cudaStream_t st) {
   if (n == 0) return EV_OK;
   return launch("pcm16_kernel", pcm16_kernel, (unsigned)((n + 255) / 256), 256, 0, st, wav, pcm, n);
+}
+
+// G.711 of a 16-bit sample, the segment encoders of ITU-T G.711 as Python's audioop.lin2ulaw / lin2alaw apply them to 16-bit
+// input: mu-law codes the top 14 bits (bias 33, magnitude clipped at 8159, all bits inverted), A-law the top 13 bits (even bits
+// inverted).  tests/golden/g711.npz holds both functions over all 65,536 inputs.
+__device__ __forceinline__ uint8_t mulaw_of(int16_t s) {
+  int v = s >> 2;
+  int mask = 0xFF;
+  if (v < 0) {
+    v = -v;
+    mask = 0x7F;
+  }
+  v = min(v, 8159) + 33;
+  int seg = 0;
+  while (seg < 8 && v > (0x40 << seg) - 1) ++seg;
+  if (seg >= 8) return (uint8_t)(0x7F ^ mask);
+  return (uint8_t)(((seg << 4) | ((v >> (seg + 1)) & 0xF)) ^ mask);
+}
+__device__ __forceinline__ uint8_t alaw_of(int16_t s) {
+  int v = s >> 3;
+  int mask = 0xD5;
+  if (v < 0) {
+    v = -v - 1;
+    mask = 0x55;
+  }
+  int seg = 0;
+  while (seg < 8 && v > (0x20 << seg) - 1) ++seg;      // |v| <= 4095: seg <= 7
+  const int q = (seg < 2 ? v >> 1 : v >> seg) & 0xF;
+  return (uint8_t)(((seg << 4) | q) ^ mask);
+}
+__device__ __forceinline__ void store_sample(void* out, int encoding, long long i, float v) {
+  switch (encoding) {
+    case EV_AUDIO_FLOAT32: static_cast<float*>(out)[i] = v; break;
+    case EV_AUDIO_PCM16: static_cast<int16_t*>(out)[i] = pcm16_of(v); break;
+    case EV_AUDIO_MULAW: static_cast<uint8_t*>(out)[i] = mulaw_of(pcm16_of(v)); break;
+    default: static_cast<uint8_t*>(out)[i] = alaw_of(pcm16_of(v)); break;
+  }
+}
+
+// Output formatting: listed item k = items[k] (k when items is null) of the waveform batch, n = n_in[b] valid samples, resampled
+// by up/down and encoded into out[out_off[k] ...] as ceil(n * up / down) samples.  Resampling is scipy.signal.resample_poly with
+// its default filter: output o is  sum_j bank[ph][j] * x[q / up - j]  with q = o * down + half_len, ph = q % up, where bank is the
+// phase-major split bank[ph][j] = h[ph + j * up] of the (2 * half_len + 1)-tap filter h (zero past its end) and x reads as zero
+// outside [0, n).  Each output is one fp32 chain over the taps in order j = 0, 1, ..., so an item's samples do not depend on the
+// batch, the item list, the tile or the CTA that computes them.  bank == null: up == down == 1, the samples are copied.
+// A CTA takes tiles of AO_TILE consecutive outputs of one item (grid-stride over the item's tiles); it stages the bank once and,
+// per tile, the input window the tile reads, with zeros outside [0, n): no sample at or past n_in[b] is ever read.
+constexpr int AO_THREADS = 256, AO_TILE = AO_THREADS, AO_CTAS_PER_SM = 8;
+__global__ void __launch_bounds__(AO_THREADS) audio_out_kernel(const float* __restrict__ wav, long long item_stride,
+                                                               const int64_t* __restrict__ n_in, const int64_t* __restrict__ items,
+                                                               const int64_t* __restrict__ out_off, const float* __restrict__ bank,
+                                                               int up, int down, int taps, int half_len, int window, int encoding,
+                                                               void* __restrict__ out) {
+  pdl_entry();
+  extern __shared__ __align__(16) float ao_smem[];
+  const int k = blockIdx.y;
+  const long long b = items ? items[k] : k;
+  const long long n = n_in[b];
+  const long long n_out = (n * up + down - 1) / down;
+  const long long tiles = (n_out + AO_TILE - 1) / AO_TILE;
+  if ((long long)blockIdx.x >= tiles) return;
+  const float* x = wav + b * item_stride;
+  const long long o_base = out_off[k];
+  if (!bank) {
+    for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
+      const long long o = t * AO_TILE + threadIdx.x;
+      if (o < n_out) store_sample(out, encoding, o_base + o, x[o]);
+    }
+    return;
+  }
+  float* hs = ao_smem;                 // [up][taps]
+  float* xs = ao_smem + up * taps;     // [window]: inputs i0 .. i0 + window - 1 of the current tile
+  for (int i = threadIdx.x; i < up * taps; i += AO_THREADS) hs[i] = bank[i];
+  for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const long long o0 = t * AO_TILE;
+    const long long i0 = (o0 * down + half_len) / up - (taps - 1);
+    __syncthreads();                   // the previous tile's reads of xs are done
+    for (int i = threadIdx.x; i < window; i += AO_THREADS) {
+      const long long s = i0 + i;
+      xs[i] = (s >= 0 && s < n) ? x[s] : 0.f;
+    }
+    __syncthreads();
+    const long long o = o0 + threadIdx.x;
+    if (o < n_out) {
+      const long long q = o * down + half_len;
+      const float* h = hs + (int)(q % up) * taps;
+      const float* xr = xs + (int)(q / up - i0);
+      float acc = 0.f;
+      for (int j = 0; j < taps; ++j) acc = fmaf(h[j], xr[-j], acc);
+      store_sample(out, encoding, o_base + o, acc);
+    }
+  }
+}
+int launch_audio_out(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
+                     const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, void* out, cudaStream_t st) {
+  EV_CHECK_ARG(n_items >= 1 && n_items <= 65535 && item_stride >= 0, "format_audio: n_items=%d must lie in [1, 65535], item_stride=%lld",
+               n_items, item_stride);
+  EV_CHECK_ARG(encoding >= EV_AUDIO_FLOAT32 && encoding <= EV_AUDIO_ALAW, "format_audio: unknown encoding %d", encoding);
+  EV_CHECK_ARG(up >= 1 && down >= 1 && up <= AO_MAX_FACTOR && down <= AO_MAX_FACTOR, "format_audio: up=%d down=%d must lie in [1, %d]", up,
+               down, AO_MAX_FACTOR);
+  int a = up, c = down;
+  while (c) { const int r = a % c; a = c; c = r; }
+  EV_CHECK_ARG(a == 1, "format_audio: up=%d and down=%d must be coprime", up, down);
+  EV_CHECK_ARG((bank == nullptr) == (up == 1 && down == 1), "format_audio: a filter bank is needed exactly when up/down != 1");
+  const int half_len = 10 * (up > down ? up : down);
+  int window = 0;
+  size_t smem = 0;
+  if (bank) {
+    const int want = (2 * half_len + 1 + up - 1) / up;
+    EV_CHECK_ARG(taps == want, "format_audio: taps_per_phase=%d, the %d-tap filter of up=%d down=%d has %d", taps, 2 * half_len + 1, up,
+                 down, want);
+    window = ((AO_TILE - 1) * down + up - 1) / up + taps;
+    smem = (size_t)(up * taps + window) * sizeof(float);
+    static std::atomic<uint64_t> attr_devs{0};
+    if (first_use_on_device(attr_devs))
+      cudaFuncSetAttribute(audio_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+  }
+  const int per_item = (AO_CTAS_PER_SM * sm_count() + n_items - 1) / n_items;
+  dim3 grid(per_item, n_items);
+  return launch("audio_out_kernel", audio_out_kernel, grid, AO_THREADS, smem, st, wav, item_stride, n_in, items, out_off, bank, up, down,
+                taps, half_len, window, encoding, out);
+}
+
+void preload_voc_kernels() {      // see preload_conv1d_gp
+  cudaFuncAttributes fa;
+  cudaFuncGetAttributes(&fa, join_mel_kernel);
+  cudaFuncGetAttributes(&fa, audio_out_kernel);
+  cudaGetLastError();
 }
 
 }  // namespace ev

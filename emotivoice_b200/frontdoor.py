@@ -12,8 +12,9 @@ Pure host code: no CUDA, no torch ops beyond tensor construction.  The style / c
 from the caller (the simbert encoder is out of scope, SURVEY.md s2 row 17).
 
 Prompt side (s8f rank 1): ``PromptEmbeddingCache`` -- batched, cached ``get_style_embedding``.
-Output side (s8f rank 2): ``fetch_pcm16`` (GPU int16 conversion + one pinned device->host copy + per-item trim) and
-``pcm16_to_wav_bytes`` (the 16 kHz mono PCM16 RIFF image the front-ends emit).
+Output side (s8f rank 2): ``fetch_audio`` (resampling to the client's rate and PCM16 / G.711 encoding of the valid samples on
+the GPU + one pinned device->host copy), ``fetch_pcm16`` (the same at 16 kHz PCM16), ``pcm16_to_wav_bytes`` (the 16 kHz mono
+PCM16 RIFF image the front-ends emit) and ``audio_to_wav_bytes`` (the same at any rate, and G.711).
 """
 import struct
 import threading
@@ -23,6 +24,8 @@ from concurrent.futures import Future
 
 import numpy as np
 import torch
+
+from . import audio
 
 Request = namedtuple("Request", "speaker prompt phonemes content")
 
@@ -257,10 +260,15 @@ class MicroBatcher:
     ``join`` group, so the text comes back as one waveform; plain requests of that forward each get a group of their own.
     ``max_batch`` counts items.  A joined request is never split across forwards; one with more segments than ``max_batch``
     runs alone.  A forward without a joined request is called exactly as before, with no ``join`` keyword.
+
+    A request that gives ``sample_rate`` and / or ``encoding`` gets a numpy array in that format instead (``fetch_audio``; the
+    model then needs ``format_audio``).  Requests in different formats share a forward: one output launch and one copy per
+    distinct format.
     """
 
     def __init__(self, forward, device="cpu", max_batch=32, max_wait_s=0.005, hop=256):
         self._forward, self._device, self._hop = forward, device, hop
+        self._sr = int(getattr(getattr(forward, "config", None), "sr", 16000))
         self._max_batch, self._max_wait = int(max_batch), float(max_wait_s)
         self._lock = threading.Condition()
         self._queue = []
@@ -270,39 +278,54 @@ class MicroBatcher:
         self._thread.start()
 
     def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0, durations=None,
-               pitch=None, energy=None):
+               pitch=None, energy=None, sample_rate=None, encoding=None):
         """``speed`` > 1 speaks faster (duration_scale = 1 / speed); ``pitch_shift`` in semitones; ``energy_scale``
         multiplies frame energy.  Each is a float or a sequence of ``len(ids)`` values, one per phoneme (a per-phoneme speed
         must lie in [1/16, 16]).  ``durations`` (integer frames), ``pitch`` and ``energy`` (the predictors' normalised units):
-        None or ``len(ids)`` values that replace the model's predictions (see ``JETSGenerator.forward``).  Invalid values
-        raise ValueError here, so they cannot fail a batch of other requests."""
+        None or ``len(ids)`` values that replace the model's predictions (see ``JETSGenerator.forward``).  ``sample_rate`` /
+        ``encoding``: see ``_output_format``.  Invalid values raise ValueError here, so they cannot fail a batch of other
+        requests."""
         ids = np.asarray(ids, dtype=np.int64)
         controls = phoneme_controls(len(ids), speed, pitch_shift, energy_scale)
         given = given_values(len(ids), durations, pitch, energy)
+        fmt = self._output_format(sample_rate, encoding)
         item = (ids, int(speaker_id), style_vec, content_vec, controls) + ((given,) if given else ())
-        return self._enqueue([item], False)
+        return self._enqueue([item], False, fmt)
 
-    def submit_joined(self, segments, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0):
+    def submit_joined(self, segments, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0,
+                      sample_rate=None, encoding=None):
         """One long text as ``segments``: a list of phoneme id arrays, e.g. ``split_phonemes`` output put through ``encode``.
         ``style_vec`` / ``content_vec``: one vector for every segment, or a list (or a 2-D array) with one vector per segment,
         for a different prompt per sentence.  ``speed`` / ``pitch_shift`` / ``energy_scale``: one float each, checked as in
         ``submit``.  The future's result is the text's float32 waveform, the segments' mel joined and vocoded as one,
-        trimmed to ``joined_lengths[g] * hop``.  Raises ValueError here for invalid arguments."""
+        trimmed to ``joined_lengths[g] * hop``, or that waveform in the format of ``sample_rate`` / ``encoding`` (see
+        ``_output_format``).  Raises ValueError here for invalid arguments."""
         segs = [np.asarray(s, dtype=np.int64) for s in segments]
         if not segs or any(s.ndim != 1 or s.size == 0 for s in segs):
             raise ValueError("segments must be a non-empty list of non-empty 1-D phoneme id arrays")
         controls = speech_controls(speed, pitch_shift, energy_scale)
         styles = _per_segment("style_vec", style_vec, len(segs))
         contents = _per_segment("content_vec", content_vec, len(segs))
+        fmt = self._output_format(sample_rate, encoding)
         items = [(s, int(speaker_id), st, ct, controls) for s, st, ct in zip(segs, styles, contents)]
-        return self._enqueue(items, True)
+        return self._enqueue(items, True, fmt)
 
-    def _enqueue(self, items, joined):
+    def _output_format(self, sample_rate, encoding):
+        """A request's output format: None when both are None (the result is the float32 waveform tensor, as always), else
+        (rate, encoding) for ``fetch_audio``: the result is then a numpy array at ``sample_rate`` (None: the model's rate) in
+        ``encoding`` (None: "pcm16").  Raises ValueError for a rate or encoding ``format_audio`` does not take."""
+        if sample_rate is None and encoding is None:
+            return None
+        encoding = "pcm16" if encoding is None else encoding
+        rate, _, _ = audio.plan(sample_rate, encoding, self._sr)
+        return rate, encoding
+
+    def _enqueue(self, items, joined, fmt):
         fut = Future()
         with self._lock:
             if self._closed:
                 raise RuntimeError("MicroBatcher is closed")
-            self._queue.append((items, fut, joined))
+            self._queue.append((items, fut, joined, fmt))
             self._lock.notify()
         return fut
 
@@ -343,27 +366,40 @@ class MicroBatcher:
             if batch is None:
                 return
             groups = {}                      # one forward per set of caller-given tracks (the common case: one group)
-            for its, f, joined in batch:
-                it = its[0]
-                groups.setdefault(tuple(sorted(it[5])) if len(it) > 5 else (), []).append((its, f, joined))
+            for entry in batch:
+                it = entry[0][0]
+                groups.setdefault(tuple(sorted(it[5])) if len(it) > 5 else (), []).append(entry)
             for group in groups.values():
                 self._run(group)
 
     def _run(self, batch):
-        futs = [f for _, f, _ in batch]
+        futs = [e[1] for e in batch]
         try:
-            kw = collate([it for its, _, _ in batch for it in its], self._device)
-            joined = any(j for _, _, j in batch)
+            kw = collate([it for e in batch for it in e[0]], self._device)
+            joined = any(e[2] for e in batch)
             if joined:                       # one group per request: a joined request's segments share its id
-                kw["join"] = [g for g, (its, _, _) in enumerate(batch) for _ in its]
+                kw["join"] = [g for g, e in enumerate(batch) for _ in e[0]]
             out = self._forward(**kw)
-            wav = out["wav_predictions"]
-            lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
-            lens = [int(wav.shape[-1]) // self._hop] * len(batch) if lens is None else [int(v) for v in lens.tolist()]
-            wav = wav.detach().cpu()
+            # request r's output is item r of the forward (group r of a joined one); one format_audio launch and one copy
+            # per distinct (rate, encoding), over the requests that asked for it
+            formats = {}
+            for r, e in enumerate(batch):
+                if e[3] is not None:
+                    formats.setdefault(e[3], []).append(r)
+            results = {}
+            for (rate, encoding), rs in formats.items():
+                results.update(zip(rs, fetch_audio(self._forward, out, rate, encoding, items=rs, hop=self._hop)))
+            if len(results) < len(batch):
+                wav = out["wav_predictions"]
+                lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
+                lens = [int(wav.shape[-1]) // self._hop] * len(batch) if lens is None else [int(v) for v in lens.tolist()]
+                wav = wav.detach().cpu()
+                for b in range(len(batch)):
+                    if b not in results:
+                        results[b] = wav[b, 0, :lens[b] * self._hop].clone()
             self.batches_run += 1
             for b, f in enumerate(futs):
-                f.set_result(wav[b, 0, :lens[b] * self._hop].clone())
+                f.set_result(results[b])
         except BaseException as e:       # deliver, keep serving
             for f in futs:
                 if not f.done():
@@ -400,22 +436,51 @@ def pcm16_to_wav_bytes(pcm, sample_rate=16000):
     return header + data
 
 
+WAV_G711_TAGS = {"mulaw": 7, "alaw": 6}       # WAVE_FORMAT_MULAW / WAVE_FORMAT_ALAW
+
+
+def audio_to_wav_bytes(samples, sample_rate, encoding="pcm16"):
+    """Samples as ``fetch_audio`` returns them -> a complete mono RIFF/WAVE file image.  "pcm16": ``pcm16_to_wav_bytes``.
+    "mulaw" / "alaw" (uint8 G.711 codes): format tag 7 / 6, 8 bits, an 18-byte ``fmt `` chunk with cbSize = 0 and a ``fact``
+    chunk holding the sample count, as non-PCM WAVE files carry them; a pad byte follows odd-length data."""
+    if encoding == "pcm16":
+        return pcm16_to_wav_bytes(samples, sample_rate)
+    if encoding not in WAV_G711_TAGS:
+        raise ValueError("a WAV image holds pcm16, mulaw or alaw samples, got %r" % (encoding,))
+    codes = np.ascontiguousarray(np.asarray(samples))
+    if codes.dtype != np.uint8 or codes.ndim != 1:
+        raise ValueError("expected a 1-D uint8 array of G.711 codes, got %s %s" % (codes.dtype, codes.shape))
+    data = codes.tobytes()
+    pad = len(data) & 1
+    if len(data) + pad > 0xFFFFFFFF - 50:
+        raise ValueError("waveform too long for a RIFF container")
+    rate = int(sample_rate)
+    header = struct.pack("<4sI4s4sIHHIIHHH4sII4sI", b"RIFF", 50 + len(data) + pad, b"WAVE", b"fmt ", 18,
+                         WAV_G711_TAGS[encoding], 1, rate, rate, 1, 8, 0, b"fact", 4, len(data), b"data", len(data))
+    return header + data + b"\0" * pad
+
+
+def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None):
+    """Finish one forward in the format a client asked for: ``model.format_audio`` resamples to ``sample_rate`` (None: the
+    model's 16 kHz) and encodes ("float32", "pcm16", "mulaw" or "alaw") only the valid samples of each output, packed, on the
+    GPU; then ONE device->host copy of that buffer into pinned memory.  ``out`` is the dict ``model(...)`` returned; ``items``
+    selects outputs (default: all).  Returns a list of 1-D numpy arrays (float32, int16 or uint8), one per batch item, or per
+    group of a joined forward.  Invalid arguments raise ValueError before anything is enqueued."""
+    packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop)
+    host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)
+    host.copy_(packed, non_blocking=True)
+    torch.cuda.current_stream(packed.device).synchronize()
+    arr = host.numpy()
+    return [arr[offs[k]:offs[k + 1]].copy() for k in range(len(offs) - 1)]
+
+
 def fetch_pcm16(model, out, hop=256):
     """Finish one forward the way the callers do (inference_am_vocoder_joint.py:130-131), without the fp32 waveform
-    ever crossing PCIe: ``wav * 32768 -> int16`` on the GPU (``model.to_pcm16``), ONE device->host copy of the int16
-    batch into pinned memory, then per-item trimming to ``mel_lengths[b] * hop`` on the host (``joined_lengths_host[g] * hop``
-    for the output of a joined forward).  ``out`` is the dict ``model(...)`` returned.  Returns a list of 1-D int16 numpy
-    arrays (one per batch item, or per group of a joined forward)."""
-    wav = out["wav_predictions"]
-    pcm = model.to_pcm16(wav)                                              # (B, 1, 256 F) int16, device (saturating, see to_pcm16)
-    host = torch.empty(pcm.shape, dtype=torch.int16, pin_memory=True)
-    host.copy_(pcm, non_blocking=True)
-    lens = out.get("joined_lengths_host", out.get("mel_lengths"))
-    lens = None if lens is None else [int(v) for v in lens.tolist()]      # tiny D2H; also orders after the copy above
-    torch.cuda.current_stream(pcm.device).synchronize()
-    B, n = pcm.shape[0], int(pcm.shape[-1])
-    arr = host.numpy().reshape(B, n)
-    return [arr[b, :(n if lens is None else min(n, lens[b] * hop))].copy() for b in range(B)]
+    ever crossing PCIe: ``wav * 32768 -> int16`` on the GPU (saturating, see ``model.to_pcm16``) for the samples up to
+    ``mel_lengths[b] * hop`` (``joined_lengths_host[g] * hop`` for the output of a joined forward), then ONE device->host copy
+    into pinned memory: ``fetch_audio`` at the model's rate.  Returns a list of 1-D int16 numpy arrays (one per batch item, or
+    per group of a joined forward)."""
+    return fetch_audio(model, out, hop=hop)
 
 
 # ---- prompt / content embeddings (SURVEY.md s8f rank 1: "batched, prompt-embedding cache") -----------------------------

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _abi, packing, synth
+from . import _abi, audio, packing, synth
 
 
 class _Holder(nn.Module):
@@ -257,6 +257,7 @@ class _Engine:
         self.pe = None
         self._arena = {}              # (stream, kind) -> uint8 workspace, grow-only
         self.call_lock = threading.RLock()      # one forward at a time enqueues on an engine (its workspaces are reused, stream-ordered)
+        self._banks = {}              # (up, down) -> device polyphase filter bank of format_audio
         self.ensure_pe(5000)          # PositionalEncoding max_len=5000 (encoder.py:206)
         self.total_up = int(np.prod([self.cfg.up_rates[i] for i in range(self.cfg.n_ups)]))
 
@@ -432,6 +433,31 @@ class _Engine:
         _abi.check(self.lib.ev_join_mel(mel.data_ptr(), mel_lens.data_ptr(), group.data_ptr(), B, F, C, G, Fg, joined.data_ptr(),
                                         lens.data_ptr(), self._stream()))
         return joined, lens
+
+    def format_audio(self, wav, n_in, items, up, down, encoding):
+        """ev_format_audio: (B,1,L) fp32 waveform, host per-item valid samples ``n_in`` (B ints <= L) and the listed item indices
+        -> (packed device tensor, (len(items)+1,) int64 host offsets).  The filter bank of a ratio is uploaded once per engine."""
+        dev = self.device
+        bank = None
+        if (up, down) != (1, 1):
+            bank = self._banks.get((up, down))
+            if bank is None:
+                bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev)
+                self._banks[(up, down)] = bank
+        offs = audio.packed_offsets(n_in, items, up, down)
+        dtype = {"float32": torch.float32, "pcm16": torch.int16, "mulaw": torch.uint8, "alaw": torch.uint8}[encoding]
+        packed = torch.empty((int(offs[-1]),), dtype=dtype, device=dev)
+        if packed.numel() == 0:
+            return packed, offs
+        B, k = len(n_in), len(items)
+        meta = torch.from_numpy(np.concatenate([np.asarray(n_in, np.int64), np.asarray(items, np.int64), offs[:-1]]))
+        meta = meta.pin_memory().to(dev, non_blocking=True)
+        p = meta.data_ptr()
+        _abi.check(self.lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), p, p + 8 * B, k, p + 8 * (B + k),
+                                            None if bank is None else bank.data_ptr(), up, down,
+                                            0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
+                                            self._stream()))
+        return packed, offs
 
 
 class _EngineOwner(nn.Module):
@@ -750,3 +776,46 @@ class JETSGenerator(_EngineOwner):
         pcm = torch.empty(wav.shape, dtype=torch.int16, device=eng.device)
         _abi.check(eng.lib.ev_wav_to_pcm16(wav.data_ptr(), pcm.data_ptr(), wav.numel(), eng._stream()))
         return pcm
+
+    @torch.no_grad()
+    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None):
+        """The output of a forward in a client's format, on the GPU: each output's valid samples, resampled to ``sample_rate``
+        (None: the model's rate, ``config.sr``, 16000) and encoded, packed back to back.
+
+        ``out`` is the dict ``forward`` returned: output b is ``wav_predictions[b]`` trimmed to ``joined_lengths_host[b] * hop``
+        for a joined forward, else ``mel_lengths_host[b] * hop`` (hop: ``upsample_factor`` unless given), else its full width.
+        ``items``: the outputs to format, in order (default: all).  ``encoding``: "float32", "pcm16" (trunc(y * 32768),
+        saturated, as ``to_pcm16``), "mulaw" or "alaw" (one byte of G.711 of that int16 value).  Resampling is
+        ``scipy.signal.resample_poly(x, up, down)`` with its default filter, up / down the reduced ratio of the two rates, each
+        at most 1024 (see ``audio.plan``); fp32 arithmetic, one chain per sample in tap order, so an output does not depend on
+        the others.  At the model's rate "float32" is the trimmed waveform itself and "pcm16" ``to_pcm16`` of it, bit for bit.
+
+        Returns (packed 1-D device tensor: float32, int16 or uint8; (len(items) + 1,) int64 numpy offsets: output k is
+        ``packed[offs[k]:offs[k + 1]]``).  No sync: the lengths are the host copies the forward read.  Invalid arguments raise
+        ValueError before anything is enqueued."""
+        sr = int(getattr(self.config, "sr", 16000))
+        _, up, down = audio.plan(sample_rate, encoding, sr)
+        wav = out["wav_predictions"]
+        if not (isinstance(wav, torch.Tensor) and wav.dim() == 3 and wav.dtype == torch.float32 and wav.is_contiguous()):
+            raise ValueError("out['wav_predictions'] must be a contiguous (B, 1, L) float32 tensor")
+        B, width = int(wav.shape[0]), int(wav.shape[-1])
+        hop = self.upsample_factor if hop is None else int(hop)
+        lens = out.get("joined_lengths_host")
+        if lens is None:
+            lens = out.get("mel_lengths_host")
+        n_in = [width] * B if lens is None else [min(width, int(v) * hop) for v in lens.tolist()]
+        if len(n_in) != B:
+            raise ValueError("out holds %d lengths for %d waveforms" % (len(n_in), B))
+        if items is None:
+            items = list(range(B))
+        else:
+            items = [int(i) for i in items]
+            if not items or any(i < 0 or i >= B for i in items):
+                raise ValueError("items must be a non-empty list of output indices in [0, %d), got %s" % (B, items))
+        if len(items) > 65535:
+            raise ValueError("format_audio takes at most 65535 outputs per call, got %d" % len(items))
+        eng = self._engine()
+        if wav.device != eng.device:
+            raise ValueError("out['wav_predictions'] is on %s but the module is on %s" % (wav.device, eng.device))
+        with eng.call_lock:
+            return eng.format_audio(wav, n_in, items, up, down, encoding)

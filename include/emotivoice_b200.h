@@ -224,6 +224,29 @@ EV_API int ev_join_mel(const float* mel, const int32_t* mel_lens, const int32_t*
  * pcm[i] = (int16) trunc(wav[i] * 32768), n elements. */
 EV_API int ev_wav_to_pcm16(const float* wav, int16_t* pcm, size_t n, void* stream);
 
+/* Output formats of ev_format_audio: fp32 samples; int16 as ev_wav_to_pcm16 computes them (saturated); one byte of G.711
+ * mu-law or A-law of that int16 value (ITU-T G.711 as Python's audioop.lin2ulaw / lin2alaw apply it to 16-bit samples). */
+enum { EV_AUDIO_FLOAT32 = 0, EV_AUDIO_PCM16 = 1, EV_AUDIO_MULAW = 2, EV_AUDIO_ALAW = 3 };
+
+/* Replaces the server-side conversion after synthesis (resampling to the client's rate, int16 / G.711 encoding, trimming each
+ * item to its length): the valid samples of several waveform items, resampled and encoded, packed back to back in one buffer.
+ *   wav: fp32 items item_stride floats apart (wav_out of ev_vocoder: item_stride = F * prod(up_rates)); n_in (B) i64: the valid
+ *   samples of item b (mel_lens[b] * prod(up_rates)), at most item_stride; samples at or past n_in[b] are never read.
+ *   items (n_items) i64: the items to format, in output order, or NULL for items 0 .. n_items - 1; 1 <= n_items <= 65535.
+ *   out_off (n_items) i64: where listed item k starts in out, in samples; it writes ceil(n_in[b] * up / down) samples there.
+ *   up / down: coprime, each in [1, 1024]; the rate changes by up / down.  bank: NULL when up == down == 1 (the samples are
+ *   copied), else the (up, taps_per_phase) f32 phase-major split of scipy.signal.resample_poly's default filter
+ *   h = firwin(20 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up: bank[p][j] = h[p + j * up], zero past
+ *   the end of h, taps_per_phase = ceil(len(h) / up).  Output o is sum_j bank[q % up][j] * x[q / up - j], q = o * down +
+ *   10 * max(up, down), with x zero outside [0, n_in[b]): scipy.signal.resample_poly(x[:n_in[b]], up, down) to fp32 accuracy,
+ *   one fp32 chain per output in tap order, so an item's output does not depend on the other items of the call.
+ *   encoding: EV_AUDIO_*; out holds 4, 2, 1 or 1 byte(s) per sample.
+ *   All arrays are device memory read in stream order (the kernel reads them after the work before it on the stream has
+ *   completed); out_off and n_in must describe disjoint output ranges.  No allocation, no sync. */
+EV_API int ev_format_audio(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
+                           const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
+                           void* stream);
+
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
 EV_API uint64_t ev_launch_count(void);
