@@ -84,6 +84,8 @@ SIGNATURES = {
     "ev_op_to_gp": (_i, [_vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _i, _i, _i, _i, _vp]),
     "ev_op_conv_post_gp": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp]),
     "ev_debug_tc_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_int)]),
+    "ev_debug_conv1d_plan": (_i, [_i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_int)]),
+    "ev_op_conv_post": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp]),
     "ev_op_layernorm": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),
     "ev_op_attention": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ev_op_attention_tc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),

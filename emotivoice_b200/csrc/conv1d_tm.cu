@@ -212,39 +212,76 @@ __global__ void __launch_bounds__(NTHREADS) conv1d_tm_kernel(ConvParams p, int a
   }
 }
 
-template <int TXN, int NV, int TM>
-static int launch_variant(const ConvParams& p, cudaStream_t st) {
-  constexpr int BM = (NTHREADS / TXN) * TM;
-  constexpr int BN = TXN * 4 * NV;
-  const int rows_a = BM + (p.K - 1) * p.dil;
-  EV_CHECK_ARG(rows_a <= 6 * NTHREADS / 4, "conv1d: receptive field too wide for the tile (rows_a=%d)", rows_a);
-  const int a_ld = ((rows_a + 7) / 8) * 8 + 2;   // == 2 (mod 8): conflict-free transposed stores
-  const size_t smem = (size_t)(2 * KC * a_ld + 2 * KC * BN) * sizeof(float);
-  static std::atomic<uint64_t> attr_devs{0};   // per instantiation
-  if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(conv1d_tm_kernel<TXN, NV, TM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  EV_CHECK_ARG(smem <= 96 * 1024, "conv1d: smem %zu too large", smem);
-  dim3 grid((p.L + BM - 1) / BM, (p.Cout + BN - 1) / BN, p.B);
-  return launch("conv1d_tm_kernel", conv1d_tm_kernel<TXN, NV, TM>, grid, NTHREADS, smem, st, p, a_ld);
-}
+// The launch of one convolution: the template variant, its tile, the A tile's rows and leading dimension, shared memory and grid.
+struct Conv1dPlan {
+  int TXN, NV, TM, BM, BN, rows_a, a_ld;
+  size_t smem;
+  int grid_x, grid_y;
+};
+constexpr size_t kSmemAttr = 96 * 1024;   // the dynamic shared-memory attribute every variant is given
 
-int launch_conv1d(const ConvParams& p, cudaStream_t st) {
+// Argument checks and the variant choice of launch_conv1d (pure host arithmetic; also exported as ev_debug_conv1d_plan).  Every
+// variant sums each output in the same (chunk, tap, kk) order as one fmaf chain, so the choice changes no result bit.
+static int plan_conv1d(const ConvParams& p, Conv1dPlan* pl) {
   EV_CHECK_ARG(p.B > 0 && p.L > 0, "conv1d: empty problem B=%d L=%d", p.B, p.L);
-  EV_CHECK_ARG(p.Cin % KC == 0, "conv1d: Cin=%d must be a multiple of %d", p.Cin, KC);
-  EV_CHECK_ARG(p.Cout % 4 == 0, "conv1d: Cout=%d must be a multiple of 4", p.Cout);
+  EV_CHECK_ARG(p.Cin > 0 && p.Cin % KC == 0, "conv1d: Cin=%d must be a positive multiple of %d", p.Cin, KC);
+  EV_CHECK_ARG(p.Cout > 0 && p.Cout % 4 == 0, "conv1d: Cout=%d must be a positive multiple of 4", p.Cout);
   EV_CHECK_ARG(p.K >= 1 && (p.K & 1) && p.dil >= 1, "conv1d: K=%d must be odd, dil=%d >= 1", p.K, p.dil);
   EV_CHECK_ARG(p.in_act == EV_ACT_NONE || p.in_act == EV_ACT_LRELU, "conv1d: unsupported input activation");
   EV_CHECK_ARG(p.B <= 65535, "conv1d: B too large");
   // tile selection: wide N -> 128x128 (8x8 per thread); N<=64 -> 128x64; N<=32 -> 256x32;
   // small problems (few CTAs) -> 64x64 so that more SMs get work.
-  if (p.Cout <= 32) return launch_variant<8, 1, 8>(p, st);
-  const long long tiles_big = (long long)((p.L + 127) / 128) * ((p.Cout + 127) / 128) * p.B;
-  if (p.Cout <= 64) {
-    if ((long long)((p.L + 127) / 128) * p.B < sm_count()) return launch_variant<16, 1, 4>(p, st);
-    return launch_variant<16, 1, 8>(p, st);
+  int txn, nv, tm;
+  const long long m_tiles = (p.L + 127) / 128;
+  if (p.Cout <= 32) {
+    txn = 8; nv = 1; tm = 8;
+  } else if (p.Cout <= 64) {
+    if (m_tiles * p.B < sm_count()) { txn = 16; nv = 1; tm = 4; } else { txn = 16; nv = 1; tm = 8; }
+  } else if (m_tiles * ((p.Cout + 127) / 128) * p.B < sm_count()) {
+    txn = 16; nv = 1; tm = 4;
+  } else {
+    txn = 16; nv = 2; tm = 8;
   }
-  if (tiles_big < sm_count()) return launch_variant<16, 1, 4>(p, st);
-  return launch_variant<16, 2, 8>(p, st);
+  Conv1dPlan r;
+  r.TXN = txn; r.NV = nv; r.TM = tm;
+  r.BM = (NTHREADS / txn) * tm;
+  r.BN = txn * 4 * nv;
+  const long long rows_a = r.BM + (long long)(p.K - 1) * p.dil;
+  EV_CHECK_ARG(rows_a <= 6 * NTHREADS / 4, "conv1d: receptive field too wide for the tile (rows_a=%lld)", rows_a);
+  r.rows_a = (int)rows_a;
+  r.a_ld = ((r.rows_a + 7) / 8) * 8 + 2;   // == 2 (mod 8): conflict-free transposed stores
+  r.smem = (size_t)(2 * KC * r.a_ld + 2 * KC * r.BN) * sizeof(float);
+  EV_CHECK_ARG(r.smem <= kSmemAttr, "conv1d: smem %zu too large", r.smem);
+  r.grid_x = (p.L + r.BM - 1) / r.BM;
+  r.grid_y = (p.Cout + r.BN - 1) / r.BN;
+  *pl = r;
+  return EV_OK;
+}
+
+int debug_conv1d_plan(const ConvParams& p, int* v) {
+  Conv1dPlan pl;
+  EV_TRY(plan_conv1d(p, &pl));
+  v[0] = pl.TXN; v[1] = pl.NV; v[2] = pl.TM; v[3] = pl.BM; v[4] = pl.BN; v[5] = pl.rows_a; v[6] = pl.a_ld;
+  v[7] = (int)pl.smem; v[8] = pl.grid_x; v[9] = pl.grid_y;
+  return EV_OK;
+}
+
+template <int TXN, int NV, int TM>
+static int launch_variant(const ConvParams& p, const Conv1dPlan& pl, cudaStream_t st) {
+  static std::atomic<uint64_t> attr_devs{0};   // per instantiation
+  if (first_use_on_device(attr_devs))
+    cudaFuncSetAttribute(conv1d_tm_kernel<TXN, NV, TM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemAttr);
+  dim3 grid(pl.grid_x, pl.grid_y, p.B);
+  return launch("conv1d_tm_kernel", conv1d_tm_kernel<TXN, NV, TM>, grid, NTHREADS, pl.smem, st, p, pl.a_ld);
+}
+
+int launch_conv1d(const ConvParams& p, cudaStream_t st) {
+  Conv1dPlan pl;
+  EV_TRY(plan_conv1d(p, &pl));
+  if (pl.TXN == 8) return launch_variant<8, 1, 8>(p, pl, st);
+  if (pl.NV == 2) return launch_variant<16, 2, 8>(p, pl, st);
+  if (pl.TM == 4) return launch_variant<16, 1, 4>(p, pl, st);
+  return launch_variant<16, 1, 8>(p, pl, st);
 }
 
 }  // namespace ev

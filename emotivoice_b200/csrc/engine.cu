@@ -959,6 +959,20 @@ int ev_op_conv1d(const float* x, const float* w, const float* bias, size_t bias_
               out_act, acc, div, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int ev_debug_conv1d_plan(int B, int L, int Cin, int Cout, int K, int dil, int* out10) {
+  EV_CHECK_ARG(out10, "ev_debug_conv1d_plan: null output");
+  ConvParams p{};
+  p.B = B; p.L = L; p.Cin = Cin; p.Cout = Cout; p.K = K; p.dil = dil; p.in_act = EV_ACT_NONE;
+  return debug_conv1d_plan(p, out10);
+}
+
+int ev_op_conv_post(const float* x, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B, int L, int C, int K,
+                    float slope, float* wav, void* stream) {
+  EV_CHECK_ARG(x && w && bias && wav, "ev_op_conv_post: null argument");
+  EV_TRY(use_device_of(x));
+  return launch_conv_post(x, w, bias, lens, lens_mul, B, L, C, K, slope, wav, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int ev_op_conv1d_tc(const float* x, const float* w_tc, int split3, const float* bias, size_t bias_bstride, const float* res,
                     float* out, int B, int L, int Cin, int Cout, int K, int dil, const int32_t* lens, int lens_mul,
                     int in_act, float in_slope, int out_act, int acc, float div, float* splitk_ws, size_t splitk_floats,

@@ -109,6 +109,8 @@ struct ConvParams {
                        // summation order, hence every output bit, independent of how utterances are batched)
 };
 int launch_conv1d(const ConvParams& p, cudaStream_t st);
+// host-only: the plan launch_conv1d would use, {TXN, NV, TM, BM, BN, rows_a, a_ld, smem bytes, grid.x, grid.y}
+int debug_conv1d_plan(const ConvParams& p, int* v10);
 // tensor-core variant (conv1d_tc.cu); p.w in the tensor-core layout [plane hi|lo][Cout/BNp][K][Cin/4][BNp][4], BNp = min(Cout,128);
 // mode 0: one tf32 MMA per K step; 1: 3xTF32 fp32 emulation (three MMAs per K step); 2: bf16 operands
 // (p.w then in the bf16 layout [Cout/BNp][K][Cin/8][BNp][8 bf16]).

@@ -73,7 +73,7 @@ __global__ void __launch_bounds__(CP_BT) conv_post_kernel(const float* __restric
 }
 int launch_conv_post(const float* x, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B,
                      int L, int C, int K, float slope, float* wav, cudaStream_t st) {
-  EV_CHECK_ARG(C % 4 == 0 && C <= 128 && K <= 15 && (K & 1), "conv_post: C=%d K=%d", C, K);
+  EV_CHECK_ARG(C > 0 && C % 4 == 0 && C <= 128 && K >= 1 && K <= 15 && (K & 1), "conv_post: C=%d K=%d", C, K);
   EV_CHECK_ARG(B > 0 && B <= 65535 && L > 0, "conv_post: bad shape");
   const size_t smem = (size_t)((CP_BT + K - 1) * (C + 1) + K * C) * sizeof(float);
   static std::atomic<uint64_t> attr_devs{0};

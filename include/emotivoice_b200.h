@@ -265,6 +265,10 @@ EV_API int ev_op_conv1d(const float* x, const float* w, const float* bias, size_
                         const float* res, float* out, int B, int L, int Cin, int Cout, int K, int dil,
                         const int32_t* lens, int lens_mul, int in_act, float in_slope, int out_act,
                         int acc, float div, void* stream);
+/* Host-only introspection (no GPU needed; without a device it assumes 132 SMs): the plan ev_op_conv1d would use for a shape.
+ * out10 = {TXN, NV, TM, BM, BN, rows_a, a_ld, smem bytes, grid.x, grid.y}: the kernel variant <TXN, NV, TM>, its BM x BN tile, the
+ * rows (BM + (K-1)*dil) and leading dimension of its shared A tile.  EV_EINVAL for a shape ev_op_conv1d rejects. */
+EV_API int ev_debug_conv1d_plan(int B, int L, int Cin, int Cout, int K, int dil, int* out10);
 /* Same contract on the tensor cores (wgmma tf32 / bf16, fp32 accumulators in registers); w_tc is in the
  * tensor-core layout (2 planes hi|lo, Cout/BNp N tiles, K, Cin/4, BNp = min(Cout,128), 4; packing.to_tc_layout);
  * split3 = 0: 1xTF32, 1: 3xTF32 fp32 emulation, 2: bf16 operands (w_tc then in the bf16 layout of
@@ -337,6 +341,10 @@ EV_API int ev_op_to_gp(const float* in, long long stride_b, long long stride_t, 
 /* wav[b,t] = tanh(bias + conv_post(leaky_relu(x, slope))) on a granule-planar input (hifigan/models.py:127-129). */
 EV_API int ev_op_conv_post_gp(const void* x, int bf16, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B,
                               int L, int C, int K, float slope, float* wav, void* stream);
+/* The same on a time-major (B, L, C) fp32 input: what ev_vocoder runs in EV_PREC_FP32_FFMA.  C % 4 == 0, C <= 128, K odd <= 15;
+ * same channel-major summation order as ev_op_conv_post_gp.  Samples >= lens[b]*lens_mul (null: L) are written as zeros. */
+EV_API int ev_op_conv_post(const float* x, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B, int L, int C,
+                           int K, float slope, float* wav, void* stream);
 /* LayerNorm over the last dim, eps 1e-12 (encoder.py:112-127). rows x C. */
 EV_API int ev_op_layernorm(const float* x, const float* w, const float* b, float* y, int rows, int C, void* stream);
 /* Multi-head self-attention core (encoder.py:84-109) on a packed (B,L,3H) q|k|v buffer. */

@@ -12,10 +12,13 @@ the reference configuration:
     the layer's C_in blocks, with one splitk_reduce launch after the convolution whenever the clamped S is > 1;
   * attention_tc (tc_mode 1 where the layer runs fp32-accurate, 0 otherwise) for d_k = 48, the FFMA attention for other
     head sizes.
+  * in "fp32_ffma" every convolution runs the fp32 FFMA kernel (conv1d_tm, MODE FFMA here; no K split, so no reduce launch) and
+    every attention the FFMA flash kernel.
 A GPU test holds the length of this list to ev_launch_count(), so it cannot drift from engine.cu unnoticed.
 
 The plan key of a convolution is (MODE, MT, KBG, BN, a_stages, b_stages, producer groups, ksplit): the template instantiation,
-the tile width, and the ring depths and producer groups that fix the mbarrier protocol the kernel runs.
+the tile width, and the ring depths and producer groups that fix the mbarrier protocol the kernel runs.  That of an FFMA
+convolution is ("conv1d_tm", TXN, NV, TM): the template variant ev_debug_conv1d_plan reports.
 """
 import ctypes
 
@@ -24,11 +27,33 @@ ENC_SPLITS = dict(qkv=4, wo=8, ffn1=4, ffn2=16)  # engine.cu kEncSplits
 DEC_SPLITS = dict(qkv=2, wo=4, ffn1=4, ffn2=8)   # engine.cu kDecSplits
 PRED_SPLIT, COND_SPLIT, MEL_SPLIT = 8, 4, 2
 PREFIX_MODE = 1
+FFMA = -1                                        # engine.cu kFfma: the fp32 FFMA kernel (conv1d_tm.cu) on the plain weights
 
 
 def decoder_mode(prec):
     """Kernel MODE of the decoder's and to_mel's convolutions in a precision."""
-    return {"fp32": 3, "tf32": 0, "bf16": 2}[prec]
+    return {"fp32": 3, "tf32": 0, "bf16": 2, "fp32_ffma": FFMA}[prec]
+
+
+def prefix_mode(prec):
+    """Kernel MODE of the duration-critical prefix (encoder, cond.wx, predictors) in a precision."""
+    return FFMA if prec == "fp32_ffma" else PREFIX_MODE
+
+
+def conv1d_plan(lib, B, L, Cin, Cout, K, dil=1):
+    """The plan ev_op_conv1d would use (ev_debug_conv1d_plan), or None for a shape it rejects."""
+    v = (ctypes.c_int * 10)()
+    if lib.ev_debug_conv1d_plan(B, L, Cin, Cout, K, dil, v) != 0:
+        return None
+    return dict(TXN=v[0], NV=v[1], TM=v[2], BM=v[3], BN=v[4], rows_a=v[5], a_ld=v[6], smem=v[7], grid=(v[8], v[9]),
+                key=("conv1d_tm", v[0], v[1], v[2]))
+
+
+def plan_of(lib, r):
+    """Plan of one layer record of am_layers: the FFMA plan or the tensor-core one."""
+    if r["mode"] == FFMA:
+        return conv1d_plan(lib, r["B"], r["L"], r["Cin"], r["Cout"], r["K"])
+    return tc_plan(lib, r["B"], r["L"], r["Cin"], r["Cout"], r["K"], r["mode"], r["ksplit"])
 
 
 def tc_plan(lib, B, L, Cin, Cout, K, mode, ksplit):
@@ -62,7 +87,7 @@ def _stack(sh, tag, B, L, mode, splits, first_ln_done, conv_lens, attn_mode, out
         if not (i == 0 and first_ln_done):
             out.append(("layernorm",))
         out.append(layer(tag + ".qkv", B, L, H, 3 * H, 1, mode, splits["qkv"], lens=conv_lens))
-        out.append(("attention_tc", attn_mode) if H // sh["heads"] == 48 else ("attention",))
+        out.append(("attention_tc", attn_mode) if H // sh["heads"] == 48 and mode != FFMA else ("attention",))
         out.append(layer(tag + ".wo", B, L, H, H, 1, mode, splits["wo"], inplace=True, lens=conv_lens))
         out.append(("layernorm",))
         out.append(layer(tag + ".ffn1", B, L, H, 4 * H, K, mode, splits["ffn1"], out_act=ACT_GELU, lens=conv_lens))
@@ -76,15 +101,16 @@ def am_layers(B, T, F, prec, invariant, sh=None):
     sh = sh or am_shapes()
     H = sh["H"]
     inv = bool(invariant)
+    pm = prefix_mode(prec)
     out = [("validate_inputs",), ("layernorm",)]
-    _stack(sh, "enc", B, T, PREFIX_MODE, ENC_SPLITS, True, inv, 1, out)
+    _stack(sh, "enc", B, T, pm, ENC_SPLITS, True, inv, 1, out)
     out += [("cond_gather",), ("cond_gemv",),
-            layer("cond.wx", B, T, H, H, 1, PREFIX_MODE, COND_SPLIT, bias_bs=H, lens=inv)]
+            layer("cond.wx", B, T, H, H, 1, pm, COND_SPLIT, bias_bs=H, lens=inv)]
     if not inv:
         out.append(("mask_rows",))
     for name, n in sh["preds"]:
         for i in range(n):
-            out.append(layer(name + ".conv", B, T, H, H, sh["pred_k"], PREFIX_MODE, PRED_SPLIT, out_act=ACT_RELU, lens=inv))
+            out.append(layer(name + ".conv", B, T, H, H, sh["pred_k"], pm, PRED_SPLIT, out_act=ACT_RELU, lens=inv))
             out.append(("layernorm",))
         out.append(("rowdot",))
     out += [("var_embed_add",), ("duration_scan",), ("gauss_upsample",)]
@@ -100,10 +126,10 @@ def engine_launches(lib, B, T, F, prec, invariant, sh=None):
     out = []
     for r in am_layers(B, T, F, prec, invariant, sh):
         if isinstance(r, dict):
-            p = tc_plan(lib, r["B"], r["L"], r["Cin"], r["Cout"], r["K"], r["mode"], r["ksplit"])
+            p = plan_of(lib, r)
             assert p is not None, r
             out.append(p["key"])
-            if p["S"] > 1:
+            if r["mode"] != FFMA and p["S"] > 1:
                 out.append(("splitk_reduce",))
         else:
             out.append(r)
@@ -115,5 +141,5 @@ def engine_conv_keys(lib, B, T, F, prec, invariant, sh=None):
     keys = set()
     for r in am_layers(B, T, F, prec, invariant, sh):
         if isinstance(r, dict):
-            keys.add((r["kind"], tc_plan(lib, r["B"], r["L"], r["Cin"], r["Cout"], r["K"], r["mode"], r["ksplit"])["key"]))
+            keys.add((r["kind"], plan_of(lib, r)["key"]))
     return keys

@@ -6,9 +6,14 @@ restates the launch rules of ev_vocoder (csrc/engine.cu) for the reference confi
     alone has fewer than two waves of tiles, with an elementwise pass forming xs / 3 after a grouped last layer (fp32 storage);
   * otherwise one launch per ResBlock layer, fused (resblock_gp) where the fused plan keeps at least two accumulators per tile
     and not for C >= 64 with k > 7 once B * L > 280 000; two conv1d_gp launches where it is not fused.
+In "fp32_ffma" (MODE FFMA) the vocoder runs on time-major activations: a transpose for a channels-first mel only, then one
+conv1d_tm launch per convolution (conv_pre, each polyphase up, c1 and c2 of every ResBlock layer, in engine order) and
+conv_post.
 A GPU test holds this list to ev_launch_count(), so it cannot drift from engine.cu unnoticed.
 """
 import ctypes
+
+import am_plans
 
 NSM = 132
 GROUP_MAX_FRAMES = 2400           # carve_voc / voc_group_frames
@@ -109,10 +114,37 @@ def _grouped_stage(lib, B, L, C, Ks, Ds, mode):
     return out
 
 
-def engine_launches(lib, B, F, mode, shapes=None):
-    """Kernel launches of one ev_vocoder call at (B, F) in kernel mode `mode`, in order: plan keys
-    (kernel, MODE, MT, KBG, BN, rate) for the tensor-core kernels, ("to_gp",), ("gp_sum_div",), ("conv_post",)."""
+def ffma_layers(B, F, shapes=None):
+    """The convolutions ev_vocoder runs in "fp32_ffma" at (B, F), in order: dicts of the layer (kind: "pre", "ups<s>",
+    "c1_C<C>", "c2_C<C>"), its shape, and mul, the lens_mul it is launched with (L = F * mul rows).  c2's acc is the
+    ResBlock accumulation of hifigan/models.py:120-126 (1 = ADD, 2 = ADD_DIV by the number of ResBlocks on the last layer)."""
     sh = shapes or voc_shapes()
+    out = [dict(kind="pre", B=B, L=F, mul=1, Cin=sh["n_mels"], Cout=sh["c0"], K=sh["pre_k"], dil=1, rate=1, act=0, res=0, acc=0)]
+    L = F
+    for s, u in enumerate(sh["ups"]):
+        out.append(dict(kind="ups%d" % s, B=B, L=L, mul=L // F, Cin=u["cin"], Cout=u["rate"] * u["cout"], K=u["K"], dil=1, rate=u["rate"],
+                        act=1, res=0, acc=0))
+        L *= u["rate"]
+        C, J = u["cout"], len(sh["res_k"])
+        for j, K in enumerate(sh["res_k"]):
+            D = len(sh["res_d"][j])
+            for l, d in enumerate(sh["res_d"][j]):
+                acc = 0 if (l < D - 1 or j == 0) else (2 if j == J - 1 else 1)
+                out.append(dict(kind="c1_C%d" % C, B=B, L=L, mul=L // F, Cin=C, Cout=C, K=K, dil=d, rate=1, act=1, res=0, acc=0))
+                out.append(dict(kind="c2_C%d" % C, B=B, L=L, mul=L // F, Cin=C, Cout=C, K=K, dil=1, rate=1, act=1, res=1, acc=acc))
+    return out
+
+
+def engine_launches(lib, B, F, mode, shapes=None, time_major=False):
+    """Kernel launches of one ev_vocoder call at (B, F) in kernel mode `mode`, in order: plan keys
+    (kernel, MODE, MT, KBG, BN, rate) for the tensor-core kernels, ("to_gp",), ("gp_sum_div",), ("conv_post",); in MODE FFMA
+    ("transpose",) for a channels-first mel, ("conv1d_tm", TXN, NV, TM) per convolution and ("conv_post",)."""
+    sh = shapes or voc_shapes()
+    if mode == am_plans.FFMA:
+        out = [] if time_major else [("transpose",)]
+        for r in ffma_layers(B, F, sh):
+            out.append(am_plans.conv1d_plan(lib, B, r["L"], r["Cin"], r["Cout"], r["K"], r["dil"])["key"])
+        return out + [("conv_post",)]
     out = [("to_gp",), gp_plan(lib, B, F, sh["n_mels"], sh["c0"], sh["pre_k"], 1, 1, mode)["key"]]
     L = F
     for u in sh["ups"]:
