@@ -12,10 +12,11 @@
 // pads c2's input with zeros, it does not convolve c1 over the padding.
 //
 // The roles and their code are gp_pipeline.cuh's, shared with conv1d_gp.cu: the consumer warpgroups run, per tile, c1 (one wgmma
-// chain per tap, accumulators in registers), epi1 into the xt tile, a named barrier over both warpgroups, c2 over the xt tile
-// (the same chains and one-behind release, with no x stage to hand back), epi2 (+ b2 + x, accumulate modes) to HBM; the weight
-// loader streams w1 then w2 of every tile, the order the consumers read them.  The x ring and the weight ring prefetch across
-// tiles, so the loads of tile i+1 run under c2 and the epilogues of tile i.
+// chain per tap, accumulators acc1 in registers), epi1 into the xt tile, a named barrier over both warpgroups, c2 over the xt tile
+// into a second accumulator set acc2 (the same chains and one-behind release, with no x stage to hand back), then c1 of their
+// next tile with epi2 (+ b2 + x, accumulate modes) of this one to HBM in chunks under its taps; the weight loader streams w1 then
+// w2 of every tile, the order the consumers read them.  The x ring and the weight ring prefetch across tiles, so the loads of
+// tile i+1 run under c2 of tile i, and the tensor core runs c1 of tile i+1 while epi2 of tile i waits on L2.
 #include "ev_common.cuh"
 #include "gp_pipeline.cuh"
 
@@ -25,6 +26,42 @@ namespace gpp {
 using namespace gpl;
 
 constexpr int MAX_A = 6;                     // x stages
+// The fused kernel launches 512 threads: gp_pipeline.cuh's 448 and two idle warps that complete warp 12-13's warpgroup, because
+// setmaxnreg acts on whole warpgroups.  At launch every thread has 65536 / 512 = 128 registers; the two consumer warpgroups then
+// take cons_regs(MT * C) each (both accumulator sets and an epilogue chunk) from what the transform and loader warpgroups give
+// back.  With full accumulators (MT * C = 128) the consumers need 216 and the other warps fit 40; with fewer, 208 and 48 (the
+// 3xTF32 transform needs more than 40).
+constexpr int PAIR_THREADS = 512;
+__host__ __device__ constexpr int cons_regs(int acc_cols) { return acc_cols == 2 * ACC_REGS ? 216 : 208; }
+__host__ __device__ constexpr int prod_regs(int acc_cols) { return (65536 / 128 - 2 * cons_regs(acc_cols)) / 2; }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// tc_common.cuh's load_pair / store_pair as predicated instructions (no branch); a load that is off returns zeros
+template <bool BF16>
+__device__ __forceinline__ pair_t<BF16> load_pair_if(bool on, const void* t, size_t e) {
+  if constexpr (BF16) {
+    uint32_t v = 0u;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p ld.global.b32 %0, [%1];\n\t}"
+                 : "+r"(v) : "l"(reinterpret_cast<const uint16_t*>(t) + e), "r"((int)on));
+    return v;
+  } else {
+    float2 v = make_float2(0.f, 0.f);
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p ld.global.v2.f32 {%0, %1}, [%2];\n\t}"
+                 : "+f"(v.x), "+f"(v.y) : "l"(reinterpret_cast<const float*>(t) + e), "r"((int)on));
+    return v;
+  }
+}
+template <bool BF16>
+__device__ __forceinline__ void store_pair_if(bool on, void* t, size_t e, float v0, float v1) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.b32 [%0], %1;\n\t}"
+                 :: "l"(reinterpret_cast<uint16_t*>(t) + e), "r"(pack_bf16(v0, v1)), "r"((int)on) : "memory");
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p st.global.v2.f32 [%0], {%1, %2};\n\t}"
+                 :: "l"(reinterpret_cast<float*>(t) + e), "f"(v0), "f"(v1), "r"((int)on) : "memory");
+}
 
 struct PPlan {
   int mt, kbg;
@@ -71,7 +108,7 @@ __host__ __device__ inline bool make_pplan(const GpPairParams& p, int mode, int 
 
 // MODE as conv1d_gp.cu: 0 tf32, 1 3xTF32, 2 bf16 activations + operands, 3 bf16x3 on fp32 activations.  C = p.C, the channels.
 template <int MODE, int MT, int KBG, int C>
-__global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_constant__ GpPairParams p, const __grid_constant__ PPlan pl,
+__global__ void __launch_bounds__(PAIR_THREADS, 1) resblock_gp_kernel(const __grid_constant__ GpPairParams p, const __grid_constant__ PPlan pl,
                                                                      const __grid_constant__ GpPairGroups gs) {
   constexpr bool SPLIT3 = (MODE == 1), BF16 = (MODE == 2), X3B = (MODE == 3);
   constexpr bool OP16 = BF16 || X3B;
@@ -80,6 +117,7 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
   constexpr int KB = CPG * KBG;
   constexpr int KBGW = KBG * CPG / OCPG;        // operand granules (weights, xt tile) per channel block
   constexpr int NA = ACC_REGS / MT;
+  constexpr int NQ = C / 8;                     // column groups (8 columns, 4 accumulator registers per thread and MT) = epi2 chunks
   // C and KB are powers of two: every channel block is full (or the only one), so its MMA K steps are a constant
   constexpr int NK = (C < KB ? C : KB) / (2 * OCPG);
   static_assert(C % KB == 0 || C < KB, "every channel block has NK K steps");
@@ -96,6 +134,8 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
   if (tid == 0) ring.init(pl.a_stages, pl.b_stages);
   __syncthreads();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (warp < NCW) setmaxnreg_inc<cons_regs(MT * C)>();
+  else setmaxnreg_dec<prod_regs(MT * C)>();
 
   const int n_cb = (C + KB - 1) / KB;
   const int gC = C / CPG;                      // activation granule planes per item
@@ -116,7 +156,12 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
   };
 
   if (warp < NCW) {
-    // ============================ consumers: c1 -> epi1 (xt tile) -> c2 -> epi2 ================================
+    // ============================ consumers: c1 -> epi1 (xt tile) -> c2, then the next tile's c1 under epi2 ==================
+    // c1 accumulates in acc1 and c2 in acc2, so the next tile's c1 can run while this tile's epi2 waits on L2: each tap of
+    // c1(i+1) issues its chain, waits for the previous one (wgmma_wait<1>), hands its stages back, then runs one chunk of epi2(i)
+    // while the chain just issued executes.  The stages are consumed in the order of one tile at a time (x(i+1) and w1(i+1) after
+    // w2(i)), so the loaders, the transform warps and the mbarrier protocol are those of conv1d_gp.  (The chunk goes after the
+    // wait: with two chains in flight ptxas cannot tell acc2 from the accumulators they write, and waits for both.)
     asm volatile("griddepcontrol.wait;" ::: "memory");
     const int wg = warp >> 2, wl = warp & 3;
     const float slope = p.slope;
@@ -124,17 +169,72 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
     const uint64_t x_desc0 = make_desc(0u, X3B ? 2u * x_lbo : x_lbo, 128u), b_desc0 = make_desc(0u, b_lbo, 128u);
     const uint64_t a2_desc0 = make_desc(smem_u32(a2_tile) + (uint32_t)(wg * 64) * 16u, a2_lbo, 128u);
     const uint32_t x_k = (X3B ? 4u : 2u) * x_lbo, x_lo_off = X3B ? x_lbo : (uint32_t)pl.x_plane_bytes;
-    float acc[MT][NA];
+    float acc1[MT][NA], acc2[MT][NA];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-      for (int i = 0; i < NA; ++i) acc[mt][i] = 0.f;
+      for (int i = 0; i < NA; ++i) {
+        acc1[mt][i] = 0.f;
+        // a zero of its own: were acc2 a copy of acc1's zero, ptxas would see epi2's reads of acc2 as reads of the acc1 registers
+        // that c1's MMAs are writing, and wait for them
+        asm volatile("mov.b32 %0, 0;" : "=f"(acc2[mt][i]));
+      }
     int a_cnt = 0, b_cnt = 0;
-    for (int tile = next_active(blockIdx.x); tile < pl.total_tiles; tile = next_active(tile + gridDim.x)) {
-      int gi, b, t0;
-      const int len = tile_len(tile, gi, b, t0);
+    // ---- epi2 of tile e_tile (acc2 + b2 + x (+ accumulate) -> out), one chunk per call: column group q (8 columns, one b2), pairs
+    // i = 4 q + 2 h of every accumulator mt at tile row rl0 + mt * BM + 8 h.  q is a run-time index, so the pairs are picked from
+    // acc2 with selects (indexing acc2 by q would put it in local memory).  A chunk issues all its loads (b2, the residual x, `out`
+    // in the accumulate modes) before its stores.  out != x (plan_pair), and in the accumulate modes every element of out is loaded
+    // and stored by exactly one thread, load first.
+    int e_tile = -1, e_gi = 0, e_b = 0, e_t0 = 0, e_len = 0;
+    const int rl0 = wg * 64 + frag_row(0, lane, wl);
+    auto epi2_chunk = [&](int q, auto div) {      // div: std::true_type where the chunk may run ACC_ADD_DIV's division
+      const GpPairGroup& E = gs.g[e_gi];
+      const int c = frag_col(4 * q, lane);
+      const size_t ec = ((size_t)e_b * gC + c / CPG) * p.L * CPG + (c % CPG);      // element index at row 0
+      const float2 ebias = __ldg(reinterpret_cast<const float2*>(E.b2 + c));
+      const bool accm = p.acc != EV_ACC_STORE;
+      // Rows past R or len are predicated off, not branched around: a divergent branch between two tap chains makes ptxas
+      // serialise every wgmma of the kernel (C7518).
+      pair_t<BF16> eres[MT][2], eout[MT][2];
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rl = rl0 + mt * BM + 8 * h, row = e_t0 + rl;
+          const bool ok = rl < E.R && row < e_len;
+          const size_t e = ec + (size_t)row * CPG;
+          eres[mt][h] = load_pair_if<BF16>(ok, E.x, e);      // the residual: L2 hit
+          eout[mt][h] = load_pair_if<BF16>(ok && accm, E.out, e);
+        }
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rl = rl0 + mt * BM + 8 * h, row = e_t0 + rl;
+          const bool ok = rl < E.R && row < e_len;
+          float a0 = acc2[mt][2 * h], a1 = acc2[mt][2 * h + 1];
+#pragma unroll
+          for (int g = 1; g < NQ; ++g) {
+            a0 = g == q ? acc2[mt][4 * g + 2 * h] : a0;
+            a1 = g == q ? acc2[mt][4 * g + 2 * h + 1] : a1;
+          }
+          float v0 = a0 + ebias.x, v1 = a1 + ebias.y;
+          const float2 r = unpack_pair(eres[mt][h]);
+          v0 += r.x; v1 += r.y;
+          const float2 o = unpack_pair(eout[mt][h]);
+          v0 = accm ? v0 + o.x : v0;
+          v1 = accm ? v1 + o.y : v1;
+          if constexpr (decltype(div)::value)
+            if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
+          store_pair_if<BF16>(ok, E.out, ec + (size_t)row * CPG, v0, v1);
+        }
+    };
+    for (int tile = next_active(blockIdx.x);; tile = next_active(tile + gridDim.x)) {
+      const bool live = tile < pl.total_tiles;      // else only the previous tile's epi2 is left
+      int gi = 0, b = 0, t0 = 0, len = 0;
+      if (live) len = tile_len(tile, gi, b, t0);
       const GpPairGroup& G = gs.g[gi];
-      const int K = G.K, dil = G.dil, R = G.R;
+      const int K = G.K, dil = G.dil;
       const int h2 = (K - 1) / 2;
       // epi1 in parts of B1Q column groups (pair i = 4 q + 2 h of every accumulator lies in column group q: 8 columns, one b1): a
       // part's b1 loads are all issued ahead of its shared-memory stores, the first part's under c1's last MMAs
@@ -147,8 +247,17 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
           if (c < C) bias1[q] = __ldg(reinterpret_cast<const float2*>(G.b1 + c));
         }
       };
-      // ---- c1 over the staged x tile
+      // ---- c1 over the staged x tile -> acc1, one chunk of the previous tile's epi2 under each tap
       {
+        if (!live) {          // this CTA has no tile left: the last epi2 on its own
+#pragma unroll 1
+          for (int q = e_tile >= 0 ? 0 : NQ; q < NQ; ++q) epi2_chunk(q, std::true_type{});
+          break;
+        }
+        // The division's slow path is a subroutine call, and ptxas serialises every wgmma of a kernel that makes a call while MMAs
+        // are in flight: in ACC_ADD_DIV mode (a solo launch, never the grouped ones) epi2 waits for c1 to complete.
+        const bool under = e_tile >= 0 && p.acc != EV_ACC_ADD_DIV;
+        int q = under ? 0 : NQ;
         OneBehind<MAX_A> rel{ring, lane};
         // Not unrolled, not peeled: with C and the K steps constants the compiler would otherwise copy the channel-block and tap
         // loops, and every copy adds a wgmma.wait_group site (tests/test_wgmma_pipeline_sass.py counts them).
@@ -162,14 +271,20 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
             const int sb = b_cnt % pl.b_stages;
             mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            tap_chain<MODE, C, NK>(acc, desc_advance(x0, (uint32_t)(j * dil) * 16u), x_k, x_lo_off, b0, (uint32_t)pl.b_plane_bytes, cb | j);
+            tap_chain<MODE, C, NK>(acc1, desc_advance(x0, (uint32_t)(j * dil) * 16u), x_k, x_lo_off, b0, (uint32_t)pl.b_plane_bytes, cb | j);
             wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
             rel.step(sb, j == K - 1 ? sa : -1);
+            if (q < NQ) epi2_chunk(q++, std::false_type{});      // while this tap's chain runs
           }
         }
+#pragma unroll 1
+        for (; q < NQ; ++q) epi2_chunk(q, std::false_type{});      // c1 had fewer taps than epi2 has chunks: under its last one
         load_b1(0);
         wgmma_wait<0>();
         rel.drain();
+        if (e_tile >= 0 && !under)
+#pragma unroll 1
+          for (q = 0; q < NQ; ++q) epi2_chunk(q, std::true_type{});
       }
       // ---- epi1: acc1 + b1 -> lrelu -> operand format -> xt tile.  Both warpgroups' c2 of the previous tile read the whole
       // ---- xt tile (their taps overlap the other's rows), so the tile is only rewritten once both have finished it.
@@ -189,7 +304,7 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
               const int r2 = mt * BM + wg * 64 + frag_row(i, lane, wl);
               const int row = t0 - h2 + r2;
               const bool ok = row >= 0 && row < len;            // xt outside the sequence is c2's ZERO padding
-              float v0 = acc[mt][i] + bias1[q].x, v1 = acc[mt][i + 1] + bias1[q].y;
+              float v0 = acc1[mt][i] + bias1[q].x, v1 = acc1[mt][i + 1] + bias1[q].y;
               if (BF16) {      // the unfused path stores xt as bf16 before activating it
                 v0 = __uint_as_float(pack_bf16(v0, 0.f) << 16);
                 v1 = __uint_as_float(pack_bf16(v1, 0.f) << 16);
@@ -210,57 +325,7 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
       }
       fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core
       bar_sync(1, NCW * 32);        // the whole xt tile is written
-      // ---- epi2 (acc2 + b2 + x (+ accumulate) -> out): pair i = 4 q + 2 h of accumulator mt is column group q (8 columns, one b2)
-      // at tile row rl0 + mt * BM + 8 h.  One column group is one chunk of 2 MT pairs: it issues all its loads (b2, the residual x,
-      // `out` in the accumulate modes) before its stores, the first chunk's under c2's last MMAs (a larger chunk spills in the MT = 1
-      // tf32 / bf16 instantiations).  out != x (plan_pair), and in the accumulate modes every element of out is loaded and stored
-      // by exactly one thread, load first.
-      const int rl0 = wg * 64 + frag_row(0, lane, wl);
-      float2 ebias;
-      pair_t<BF16> eres[MT][2], eout[MT][2];
-      auto column = [&](int q, int& c) {
-        c = frag_col(4 * q, lane);
-        return ((size_t)b * gC + c / CPG) * p.L * CPG + (c % CPG);      // element index at row 0
-      };
-      auto epi_load = [&](int q) {
-        int c;
-        const size_t ec = column(q, c);
-        if (c >= C) return;
-        ebias = __ldg(reinterpret_cast<const float2*>(G.b2 + c));
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int rl = rl0 + mt * BM + 8 * h, row = t0 + rl;
-            if (rl >= R || row >= len) continue;
-            const size_t e = ec + (size_t)row * CPG;
-            eres[mt][h] = load_pair<BF16>(G.x, e);      // the residual: L2 hit
-            if (p.acc != EV_ACC_STORE) eout[mt][h] = load_pair<BF16>(G.out, e);
-          }
-      };
-      auto epi_store = [&](int q) {
-        int c;
-        const size_t ec = column(q, c);
-        if (c >= C) return;
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int rl = rl0 + mt * BM + 8 * h, row = t0 + rl;
-            if (rl >= R || row >= len) continue;
-            const int i = 4 * q + 2 * h;
-            float v0 = acc[mt][i] + ebias.x, v1 = acc[mt][i + 1] + ebias.y;
-            const float2 r = unpack_pair(eres[mt][h]);
-            v0 += r.x; v1 += r.y;
-            if (p.acc != EV_ACC_STORE) {
-              const float2 o = unpack_pair(eout[mt][h]);
-              v0 += o.x; v1 += o.y;
-              if (p.acc == EV_ACC_ADD_DIV) { v0 /= p.div; v1 /= p.div; }
-            }
-            store_pair<BF16>(G.out, ec + (size_t)row * CPG, v0, v1);
-          }
-      };
-      // ---- c2 over the xt tile
+      // ---- c2 over the xt tile -> acc2
       {
         OneBehind<MAX_A> rel{ring, lane};
 #pragma unroll 1                            // as in c1
@@ -271,20 +336,15 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
             const int sb = b_cnt % pl.b_stages;
             mbar_wait(ring.b_full(sb), (b_cnt / pl.b_stages) & 1);
             const uint64_t b0 = desc_advance(b_desc0, smem_u32(b_tiles + sb * pl.b_stage_bytes));
-            tap_chain<MODE, C, NK>(acc, desc_advance(a0, (uint32_t)j * 16u), 2u * a2_lbo, (uint32_t)pl.a2_plane_bytes, b0, (uint32_t)pl.b_plane_bytes, cb | j);
+            tap_chain<MODE, C, NK>(acc2, desc_advance(a0, (uint32_t)j * 16u), 2u * a2_lbo, (uint32_t)pl.a2_plane_bytes, b0, (uint32_t)pl.b_plane_bytes, cb | j);
             wgmma_wait<1>();          // the previous tap's chain has completed: its stages may be refilled
             rel.step(sb, -1);
           }
         }
-        epi_load(0);
         wgmma_wait<0>();
         rel.drain();
       }
-#pragma unroll
-      for (int q = 0; q < NA / 4; ++q) {
-        if (q > 0) epi_load(q);
-        epi_store(q);
-      }
+      e_tile = tile; e_gi = gi; e_b = b; e_t0 = t0; e_len = len;
     }
   } else if (warp < W_ALOAD) {
     // ============================ transform warps ========================================================================
@@ -311,7 +371,7 @@ __global__ void __launch_bounds__(THREADS, 1) resblock_gp_kernel(const __grid_co
       }
     }
     __syncwarp();
-  } else {
+  } else if (warp == W_BLOAD) {
     // ============================ weight loader: the consumers' order  w1(i), w2(i), w1(i+1), ... ====================
     if (lane == 0) {
       int b_cnt = 0;
@@ -396,7 +456,7 @@ static int dispatch_pair(const GpPairParams& p, const gpp::PPlan& pl, const GpPa
   EV_CHECK_ARG(k, "resblock_gp: no kernel for mode %d, KBG %d, MT %d, C %d", mode, pl.kbg, pl.mt, p.C);
   const int nsm = sm_count();
   const int grid = pl.total_tiles < nsm ? pl.total_tiles : nsm;
-  return launch("resblock_gp_kernel", k, (unsigned)grid, gpl::THREADS, pl.smem_total, st, p, pl, gs);
+  return launch("resblock_gp_kernel", k, (unsigned)grid, gpp::PAIR_THREADS, pl.smem_total, st, p, pl, gs);
 }
 
 void preload_resblock_gp() {      // see preload_conv1d_gp
