@@ -1,0 +1,296 @@
+"""Log-mel spectrograms and frame energy of recordings on the GPU, with the reference's names and signatures:
+``TacotronSTFT`` (models/prompt_tts_modified/tacotron_stft.py:46-80), ``mel_spectrogram_torch`` (mel_process.py:77-110) and
+``Energy`` (models/prompt_tts_modified/feats.py:159-213).
+
+These are the features the reference's data preparation computes per utterance on the CPU: the mel targets the acoustic model
+and the vocoder were trained on (prompt_dataset.py:29-49), the mel distance of its validation and training step
+(train_am_vocoder_joint.py:99-118) and the energy targets (prompt_dataset.py:82-86).  All three are one launch of
+``stft_feats_kernel`` (csrc/feats_kernels.cu): a fused 1024-point fp32 FFT per frame, magnitude, mel bands, log and energy.
+They differ only in the padding, the magnitude's epsilon and the rounding of the Hann window, which each passes its own.
+
+librosa, which the reference uses for the mel basis and the energy's STFT, is not a dependency: ``mel_filterbank`` restates
+``librosa.filters.mel`` (Slaney scale and norm) and is checked against torchaudio's ``melscale_fbanks``.  Inputs and outputs are
+CUDA tensors; forward only (no gradients), FFT size 1024 only.
+"""
+import numpy as np
+import torch
+import torch.nn as nn
+
+from . import _abi
+
+N_FFT = 1024
+_MAX_MELS = 128
+_STATUS_RANGE = 1               # ev_stft_features: a sample outside [-1, 1]
+
+
+def _check(t, name):
+    if not torch.is_tensor(t) or t.device.type != "cuda":
+        raise RuntimeError("%s must be a CUDA tensor: emotivoice_b200 has no CPU path" % name)
+
+
+def _hz_to_mel(frequencies):
+    """librosa.hz_to_mel(htk=False): the Slaney scale, linear below 1 kHz and logarithmic above."""
+    frequencies = np.asanyarray(frequencies)
+    f_min, f_sp = 0.0, 200.0 / 3
+    mels = (frequencies - f_min) / f_sp
+    min_log_hz = 1000.0
+    min_log_mel = (min_log_hz - f_min) / f_sp
+    logstep = np.log(6.4) / 27.0
+    if frequencies.ndim:
+        log_t = frequencies >= min_log_hz
+        mels[log_t] = min_log_mel + np.log(frequencies[log_t] / min_log_hz) / logstep
+    elif frequencies >= min_log_hz:
+        mels = min_log_mel + np.log(frequencies / min_log_hz) / logstep
+    return mels
+
+
+def _mel_to_hz(mels):
+    """librosa.mel_to_hz(htk=False)."""
+    mels = np.asanyarray(mels)
+    f_min, f_sp = 0.0, 200.0 / 3
+    freqs = f_min + f_sp * mels
+    min_log_hz = 1000.0
+    min_log_mel = (min_log_hz - f_min) / f_sp
+    logstep = np.log(6.4) / 27.0
+    if mels.ndim:
+        log_t = mels >= min_log_mel
+        freqs[log_t] = min_log_hz * np.exp(logstep * (mels[log_t] - min_log_mel))
+    elif mels >= min_log_mel:
+        freqs = min_log_hz * np.exp(logstep * (mels - min_log_mel))
+    return freqs
+
+
+def mel_filterbank(sr, n_fft, n_mels=128, fmin=0.0, fmax=None):
+    """librosa.filters.mel(sr=, n_fft=, n_mels=, fmin=, fmax=) with its defaults htk=False, norm="slaney", dtype=float32,
+    restated with the same operations in the same order: (n_mels, 1 + n_fft // 2) float32."""
+    if fmax is None:
+        fmax = float(sr) / 2
+    n_mels = int(n_mels)
+    weights = np.zeros((n_mels, int(1 + n_fft // 2)), dtype=np.float32)
+    fftfreqs = np.fft.rfftfreq(n=n_fft, d=1.0 / sr)
+    mel_f = _mel_to_hz(np.linspace(_hz_to_mel(fmin), _hz_to_mel(fmax), n_mels + 2))
+    fdiff = np.diff(mel_f)
+    ramps = np.subtract.outer(mel_f, fftfreqs)
+    for i in range(n_mels):
+        lower = -ramps[i] / fdiff[i]
+        upper = ramps[i + 2] / fdiff[i + 1]
+        weights[i] = np.maximum(0, np.minimum(lower, upper))
+    enorm = 2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels])
+    weights *= enorm[:, np.newaxis]
+    return weights
+
+
+def band_table(basis):
+    """Dense (n_mels, n_bins) float32 basis -> (bands (n_mels, 3) int32 {first bin, bin count, offset}, weights float32): each
+    band's entries from its first to its last nonzero bin.  An all-zero band has count 0."""
+    basis = np.asarray(basis, dtype=np.float32)
+    bands = np.zeros((basis.shape[0], 3), np.int32)
+    parts, off = [], 0
+    for j, row in enumerate(basis):
+        nz = np.nonzero(row)[0]
+        first, cnt = (int(nz[0]), int(nz[-1]) - int(nz[0]) + 1) if nz.size else (0, 0)
+        bands[j] = (first, cnt, off)
+        parts.append(row[first:first + cnt])
+        off += cnt
+    return bands, (np.concatenate(parts) if off else np.zeros(1, np.float32)).astype(np.float32)
+
+
+def hann_window_scipy():
+    """fp32(scipy.signal.get_window('hann', 1024, fftbins=True)): the window of stft.py:121-123 and of librosa.stft."""
+    from scipy.signal import get_window
+    return get_window("hann", N_FFT, fftbins=True).astype(np.float32)
+
+
+def twiddles():
+    """(1024, 2) float32 (cos, -sin)(2 pi k / 1024), computed in fp64 and rounded."""
+    a = 2.0 * np.pi * np.arange(N_FFT, dtype=np.float64) / N_FFT
+    return np.stack([np.cos(a), -np.sin(a)], axis=1).astype(np.float32)
+
+
+_DEV_CACHE = {}
+_BANDS = {}      # mel_spectrogram_torch's band tables per (sampling_rate, num_mels, fmin, fmax, device), like its mel_basis dict
+
+
+def _on_device(key, make, dev):
+    k = (key, str(dev))
+    t = _DEV_CACHE.get(k)
+    if t is None:
+        t = torch.from_numpy(np.ascontiguousarray(make())).to(dev)
+        _DEV_CACHE[k] = t
+    return t
+
+
+def n_frames(n, pad, hop):
+    """Frames of an n-sample item reflect-padded by pad at both ends (conv1d / stft with center=False)."""
+    return (int(n) + 2 * int(pad) - N_FFT) // int(hop) + 1
+
+
+def _check_hop(hop):
+    if not (1 <= int(hop) <= N_FFT):
+        raise ValueError("hop length %d is not supported: it must be in [1, 1024]" % int(hop))
+
+
+def _check_fft(n_fft, win_length):
+    if int(n_fft) != N_FFT or int(win_length) != N_FFT:
+        raise ValueError("n_fft %d / win_length %d are not supported: the FFT size is 1024 and the window spans all of it"
+                         % (int(n_fft), int(win_length)))
+
+
+def _lengths(y, lengths, pad):
+    """Host item lengths (a sequence or a CPU tensor; None: every row is N samples), checked like F.pad(reflect) would."""
+    B, N = y.shape
+    if lengths is None:
+        ls = [N] * B
+    else:
+        if torch.is_tensor(lengths):
+            if lengths.device.type != "cpu":
+                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
+            lengths = lengths.tolist()
+        ls = [int(v) for v in lengths]
+        if len(ls) != B:
+            raise ValueError("%d lengths for %d items" % (len(ls), B))
+        if any(v > N for v in ls):
+            raise ValueError("a length exceeds the %d samples of a row" % N)
+    for v in ls:
+        if v <= pad:
+            raise RuntimeError("an item of %d samples is not longer than the reflect padding %d" % (v, pad))
+        if v + 2 * pad < N_FFT:
+            raise RuntimeError("an item of %d samples padded by %d on each side is shorter than the 1024-point frame" % (v, pad))
+    return ls
+
+
+def device_bands(basis, dev):
+    """band_table of a dense basis as device tensors (bands, weights)."""
+    bt, bw = band_table(basis.detach().cpu().numpy() if torch.is_tensor(basis) else basis)
+    if bt.shape[0] > _MAX_MELS:
+        raise ValueError("%d mel bands are not supported: at most %d" % (bt.shape[0], _MAX_MELS))
+    return torch.from_numpy(bt).to(dev), torch.from_numpy(bw).to(dev)
+
+
+def stft_features(y, pad, hop, window, mag_eps, bands=None, energy=False, lengths=None, check_range=False):
+    """One launch of the fused kernel on y (B, N): -> (mel (B, n_mels, F) or None, energy (B, F) or None, status word or None).
+    bands: device_bands(basis) or None; F = n_frames(N, pad, hop); frames past an item's own count are 0."""
+    _check(y, "y")
+    _check_hop(hop)
+    if y.dim() != 2:
+        raise ValueError("expected a (B, N) waveform, got shape %s" % (tuple(y.shape),))
+    ls = _lengths(y, lengths, pad)
+    lib = _abi.load()
+    dev = y.device
+    x = y.detach().to(torch.float32).contiguous()
+    B, N = x.shape
+    F = n_frames(N, pad, hop)
+    mel = out_e = band_w = None
+    n_mels = 0
+    if bands is not None:
+        bands, band_w = bands
+        n_mels = bands.shape[0]
+        mel = torch.empty((B, n_mels, F), dtype=torch.float32, device=dev)
+    if energy:
+        out_e = torch.empty((B, F), dtype=torch.float32, device=dev)
+    ns = None if lengths is None else torch.tensor(ls, dtype=torch.int64).to(dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev) if check_range else None
+    win = window.detach().to(device=dev, dtype=torch.float32).contiguous()
+    tw = _on_device("twiddles", twiddles, dev)
+    _abi.check(lib.ev_stft_features(x.data_ptr(), N, None if ns is None else ns.data_ptr(), B, int(pad), int(hop), F, win.data_ptr(),
+                                    tw.data_ptr(), float(mag_eps), None if bands is None else bands.data_ptr(),
+                                    None if band_w is None else band_w.data_ptr(), n_mels, None if mel is None else mel.data_ptr(),
+                                    None if out_e is None else out_e.data_ptr(), None if status is None else status.data_ptr(),
+                                    torch.cuda.current_stream(dev).cuda_stream))
+    return mel, out_e, status
+
+
+class TacotronSTFT(nn.Module):
+    """tacotron_stft.py:46-80 with the reference's constructor.  ``mel_spectrogram(y)``: y (B, N) CUDA float in [-1, 1] ->
+    (B, n_mel_channels, N // hop_length + 1) float32.  No inverse and no phases."""
+
+    def __init__(self, filter_length=1024, hop_length=256, win_length=1024, n_mel_channels=80, sampling_rate=22050, mel_fmin=0.0,
+                 mel_fmax=8000.0):
+        super().__init__()
+        _check_fft(filter_length, win_length)
+        _check_hop(hop_length)
+        self.n_mel_channels = n_mel_channels
+        self.sampling_rate = sampling_rate
+        self.filter_length, self.hop_length, self.win_length = int(filter_length), int(hop_length), int(win_length)
+        mel_basis = mel_filterbank(sr=sampling_rate, n_fft=filter_length, n_mels=n_mel_channels, fmin=mel_fmin, fmax=mel_fmax)
+        self.register_buffer("mel_basis", torch.from_numpy(mel_basis).float())
+        self.register_buffer("window", torch.from_numpy(hann_window_scipy()))
+        self._bands = None
+
+    def mel_spectrogram(self, y, lengths=None):
+        """Raises AssertionError, like the reference's asserts (tacotron_stft.py:73-74), when a sample of an item is outside
+        [-1, 1]; reading the kernel's status word back is the call's one sync."""
+        _check(y, "y")
+        dev = y.device
+        if self._bands is None or self._bands[0] != (dev, self.mel_basis._version):
+            self._bands = ((dev, self.mel_basis._version), device_bands(self.mel_basis, dev))
+        mel, _, status = stft_features(y, self.filter_length // 2, self.hop_length, self.window.to(dev), 0.0, bands=self._bands[1],
+                                       lengths=lengths, check_range=True)
+        if int(status.item()) & _STATUS_RANGE:
+            raise AssertionError("TacotronSTFT.mel_spectrogram: a sample is outside [-1, 1]")
+        return mel
+
+
+def mel_spectrogram_torch(y, n_fft, num_mels, sampling_rate, hop_size, win_size, fmin, fmax, center=False, lengths=None):
+    """mel_process.py:77-110: y (B, N) CUDA float -> (B, num_mels, F), F = (N + 2p - n_fft) // hop_size + 1 with
+    p = (n_fft - hop_size) // 2.  Out-of-range samples are not checked (the reference only prints them)."""
+    _check(y, "y")
+    _check_fft(n_fft, win_size)
+    _check_hop(hop_size)
+    if center:
+        raise ValueError("mel_spectrogram_torch: center=True is not supported, only the reference's center=False")
+    dev = y.device
+    key = (int(sampling_rate), int(num_mels), float(fmin), None if fmax is None else float(fmax), str(dev))
+    bands = _BANDS.get(key)
+    if bands is None:
+        bands = _BANDS[key] = device_bands(mel_filterbank(sr=sampling_rate, n_fft=n_fft, n_mels=num_mels, fmin=fmin, fmax=fmax), dev)
+    window = _on_device("torch_hann", lambda: torch.hann_window(N_FFT).numpy(), dev)
+    mel, _, _ = stft_features(y, (N_FFT - int(hop_size)) // 2, hop_size, window, 1e-6, bands=bands, lengths=lengths)
+    return mel
+
+
+class Energy:
+    """feats.py:159-213 with the reference's constructor.  ``get_energy(wav)``: wav (N,) or (B, N) CUDA float -> frame energy
+    (F,) or (B, F), F = N // hop_length + 1; with ``duration`` (1-D input) the per-token means.  The caller keeps the
+    ``energy_stats`` normalisation (prompt_dataset.py:141)."""
+
+    def __init__(self, sr=24000, n_fft=2048, hop_length=300, win_length=None, window="hann", center=True, pad_mode="reflect"):
+        self.sr = sr
+        self.n_fft = n_fft
+        self.win_length = win_length
+        self.hop_length = hop_length
+        self.window = window
+        self.center = center
+        self.pad_mode = pad_mode
+        _check_fft(n_fft, n_fft if win_length is None else win_length)
+        _check_hop(hop_length)
+        if window != "hann":
+            raise ValueError("window %r is not supported: only 'hann'" % (window,))
+        if not center:
+            raise ValueError("Energy(center=False) is not supported, only center=True")
+        if pad_mode != "reflect":
+            raise ValueError("pad_mode %r is not supported: only 'reflect'" % (pad_mode,))
+
+    def _calculate_energy(self, wav, lengths=None):
+        dev = wav.device
+        window = _on_device("scipy_hann", hann_window_scipy, dev)
+        _, e, _ = stft_features(wav, N_FFT // 2, self.hop_length, window, 0.0, energy=True, lengths=lengths)
+        return e
+
+    def get_energy(self, wav, use_token_averaged_energy=True, duration=None, lengths=None):
+        _check(wav, "wav")
+        one = wav.dim() == 1
+        average = use_token_averaged_energy and duration is not None
+        if average and not one:
+            raise ValueError("duration is per item: token averaging takes a 1-D waveform, as in the reference")
+        energy = self._calculate_energy(wav[None] if one else wav, lengths)
+        if average:
+            return self._average_by_duration(energy, duration)[0]
+        return energy[0] if one else energy
+
+    def _average_by_duration(self, energy, d):
+        """feats.py:198-207 through ev_op_average_by_duration: energy (1, F), d (T,) -> (1, T)."""
+        from . import align
+        d = (d.detach() if torch.is_tensor(d) else torch.from_numpy(np.asarray(d))).to(device=energy.device, dtype=torch.float32).reshape(1, -1)
+        T, F = d.shape[1], energy.shape[1]
+        return align.average_by_duration(d, energy, torch.tensor([T]), torch.tensor([F]))

@@ -458,6 +458,28 @@ EV_API int ev_op_align_logp(const float* text_feat, const float* feats_feat, con
  * x (B,C,T) channels-first, out (B,C,segment_size). */
 EV_API int ev_op_get_segments(const float* x, const int64_t* start_idxs, int B, int C, int T, int segment_size, float* out, void* stream);
 
+/* ---- features of recordings (not used by any inference path) -------------------------------------------------------------
+ * Log-mel spectrogram and frame energy of fp32 waveforms, 1024-point STFT, one launch:
+ *   TacotronSTFT.mel_spectrogram (tacotron_stft.py:71-80, stft.py:132-160, audio_processing.py:50-51): pad 512, mag_eps 0;
+ *   mel_spectrogram_torch (mel_process.py:77-110): pad (1024 - hop) / 2, mag_eps 1e-6;
+ *   Energy.get_energy (feats.py:178-196, librosa.stft center=True): pad 512, energy only.
+ * Item b is wav[b * item_stride + t], t < n_samples[b] (n_samples (B) i64, or NULL: item_stride samples each), reflect-padded
+ * by pad samples at both of its own ends (edge sample not repeated); samples at or past n_samples[b] are never read.  Frame f
+ * of an item is padded samples [f * hop, f * hop + 1024) times window (1024 f32, the caller's rounding of the periodic Hann
+ * window); its item has F_b = (n_samples[b] + 2 pad - 1024) / hop + 1 frames (clamped to F).  X = rfft of the frame (fp32,
+ * twiddle (1024, 2) f32 = (cos, -sin)(2 pi k / 1024) rounded from fp64), |X_k| = sqrt(re^2 + im^2 + mag_eps), k = 0..512.
+ *   mel (B, n_mels, F) or NULL: log(max(sum_k M[j,k] |X_k|, 1e-5)), the sum over band j's bins in ascending order: bands
+ *   (n_mels, 3) i32 = {first bin, bin count, offset into band_w}, band_w f32 = the basis entries M[j, first .. first+count).
+ *   n_mels <= 128.
+ *   energy (B, F) or NULL: sqrt(max(sum_{k=0..512} |X_k|^2, 1e-10)) (|X_k|^2 without mag_eps).
+ *   Frames f >= F_b are stored as 0.  status (i32, may be NULL) |= 1 when a sample in [0, n_samples[b]) is outside [-1, 1] or
+ *   NaN (the reference's assert), |= 2 when an item is not longer than pad, is longer than item_stride or fills no frame (its
+ *   outputs are all 0).  hop in [1, 1024], pad in [0, 1024).  Each output depends only on its own item: a batch is bitwise its
+ *   items' single calls.  No allocation, no sync. */
+EV_API int ev_stft_features(const float* wav, long long item_stride, const int64_t* n_samples, int B, int pad, int hop, int F,
+                            const float* window, const float* twiddle, float mag_eps, const int32_t* bands, const float* band_w,
+                            int n_mels, float* mel, float* energy, int32_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
