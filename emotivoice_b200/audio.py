@@ -1,5 +1,6 @@
 """Host side of the output formats (``JETSGenerator.format_audio``, ``frontdoor.fetch_audio``): which rates and encodings are
-accepted, the resampling ratio, and the polyphase filter bank ``ev_format_audio`` runs.  Pure host code, no CUDA.
+accepted, the resampling ratio, the polyphase filter bank ``ev_format_audio`` runs, and the loudness targets and K-weighting
+filter of ``ev_loudness``.  Pure host code, no CUDA.
 
 Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the filter is
 ``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
@@ -66,3 +67,44 @@ def packed_offsets(n_in, items, up, down):
     """Where each listed item's output starts in the packed buffer: (len(items) + 1,) int64, the last entry the total."""
     counts = [resampled_length(n_in[b], up, down) for b in items]
     return np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
+
+
+LOUDNESS_RANGE = (-70.0, 0.0)   # LUFS: a target below the absolute gate could never be measured
+
+
+def check_loudness(target):
+    """A loudness target -> float LUFS.  Raises ValueError unless it is a finite real number in [-70, 0]."""
+    if isinstance(target, (bool, np.bool_)) or not isinstance(target, (int, float, np.integer, np.floating)):
+        raise ValueError("loudness must be a number of LUFS, got %r" % (target,))
+    t = float(target)
+    if not (math.isfinite(t) and LOUDNESS_RANGE[0] <= t <= LOUDNESS_RANGE[1]):
+        raise ValueError("loudness must be a finite target in [%g, %g] LUFS, got %r" % (LOUDNESS_RANGE + (target,)))
+    return t
+
+
+def k_weighting(sr):
+    """ITU-R BS.1770-4's K-weighting at ``sr`` Hz -> (10,) float64: (b0, b1, b2, a1, a2) of the high shelf, then of the high
+    pass, a0 = 1.  Both come from their analog prototypes through the bilinear transform, pre-warped at f0, with the constants
+    libebur128 and pyloudnorm use; at 48 kHz they are the standard's table."""
+    K = math.tan(math.pi * 1681.974450955533 / sr)
+    Q = 0.7071752369554196
+    Vh = 10.0 ** (3.999843853973347 / 20.0)
+    Vb = Vh ** 0.4996667741545416
+    a0 = 1.0 + K / Q + K * K
+    shelf = [(Vh + Vb * K / Q + K * K) / a0, 2.0 * (K * K - Vh) / a0, (Vh - Vb * K / Q + K * K) / a0,
+             2.0 * (K * K - 1.0) / a0, (1.0 - K / Q + K * K) / a0]
+    K = math.tan(math.pi * 38.13547087602444 / sr)
+    Q = 0.5003270373238773
+    a0 = 1.0 + K / Q + K * K
+    high_pass = [1.0, -2.0, 1.0, 2.0 * (K * K - 1.0) / a0, (1.0 - K / Q + K * K) / a0]
+    return np.array(shelf + high_pass, dtype=np.float64)
+
+
+def restart_warmup(kcoef):
+    """Samples ``ev_loudness`` filters before each 100 ms sub-block, from zero state: the smallest multiple of 32 with
+    W * r^W <= 1e-10, r the largest pole radius of the cascade (2048 at 16 kHz)."""
+    r = max(float(np.max(np.abs(np.roots([1.0, kcoef[i + 3], kcoef[i + 4]])))) for i in (0, 5))
+    W = 32
+    while math.log(W) + W * math.log(r) > math.log(1e-10):
+        W += 32
+    return W

@@ -251,11 +251,12 @@ int launch_transpose_cf_to_tm(const float* in, float* out, int B, int C, int L, 
 int launch_conv_post(const float* x, const float* w, const float* bias, const int32_t* lens, int lens_mul, int B,
                      int L, int C, int K, float slope, float* wav, cudaStream_t st);
 int launch_pcm16(const float* wav, int16_t* pcm, size_t n, cudaStream_t st);
-// resample by up/down (scipy.signal.resample_poly, default filter) + encode the valid samples of listed waveform items, packed
-// (ev_format_audio)
+// resample by up/down (scipy.signal.resample_poly, default filter) + scale by an optional per-item gain + encode the valid samples
+// of listed waveform items, packed (ev_format_audio, ev_format_audio_gain)
 constexpr int AO_MAX_FACTOR = 1024;
 int launch_audio_out(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
-                     const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, void* out, cudaStream_t st);
+                     const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, const float* gain, void* out,
+                     cudaStream_t st);
 // valid rows of mel (B,F,C) of consecutive items with one group id, concatenated -> joined (G,Fg,C), zero past each group's
 // length; group_lens[g] = min(group frames, Fg).  B <= 4096.
 int launch_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* group, int B, int F, int C, int G, int Fg, float* joined,

@@ -215,12 +215,14 @@ __device__ __forceinline__ void store_sample(void* out, int encoding, long long 
 // batch, the item list, the tile or the CTA that computes them.  bank == null: up == down == 1, the samples are copied.
 // A CTA takes tiles of AO_TILE consecutive outputs of one item (grid-stride over the item's tiles); it stages the bank once and,
 // per tile, the input window the tile reads, with zeros outside [0, n): no sample at or past n_in[b] is ever read.
+// gain (one per listed item, or null): each output is encoded as fp32(acc * gain[k]); it is read after pdl_entry() because the
+// launch just before this one (ev_loudness's gate kernel) writes it.
 constexpr int AO_THREADS = 256, AO_TILE = AO_THREADS, AO_CTAS_PER_SM = 8;
 __global__ void __launch_bounds__(AO_THREADS) audio_out_kernel(const float* __restrict__ wav, long long item_stride,
                                                                const int64_t* __restrict__ n_in, const int64_t* __restrict__ items,
                                                                const int64_t* __restrict__ out_off, const float* __restrict__ bank,
                                                                int up, int down, int taps, int half_len, int window, int encoding,
-                                                               void* __restrict__ out) {
+                                                               const float* __restrict__ gain, void* __restrict__ out) {
   pdl_entry();
   extern __shared__ __align__(16) float ao_smem[];
   const int k = blockIdx.y;
@@ -234,7 +236,7 @@ __global__ void __launch_bounds__(AO_THREADS) audio_out_kernel(const float* __re
   if (!bank) {
     for (long long t = blockIdx.x; t < tiles; t += gridDim.x) {
       const long long o = t * AO_TILE + threadIdx.x;
-      if (o < n_out) store_sample(out, encoding, o_base + o, x[o]);
+      if (o < n_out) store_sample(out, encoding, o_base + o, gain ? x[o] * gain[k] : x[o]);
     }
     return;
   }
@@ -257,12 +259,14 @@ __global__ void __launch_bounds__(AO_THREADS) audio_out_kernel(const float* __re
       const float* xr = xs + (int)(q / up - i0);
       float acc = 0.f;
       for (int j = 0; j < taps; ++j) acc = fmaf(h[j], xr[-j], acc);
+      if (gain) acc *= gain[k];
       store_sample(out, encoding, o_base + o, acc);
     }
   }
 }
 int launch_audio_out(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
-                     const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, void* out, cudaStream_t st) {
+                     const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, const float* gain, void* out,
+                     cudaStream_t st) {
   EV_CHECK_ARG(n_items >= 1 && n_items <= 65535 && item_stride >= 0, "format_audio: n_items=%d must lie in [1, 65535], item_stride=%lld",
                n_items, item_stride);
   EV_CHECK_ARG(encoding >= EV_AUDIO_FLOAT32 && encoding <= EV_AUDIO_ALAW, "format_audio: unknown encoding %d", encoding);
@@ -288,7 +292,7 @@ int launch_audio_out(const float* wav, long long item_stride, const int64_t* n_i
   const int per_item = (AO_CTAS_PER_SM * sm_count() + n_items - 1) / n_items;
   dim3 grid(per_item, n_items);
   return launch("audio_out_kernel", audio_out_kernel, grid, AO_THREADS, smem, st, wav, item_stride, n_in, items, out_off, bank, up, down,
-                taps, half_len, window, encoding, out);
+                taps, half_len, window, encoding, gain, out);
 }
 
 void preload_voc_kernels() {      // see preload_conv1d_gp

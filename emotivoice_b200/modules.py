@@ -258,6 +258,7 @@ class _Engine:
         self._arena = {}              # (stream, kind) -> uint8 workspace, grow-only
         self.call_lock = threading.RLock()      # one forward at a time enqueues on an engine (its workspaces are reused, stream-ordered)
         self._banks = {}              # (up, down) -> device polyphase filter bank of format_audio
+        self._kcoef = {}              # sample rate -> K-weighting coefficients of ev_loudness (host float64)
         self.ensure_pe(5000)          # PositionalEncoding max_len=5000 (encoder.py:206)
         self.total_up = int(np.prod([self.cfg.up_rates[i] for i in range(self.cfg.n_ups)]))
 
@@ -434,9 +435,40 @@ class _Engine:
                                         lens.data_ptr(), self._stream()))
         return joined, lens
 
-    def format_audio(self, wav, n_in, items, up, down, encoding):
+    def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
+        """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
+        kc = self._kcoef.get(sr)
+        if kc is None:
+            kc = self._kcoef[sr] = np.ascontiguousarray(audio.k_weighting(sr))
+        res = torch.empty((3, k), dtype=torch.float32, device=self.device)
+        nbytes = self.lib.ev_loudness_workspace_bytes(k, int(wav.stride(0)), sr)
+        ws = self._ws("loudness", nbytes)
+        _abi.check(self.lib.ev_loudness(wav.data_ptr(), int(wav.stride(0)), n_in_ptr, items_ptr, k, sr, kc.ctypes.data, float(target),
+                                        res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(), ws.numel(),
+                                        self._stream()))
+        return res[0], res[1], res[2]
+
+    def _meta(self, arrays):
+        """Host int64 arrays -> one device int64 tensor (one pinned copy) and the device address of each array in it."""
+        meta = torch.from_numpy(np.concatenate([np.asarray(a, np.int64) for a in arrays]))
+        meta = meta.pin_memory().to(self.device, non_blocking=True)
+        ptrs, p = [], meta.data_ptr()
+        for a in arrays:
+            ptrs.append(p)
+            p += 8 * len(a)
+        return meta, ptrs
+
+    def measure_loudness(self, wav, n_in, items, sr):
+        """ev_loudness: (B,1,L) fp32 waveform at ``sr`` Hz, host per-item valid samples and the listed items -> device
+        (lufs, peak) float32 (len(items),)."""
+        meta, (p_n, p_items) = self._meta([n_in, items])
+        lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
+        return lufs, pk
+
+    def format_audio(self, wav, n_in, items, up, down, encoding, loudness=None, sr=None):
         """ev_format_audio: (B,1,L) fp32 waveform, host per-item valid samples ``n_in`` (B ints <= L) and the listed item indices
-        -> (packed device tensor, (len(items)+1,) int64 host offsets).  The filter bank of a ratio is uploaded once per engine."""
+        -> (packed device tensor, (len(items)+1,) int64 host offsets).  The filter bank of a ratio is uploaded once per engine.
+        ``loudness`` (LUFS, or None): ev_loudness at ``sr`` Hz first, and its gains go to ev_format_audio_gain."""
         dev = self.device
         bank = None
         if (up, down) != (1, 1):
@@ -449,14 +481,19 @@ class _Engine:
         packed = torch.empty((int(offs[-1]),), dtype=dtype, device=dev)
         if packed.numel() == 0:
             return packed, offs
-        B, k = len(n_in), len(items)
-        meta = torch.from_numpy(np.concatenate([np.asarray(n_in, np.int64), np.asarray(items, np.int64), offs[:-1]]))
-        meta = meta.pin_memory().to(dev, non_blocking=True)
-        p = meta.data_ptr()
-        _abi.check(self.lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), p, p + 8 * B, k, p + 8 * (B + k),
-                                            None if bank is None else bank.data_ptr(), up, down,
-                                            0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
-                                            self._stream()))
+        k = len(items)
+        meta, (p_n, p_items, p_off) = self._meta([n_in, items, offs[:-1]])
+        if loudness is None:
+            _abi.check(self.lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), p_n, p_items, k, p_off,
+                                                None if bank is None else bank.data_ptr(), up, down,
+                                                0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
+                                                self._stream()))
+            return packed, offs
+        _, _, gain = self._loudness(wav, p_n, p_items, k, sr, loudness)
+        _abi.check(self.lib.ev_format_audio_gain(wav.data_ptr(), int(wav.stride(0)), p_n, p_items, k, p_off,
+                                                 None if bank is None else bank.data_ptr(), up, down,
+                                                 0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
+                                                 gain.data_ptr(), self._stream()))
         return packed, offs
 
 
@@ -777,24 +814,8 @@ class JETSGenerator(_EngineOwner):
         _abi.check(eng.lib.ev_wav_to_pcm16(wav.data_ptr(), pcm.data_ptr(), wav.numel(), eng._stream()))
         return pcm
 
-    @torch.no_grad()
-    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None):
-        """The output of a forward in a client's format, on the GPU: each output's valid samples, resampled to ``sample_rate``
-        (None: the model's rate, ``config.sr``, 16000) and encoded, packed back to back.
-
-        ``out`` is the dict ``forward`` returned: output b is ``wav_predictions[b]`` trimmed to ``joined_lengths_host[b] * hop``
-        for a joined forward, else ``mel_lengths_host[b] * hop`` (hop: ``upsample_factor`` unless given), else its full width.
-        ``items``: the outputs to format, in order (default: all).  ``encoding``: "float32", "pcm16" (trunc(y * 32768),
-        saturated, as ``to_pcm16``), "mulaw" or "alaw" (one byte of G.711 of that int16 value).  Resampling is
-        ``scipy.signal.resample_poly(x, up, down)`` with its default filter, up / down the reduced ratio of the two rates, each
-        at most 1024 (see ``audio.plan``); fp32 arithmetic, one chain per sample in tap order, so an output does not depend on
-        the others.  At the model's rate "float32" is the trimmed waveform itself and "pcm16" ``to_pcm16`` of it, bit for bit.
-
-        Returns (packed 1-D device tensor: float32, int16 or uint8; (len(items) + 1,) int64 numpy offsets: output k is
-        ``packed[offs[k]:offs[k + 1]]``).  No sync: the lengths are the host copies the forward read.  Invalid arguments raise
-        ValueError before anything is enqueued."""
-        sr = int(getattr(self.config, "sr", 16000))
-        _, up, down = audio.plan(sample_rate, encoding, sr)
+    def _outputs(self, out, items, hop):
+        """The outputs of a forward as ``format_audio`` takes them -> (wav, n_in, items, engine), or ValueError."""
         wav = out["wav_predictions"]
         if not (isinstance(wav, torch.Tensor) and wav.dim() == 3 and wav.dtype == torch.float32 and wav.is_contiguous()):
             raise ValueError("out['wav_predictions'] must be a contiguous (B, 1, L) float32 tensor")
@@ -817,5 +838,44 @@ class JETSGenerator(_EngineOwner):
         eng = self._engine()
         if wav.device != eng.device:
             raise ValueError("out['wav_predictions'] is on %s but the module is on %s" % (wav.device, eng.device))
+        return wav, n_in, items, eng
+
+    @torch.no_grad()
+    def measure_loudness(self, out, items=None, hop=None):
+        """Integrated loudness (ITU-R BS.1770-4, LUFS) and sample peak of each output of a forward, on the GPU, at the model's
+        rate.  ``out`` / ``items`` / ``hop``: the outputs ``format_audio`` would encode (a joined forward's groups are measured
+        as one waveform each).  Returns (lufs, peak): device float32 tensors of len(items); lufs is -inf for an output shorter
+        than 400 ms or with no 400 ms block above the gates (silence).  No sync."""
+        wav, n_in, items, eng = self._outputs(out, items, hop)
         with eng.call_lock:
-            return eng.format_audio(wav, n_in, items, up, down, encoding)
+            return eng.measure_loudness(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
+
+    @torch.no_grad()
+    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None):
+        """The output of a forward in a client's format, on the GPU: each output's valid samples, resampled to ``sample_rate``
+        (None: the model's rate, ``config.sr``, 16000) and encoded, packed back to back.
+
+        ``out`` is the dict ``forward`` returned: output b is ``wav_predictions[b]`` trimmed to ``joined_lengths_host[b] * hop``
+        for a joined forward, else ``mel_lengths_host[b] * hop`` (hop: ``upsample_factor`` unless given), else its full width.
+        ``items``: the outputs to format, in order (default: all).  ``encoding``: "float32", "pcm16" (trunc(y * 32768),
+        saturated, as ``to_pcm16``), "mulaw" or "alaw" (one byte of G.711 of that int16 value).  Resampling is
+        ``scipy.signal.resample_poly(x, up, down)`` with its default filter, up / down the reduced ratio of the two rates, each
+        at most 1024 (see ``audio.plan``); fp32 arithmetic, one chain per sample in tap order, so an output does not depend on
+        the others.  At the model's rate "float32" is the trimmed waveform itself and "pcm16" ``to_pcm16`` of it, bit for bit.
+
+        ``loudness`` (a target in LUFS, in [-70, 0], or None): each output is first measured as ``measure_loudness`` does and
+        scaled by g = min(10^((loudness - L) / 20), 10^(-1/20) / peak) before it is resampled and encoded (a -1 dBFS sample-peak
+        ceiling; g = 1 where L = -inf).  g is computed in fp64 and applied in fp32 as fp32(y * g), y the resampled sample; the
+        gain is the same at every output rate, since resampling is linear.  None: no measurement, and the output is exactly
+        as without the argument.
+
+        Returns (packed 1-D device tensor: float32, int16 or uint8; (len(items) + 1,) int64 numpy offsets: output k is
+        ``packed[offs[k]:offs[k + 1]]``).  No sync: the lengths are the host copies the forward read.  Invalid arguments raise
+        ValueError before anything is enqueued."""
+        sr = int(getattr(self.config, "sr", 16000))
+        _, up, down = audio.plan(sample_rate, encoding, sr)
+        if loudness is not None:
+            loudness = audio.check_loudness(loudness)
+        wav, n_in, items, eng = self._outputs(out, items, hop)
+        with eng.call_lock:
+            return eng.format_audio(wav, n_in, items, up, down, encoding, loudness, sr)

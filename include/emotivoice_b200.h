@@ -246,6 +246,36 @@ enum { EV_AUDIO_FLOAT32 = 0, EV_AUDIO_PCM16 = 1, EV_AUDIO_MULAW = 2, EV_AUDIO_AL
 EV_API int ev_format_audio(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
                            const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
                            void* stream);
+/* ev_format_audio with a per-item gain: gain (n_items) f32 device array, or NULL.  Listed item k's outputs are encoded from
+ * fp32(y * gain[k]), y the resampled sample ev_format_audio computes (at up == down == 1 the sample itself).  With gain == NULL
+ * this is ev_format_audio, bit for bit.  gain is read in stream order, so it may be written by the launch just before
+ * (ev_loudness). */
+EV_API int ev_format_audio_gain(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
+                                const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
+                                const float* gain, void* stream);
+
+/* Integrated loudness (ITU-R BS.1770-4, one channel) of listed waveform items and the gain that brings each to a target: the
+ * server-side loudness normalisation of responses (EBU R128 at -23 LUFS, podcasts at -16), before ev_format_audio_gain encodes
+ * them.  Arguments as ev_format_audio: wav items item_stride floats apart, n_in (B) i64 valid samples (at most item_stride;
+ * samples at or past n_in[b] are never read), items (n_items) i64 or NULL for 0 .. n_items - 1, 1 <= n_items <= 65535.
+ *   sample_rate: the items' rate, a multiple of 10 in [4000, 192000] (100 ms sub-blocks of sample_rate / 10 samples).
+ *   kcoef: HOST array of 10 doubles, the K-weighting cascade (b0, b1, b2, a1, a2) of the high shelf, then of the high pass, with
+ *   a0 = 1 (emotivoice_b200.audio.k_weighting(sample_rate)).  The cascade runs in fp32 (direct form I) on each 100 ms
+ *   sub-block, restarted from zero state W samples before it (W the smallest multiple of 32 with W * r^W <= 1e-10, r the
+ *   cascade's largest pole radius; 2048 at 16 kHz), so every sub-block is computed on its own.
+ *   Gating blocks are 400 ms with 75 % overlap, only those entirely inside the item; block loudness l = -0.691 +
+ *   10 log10(mean square); the absolute gate keeps l > -70, the relative gate l > (loudness of the blocks kept) - 10; fp64 sums
+ *   in a fixed order, so an item's results do not depend on the other items of the call.
+ *   lufs (n_items) f32: integrated loudness L, -inf for an item shorter than 400 ms or with no block passing the gates.
+ *   peak (n_items) f32: max |x| over the item's valid samples.
+ *   gain (n_items) f32: fp32 of min(10^((target_lufs - L) / 20), 10^(-1/20) / peak) computed in fp64 (a -1 dBFS sample-peak
+ *   ceiling); 1 where L = -inf.  target_lufs in [-70, 0].
+ *   ws / ws_bytes: device workspace of at least ev_loudness_workspace_bytes(n_items, item_stride, sample_rate) bytes.
+ * Two launches; device arrays are read in stream order.  No allocation, no sync. */
+EV_API size_t ev_loudness_workspace_bytes(int n_items, long long max_n, int sample_rate);  /* 0 for arguments out of range */
+EV_API int ev_loudness(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items, int sample_rate,
+                       const double* kcoef, float target_lufs, float* lufs, float* peak, float* gain, void* ws, size_t ws_bytes,
+                       void* stream);
 
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
