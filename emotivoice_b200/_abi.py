@@ -70,6 +70,9 @@ SIGNATURES = {
     "ev_format_audio_gain": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "ev_loudness_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),
     "ev_loudness": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ev_flac_bound_bytes": (_sz, [ctypes.c_longlong]),
+    "ev_flac_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
+    "ev_flac_encode": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _vp, _sz, _vp]),
     "ev_launch_count": (_u64, []),
     "ev_op_conv1d": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp]),
     "ev_op_conv1d_tc": (_i, [_vp, _vp, _i, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp, _sz, _vp]),

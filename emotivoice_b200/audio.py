@@ -1,6 +1,6 @@
 """Host side of the output formats (``JETSGenerator.format_audio``, ``frontdoor.fetch_audio``): which rates and encodings are
-accepted, the resampling ratio, the polyphase filter bank ``ev_format_audio`` runs, and the loudness targets and K-weighting
-filter of ``ev_loudness``.  Pure host code, no CUDA.
+accepted, the resampling ratio, the polyphase filter bank ``ev_format_audio`` runs, the loudness targets and K-weighting
+filter of ``ev_loudness``, and the frame-header rate code of ``ev_flac_encode``.  Pure host code, no CUDA.
 
 Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the filter is
 ``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
@@ -11,7 +11,8 @@ import math
 import numpy as np
 
 ENCODINGS = {"float32": 0, "pcm16": 1, "mulaw": 2, "alaw": 3}        # EV_AUDIO_* (include/emotivoice_b200.h)
-NUMPY_DTYPES = {"float32": np.float32, "pcm16": np.int16, "mulaw": np.uint8, "alaw": np.uint8}
+FLAC = "flac"                   # a complete .flac file image per output (ev_flac_encode); not an EV_AUDIO_* sample encoding
+NUMPY_DTYPES = {"float32": np.float32, "pcm16": np.int16, "mulaw": np.uint8, "alaw": np.uint8, FLAC: np.uint8}
 RATE_RANGE = (4000, 192000)
 MAX_FACTOR = 1024               # largest up or down ev_format_audio takes (the bank of up = 1024 is ~86 KB of shared memory)
 
@@ -19,9 +20,9 @@ MAX_FACTOR = 1024               # largest up or down ev_format_audio takes (the 
 def plan(sample_rate, encoding, source_rate):
     """-> (rate, up, down): the output rate (``source_rate`` for None) and the coprime resampling factors.  Accepts an integer
     rate in [4000, 192000] Hz whose ratio to ``source_rate`` reduces to up / down with both at most 1024, and an encoding of
-    ``ENCODINGS``.  Raises ValueError otherwise."""
-    if encoding not in ENCODINGS:
-        raise ValueError("encoding must be one of %s, got %r" % (sorted(ENCODINGS), encoding))
+    ``ENCODINGS`` or "flac".  Raises ValueError otherwise."""
+    if encoding not in ENCODINGS and encoding != FLAC:
+        raise ValueError("encoding must be one of %s, got %r" % (sorted(ENCODINGS) + [FLAC], encoding))
     if sample_rate is None:
         rate = int(source_rate)
     else:
@@ -108,3 +109,23 @@ def restart_warmup(kcoef):
     while math.log(W) + W * math.log(r) > math.log(1e-10):
         W += 32
     return W
+
+
+FLAC_STANDARD_RATES = {88200: 1, 176400: 2, 192000: 3, 8000: 4, 16000: 5, 22050: 6, 24000: 7, 32000: 8, 44100: 9, 48000: 10, 96000: 11}
+
+
+def flac_rate_code(rate):
+    """The sample rate field of a FLAC frame header (RFC 9639 section 9.1.2) -> (code, value of the field that follows the
+    header's fixed part, its bits).  The standard code where one exists; else 12 (8-bit kHz) for a whole number of kHz up to
+    255, 13 (16-bit Hz) up to 65535 Hz, 14 (16-bit tens of Hz) for a multiple of 10; else 0: the rate is only in STREAMINFO,
+    and such a stream is outside FLAC's streamable subset."""
+    rate = int(rate)
+    if rate in FLAC_STANDARD_RATES:
+        return FLAC_STANDARD_RATES[rate], 0, 0
+    if rate % 1000 == 0 and rate // 1000 <= 255:
+        return 12, rate // 1000, 8
+    if rate <= 65535:
+        return 13, rate, 16
+    if rate % 10 == 0:
+        return 14, rate // 10, 16
+    return 0, 0, 0

@@ -467,8 +467,8 @@ def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=
     GPU, after normalising each output to ``loudness`` LUFS when that is given (BS.1770-4 integrated loudness, -1 dBFS
     sample-peak ceiling; see ``format_audio``); then ONE device->host copy of that buffer into pinned memory.  ``out`` is the
     dict ``model(...)`` returned; ``items`` selects outputs (default: all).  Returns a list of 1-D numpy arrays (float32, int16
-    or uint8), one per batch item, or per group of a joined forward.  Invalid arguments raise ValueError before anything is
-    enqueued."""
+    or uint8), one per batch item, or per group of a joined forward.  "flac": each array is the bytes of a complete .flac file
+    whose samples are the "pcm16" result.  Invalid arguments raise ValueError before anything is enqueued."""
     extra = {} if loudness is None else {"loudness": loudness}
     packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, **extra)
     host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)

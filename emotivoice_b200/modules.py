@@ -496,6 +496,28 @@ class _Engine:
                                                  gain.data_ptr(), self._stream()))
         return packed, offs
 
+    def format_flac(self, wav, n_in, items, up, down, rate, loudness=None, sr=None):
+        """``format_audio`` to PCM16 at ``rate`` Hz, then ev_flac_encode -> (uint8 device tensor of the len(items) .flac images
+        back to back, (len(items)+1,) int64 host offsets).  The image sizes are known only after encoding: one device->host
+        read of the offsets, the call's only sync."""
+        lib = self.lib
+        pcm, offs = self.format_audio(wav, n_in, items, up, down, "pcm16", loudness, sr)
+        counts = np.ascontiguousarray(np.diff(offs), dtype=np.int64)
+        k = len(items)
+        bound = sum(int(lib.ev_flac_bound_bytes(int(n))) for n in counts)
+        out = torch.empty((bound,), dtype=torch.uint8, device=self.device)
+        out_off = torch.empty((k + 1,), dtype=torch.int64, device=self.device)
+        pcm_off = torch.from_numpy(offs).pin_memory().to(self.device, non_blocking=True)
+        nbytes = lib.ev_flac_workspace_bytes(k, int(counts.max()))
+        ws = self._ws("flac", nbytes)
+        _abi.check(lib.ev_flac_encode(pcm.data_ptr(), pcm_off.data_ptr(), k, counts.ctypes.data, int(rate), out.data_ptr(), bound,
+                                      out_off.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
+        host = torch.empty((k + 1,), dtype=torch.int64, pin_memory=True)
+        host.copy_(out_off, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        flac_offs = host.numpy().copy()
+        return out[:int(flac_offs[-1])], flac_offs
+
 
 class _EngineOwner(nn.Module):
     """Lazy (re)packing of the parameter tree into an engine on the parameters' device."""
@@ -869,13 +891,23 @@ class JETSGenerator(_EngineOwner):
         gain is the same at every output rate, since resampling is linear.  None: no measurement, and the output is exactly
         as without the argument.
 
+        ``encoding="flac"``: each output becomes a complete .flac file image (RFC 9639: mono, 16 bits, 4096-sample blocks) of
+        exactly the samples "pcm16" gives, encoded on the GPU by ev_flac_encode; decoding it returns that PCM16 bit for bit.
+        The images' sizes exist only after encoding, so this encoding makes ONE device->host read of the len(items) + 1
+        offsets (a sync); every other encoding is sync-free.
+
         Returns (packed 1-D device tensor: float32, int16 or uint8; (len(items) + 1,) int64 numpy offsets: output k is
-        ``packed[offs[k]:offs[k + 1]]``).  No sync: the lengths are the host copies the forward read.  Invalid arguments raise
-        ValueError before anything is enqueued."""
+        ``packed[offs[k]:offs[k + 1]]``).  No sync except for "flac": the lengths are the host copies the forward read.
+        Invalid arguments raise ValueError before anything is enqueued."""
         sr = int(getattr(self.config, "sr", 16000))
-        _, up, down = audio.plan(sample_rate, encoding, sr)
+        rate, up, down = audio.plan(sample_rate, encoding, sr)
         if loudness is not None:
             loudness = audio.check_loudness(loudness)
         wav, n_in, items, eng = self._outputs(out, items, hop)
+        if encoding == audio.FLAC:
+            if any(n_in[b] < 1 for b in items):
+                raise ValueError("an output with no samples cannot be a FLAC stream (valid samples %s)" % [n_in[b] for b in items])
+            with eng.call_lock:
+                return eng.format_flac(wav, n_in, items, up, down, rate, loudness, sr)
         with eng.call_lock:
             return eng.format_audio(wav, n_in, items, up, down, encoding, loudness, sr)

@@ -277,6 +277,25 @@ EV_API int ev_loudness(const float* wav, long long item_stride, const int64_t* n
                        const double* kcoef, float target_lufs, float* lufs, float* peak, float* gain, void* ws, size_t ws_bytes,
                        void* stream);
 
+/* FLAC (RFC 9639) file images of int16 items, the lossless compressed response of a TTS server: item k is pcm[pcm_off[k] ..
+ * pcm_off[k + 1]) (pcm_off (n_items + 1) i64 DEVICE array, items packed back to back as ev_format_audio writes EV_AUDIO_PCM16),
+ * n_samples (n_items) i64 HOST array of the same counts (each in [1, 2^36]; it sizes the grid and the checks below).
+ *   Each image: fLaC, STREAMINFO (last-metadata flag; block sizes 4096 / 4096, the real min / max frame size, sample_rate, one
+ *   channel, 16 bits, the sample count, MD5 all zero = unknown), then frames of 4096 samples (the last one shorter): sync
+ *   0xFFF8, the standard sample rate code where one exists, else 8-bit kHz, 16-bit Hz or 16-bit tens of Hz, else 0000 (from
+ *   STREAMINFO), CRC-8 and CRC-16.  Each subframe is the smallest exact bit count of CONSTANT, FIXED 0-4, LPC 1-12 (integer
+ *   Welch window, fp64 Levinson-Durbin without contraction) and VERBATIM, with Rice partitions of 4-bit parameters; the stream
+ *   is byte for byte the one oracle/flac_oracle.py defines.  It is in FLAC's streamable subset except at rates above 65535 Hz
+ *   that are not a multiple of 10, whose frame headers need code 0000.
+ *   out (out_bytes >= sum of ev_flac_bound_bytes(n_samples[k])): the images back to back; out_off (n_items + 1) i64 device:
+ *   image k is out[out_off[k] .. out_off[k + 1]).  sample_rate in [4000, 192000].  ws: ev_flac_workspace_bytes(n_items,
+ *   max n_samples) bytes of device workspace.  Four launches; each image depends only on its own item.  If pcm_off disagrees
+ *   with n_samples the images are wrong, but nothing outside the items or out is touched.  No allocation, no sync. */
+EV_API size_t ev_flac_bound_bytes(long long n_samples);                        /* worst-case image (VERBATIM frames); 0 out of range */
+EV_API size_t ev_flac_workspace_bytes(int n_items, long long max_n);          /* 0 for arguments out of range */
+EV_API int ev_flac_encode(const int16_t* pcm, const int64_t* pcm_off, int n_items, const int64_t* n_samples, int sample_rate,
+                          uint8_t* out, size_t out_bytes, int64_t* out_off, void* ws, size_t ws_bytes, void* stream);
+
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
 EV_API uint64_t ev_launch_count(void);
