@@ -111,6 +111,8 @@ SIGNATURES = {
     "ev_op_align_logp": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "ev_op_get_segments": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "ev_stft_features": (_i, [_vp, ctypes.c_longlong, _vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "ev_pitch_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i, ctypes.c_double, _i]),
+    "ev_pitch": (_i, [_vp, ctypes.c_longlong, _vp, _i, _i, ctypes.c_double, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_style_create": (_i, [ctypes.POINTER(_vp), _i, ctypes.POINTER(EvStyleConfig)]),
     "ev_style_destroy": (None, [_vp]),
     "ev_style_bind_weights": (_i, [_vp, _vp, _sz, _vp, _i]),

@@ -1,6 +1,7 @@
 """Log-mel spectrograms and frame energy of recordings on the GPU, with the reference's names and signatures:
-``TacotronSTFT`` (models/prompt_tts_modified/tacotron_stft.py:46-80), ``mel_spectrogram_torch`` (mel_process.py:77-110) and
-``Energy`` (models/prompt_tts_modified/feats.py:159-213).
+``TacotronSTFT`` (models/prompt_tts_modified/tacotron_stft.py:46-80), ``mel_spectrogram_torch`` (mel_process.py:77-110),
+``Energy`` (models/prompt_tts_modified/feats.py:159-213) and ``Pitch`` (feats.py:83-156), pyworld.dio + pyworld.stonemask
+restated on the GPU in fp64 (``ev_pitch``, csrc/pitch_kernels.cu).
 
 These are the features the reference's data preparation computes per utterance on the CPU: the mel targets the acoustic model
 and the vocoder were trained on (prompt_dataset.py:29-49), the mel distance of its validation and training step
@@ -294,3 +295,110 @@ class Energy:
         d = (d.detach() if torch.is_tensor(d) else torch.from_numpy(np.asarray(d))).to(device=energy.device, dtype=torch.float32).reshape(1, -1)
         T, F = d.shape[1], energy.shape[1]
         return align.average_by_duration(d, energy, torch.tensor([T]), torch.tensor([F]))
+
+
+# ---- pitch ---------------------------------------------------------------------------------------------------------------
+PITCH_SR_RANGE = (8000, 48000)    # Hz, integers: covers 16, 22.05, 24 and 48 kHz
+PITCH_HOP_RANGE = (16, 4096)      # samples
+_PITCH_CONTINUOUS, _PITCH_LOG = 1, 2
+
+
+def pitch_frame_period(sr, hop):
+    """feats.py:119: the frame period in ms handed to pyworld.dio."""
+    return 1000 * hop / sr
+
+
+def pitch_frames(n, sr, hop):
+    """pyworld's frame count of an n-sample item, int(1000 n / fs / frame_period) + 1 in double (N // hop + 1 at the configs)."""
+    return int(1000.0 * int(n) / int(sr) / pitch_frame_period(sr, hop)) + 1
+
+
+def pitch_min_samples(sr):
+    """The shortest item get_pitch takes: the length of DIO's 50 Hz low-cut filter, 2 round(sr / 50) + 1 samples."""
+    return 2 * int(sr / 50.0 + 0.5) + 1
+
+
+def _check_pitch_config(sr, hop):
+    if int(sr) != sr or not PITCH_SR_RANGE[0] <= int(sr) <= PITCH_SR_RANGE[1]:
+        raise ValueError("sample rate %r is not supported: it must be an integer in [%d, %d] Hz" % ((sr,) + PITCH_SR_RANGE))
+    if int(hop) != hop or not PITCH_HOP_RANGE[0] <= int(hop) <= PITCH_HOP_RANGE[1]:
+        raise ValueError("hop length %r is not supported: it must be an integer in [%d, %d]" % ((hop,) + PITCH_HOP_RANGE))
+
+
+def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=False):
+    """One ev_pitch call on wav (B, N) CUDA float32/float64 -> pitch (B, F) float64 [, DIO's raw contour (B, F)],
+    F = pitch_frames(N, sr, hop); frames past an item's own count are 0."""
+    _check(wav, "wav")
+    _check_pitch_config(sr, hop)
+    if wav.dim() != 2:
+        raise ValueError("expected a (B, N) waveform, got shape %s" % (tuple(wav.shape),))
+    if wav.dtype not in (torch.float32, torch.float64):
+        raise ValueError("wav must be float32 or float64, got %s" % wav.dtype)
+    B, N = wav.shape
+    if lengths is None:
+        ls = [N] * B
+    else:
+        if torch.is_tensor(lengths):
+            if lengths.device.type != "cpu":
+                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
+            lengths = lengths.tolist()
+        ls = [int(v) for v in lengths]
+        if len(ls) != B:
+            raise ValueError("%d lengths for %d items" % (len(ls), B))
+        if any(v > N for v in ls):
+            raise ValueError("a length exceeds the %d samples of a row" % N)
+    m = pitch_min_samples(sr)
+    if any(v < m for v in ls):
+        raise ValueError("an item of %d samples is too short to filter: at least %d at %d Hz" % (min(ls), m, int(sr)))
+    lib = _abi.load()
+    dev = wav.device
+    x = wav.detach().to(torch.float64).contiguous()
+    fp = pitch_frame_period(int(sr), int(hop))
+    F = pitch_frames(N, sr, hop)
+    nbytes = lib.ev_pitch_workspace_bytes(B, N, int(sr), fp, F)
+    if nbytes == 0:
+        raise ValueError("ev_pitch rejects B=%d N=%d sr=%d hop=%d" % (B, N, int(sr), int(hop)))
+    ws = torch.empty((nbytes + 15) // 16 * 2, dtype=torch.float64, device=dev)
+    ns = None if lengths is None else torch.tensor(ls, dtype=torch.int64).to(dev)
+    out = torch.empty((B, F), dtype=torch.float64, device=dev)
+    f0 = torch.empty((B, F), dtype=torch.float64, device=dev) if raw else None
+    flags = (_PITCH_CONTINUOUS if continuous else 0) | (_PITCH_LOG if log else 0)
+    _abi.check(lib.ev_pitch(x.data_ptr(), N, None if ns is None else ns.data_ptr(), B, int(sr), fp, F, flags,
+                            None if f0 is None else f0.data_ptr(), out.data_ptr(), None, ws.data_ptr(), ws.numel() * 8,
+                            torch.cuda.current_stream(dev).cuda_stream))
+    return (out, f0) if raw else out
+
+
+class Pitch:
+    """feats.py:83-156 with the reference's constructor.  ``get_pitch(wav)``: wav (N,) or (B, N) CUDA float32/float64 -> F0 in Hz
+    (F,) or (B, F) float64, F = pyworld's frame count (N // hop_length + 1 at 16 kHz / 256 and 24 kHz / 300): pyworld.dio and
+    pyworld.stonemask at their defaults (restated; not checked against pyworld), then optionally the continuous interpolation
+    and the log.  With ``use_token_averaged_pitch`` and ``duration`` (1-D input) the per-token means, through
+    ``align.average_by_duration`` (fp32).  ``pitch_min`` / ``pitch_max`` are kept and unused, as in the reference, which never
+    passes them to dio.  The caller keeps the ``pitch_stats`` normalisation (prompt_dataset.py:140)."""
+
+    def __init__(self, sr=24000, hop_length=300, pitch_min=80, pitch_max=7600):
+        self.sr = sr
+        self.hop_length = hop_length
+        self.pitch_min = pitch_min
+        self.pitch_max = pitch_max
+        _check_pitch_config(sr, hop_length)
+
+    def get_pitch(self, wav, use_continuous_pitch=True, use_log_pitch=False, use_token_averaged_pitch=False, duration=None,
+                  lengths=None):
+        _check(wav, "wav")
+        one = wav.dim() == 1
+        average = use_token_averaged_pitch and duration is not None
+        if average and not one:
+            raise ValueError("duration is per item: token averaging takes a 1-D waveform, as in the reference")
+        p = pitch_track(wav[None] if one else wav, self.sr, self.hop_length, use_continuous_pitch, use_log_pitch, lengths)
+        if average:
+            return self._average_by_duration(p, duration)[0].to(torch.float64)
+        return p[0] if one else p
+
+    def _average_by_duration(self, pitch, d):
+        """feats.py:133-147 (its zero mask is a no-op) through ev_op_average_by_duration: pitch (1, F), d (T,) -> (1, T) float32."""
+        from . import align
+        d = (d.detach() if torch.is_tensor(d) else torch.from_numpy(np.asarray(d))).to(device=pitch.device, dtype=torch.float32).reshape(1, -1)
+        T, F = d.shape[1], pitch.shape[1]
+        return align.average_by_duration(d, pitch, torch.tensor([T]), torch.tensor([F]))

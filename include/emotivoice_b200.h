@@ -529,6 +529,25 @@ EV_API int ev_stft_features(const float* wav, long long item_stride, const int64
                             const float* window, const float* twiddle, float mag_eps, const int32_t* bands, const float* band_w,
                             int n_mels, float* mel, float* energy, int32_t* status, void* stream);
 
+/* Pitch of fp64 recordings: pyworld.dio then pyworld.stonemask at pyworld's defaults (f0_floor 71, f0_ceil 800, 2 channels per
+ * octave, speed 1, allowed_range 0.1), as feats.Pitch._calculate_pitch (feats.py:114-131) calls them, restated from the published
+ * algorithms (oracle/pitch_oracle.py lists every assumed detail; not checked against pyworld).  Item b is x[b * item_stride + t],
+ * t < n_samples[b] (n_samples (B) i64, or NULL: item_stride samples each); nothing at or past n_samples[b] is read.  fs in
+ * [8000, 48000] Hz, frame_period in [0.25, 1000] ms, F = int(1000 item_stride / fs / frame_period) + 1 (the row's frame
+ * count); item b has F_b = int(1000 n_samples[b] / fs / frame_period) + 1 frames at times f * frame_period / 1000 s.
+ *   raw_f0 (B, F) f64 or NULL: DIO's contour.
+ *   pitch (B, F) f64: StoneMask's refined contour; with flags & 1 the reference's continuous interpolation (ends held, linear
+ *   between voiced frames, as feats.py:92-112), then with flags & 2 the log of every nonzero frame.
+ * Frames f >= F_b are stored as 0; an item of at most int(0.5 + 1000 / frame_period / 71) * 2 + 1 frames is all 0 (WORLD's
+ * FixF0Contour).  status (i32, may be NULL) |= 1 when a sample is not finite, |= 2 when an item is shorter than the low-cut
+ * filter (2 round(fs / 50) + 1 samples) or longer than item_stride (its outputs are all 0).  workspace: at least
+ * ev_pitch_workspace_bytes(B, item_stride, fs, frame_period, F) bytes, 16-byte aligned (0 for arguments ev_pitch rejects).
+ * fp64 throughout.  Each output depends only on its own item: a batch is bitwise its items' single calls.  No allocation, no
+ * sync. */
+EV_API size_t ev_pitch_workspace_bytes(int B, long long item_stride, int fs, double frame_period, int F);
+EV_API int ev_pitch(const double* x, long long item_stride, const int64_t* n_samples, int B, int fs, double frame_period, int F,
+                    int flags, double* raw_f0, double* pitch, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
