@@ -3,8 +3,10 @@
 
 The reference copies ``log_p_attn`` to the host and runs a numba loop per sample in the middle of every training step
 (model_open_source.py:114-118); here one kernel launch handles the batch and nothing leaves the device.  Paths and durations are
-bit-exact with the reference (the kernel restates its float64 dynamic programme); ``bin_loss`` and the averages are float32
-means (1e-6).
+bit-exact with the reference (the kernel restates its float64 dynamic programme).  ``bin_loss`` and the averages are float32
+roundings of float64 means: within 1 ulp of the exact mean.  The reference's averages are float32 running sums (numba), which
+drift from the exact mean by a few ulp at the magnitudes of energy and pitch tracks; durations that sum past the track clip to
+it, and negative durations slice the track the way numpy does, as in the reference.
 
 Also here (the rest of SURVEY.md s8f rank 4): ``AlignmentModule`` (alignment.py:13-87: five convolutions on the tensor cores in
 the fp32-accurate 3xTF32 mode, the L2-distance / masked log-softmax kernel, the beta-binomial prior built on the host exactly
@@ -61,7 +63,9 @@ def average_by_duration(ds, xs, text_lengths, feats_lengths):
 
 class AlignmentModule(nn.Module):
     """alignment.py:13-56 with the reference's constructor, parameter names (``t_conv1.weight`` ...) and forward signature.
-    ``text`` (B, T_text, adim), ``feats`` (B, T_feats, odim) -> ``log_p_attn`` (B, T_feats, T_text).  Forward only."""
+    ``text`` (B, T_text, adim), ``feats`` (B, T_feats, odim) -> ``log_p_attn`` (B, T_feats, T_text).  Forward only.
+    ``x_masks`` must be a suffix mask (True from each item's text length on, as model_open_source.py builds it): only its count
+    of unmasked tokens per item is used."""
 
     CONVS = (("t_conv1", 3), ("t_conv2", 1), ("f_conv1", 3), ("f_conv2", 3), ("f_conv3", 1))
 

@@ -85,8 +85,12 @@ int launch_mas(const float* log_p, const int64_t* text_lens, const int64_t* feat
   return launch("mas_kernel", mas_kernel, B, 256, smem, st, log_p, text_lens, feats_lens, T_mel, T_inp, path, durations, bin_loss, dec_ws);
 }
 
-// out[b, n] = mean(xs[b, start_n : start_n + d_n]) (0 when d_n == 0), start = exclusive cumsum of the durations; tokens past
-// text_lens[b] stay 0 (alignment.py:145-165).  One CTA per item; thread 0 builds the prefix, then threads over tokens.
+// out[b, n] = mean(xs[b, start_n : start_n + d_n]) (0 when the slice is empty), start = exclusive cumsum of the durations; tokens
+// past text_lens[b] stay 0 (alignment.py:145-165).  One CTA per item; thread 0 builds the prefix, then threads over tokens.
+// Each slice bound is normalised like a numpy slice of the length-F row: a negative bound counts from the end (+ F), then both
+// are clipped to [0, F].  So negative durations give the reference's answer, and no index outside the item's [0, F) is formed.
+__device__ __forceinline__ int abd_slice_bound(int v, int F) { return min(max(v < 0 ? v + F : v, 0), F); }
+
 __global__ void __launch_bounds__(256) avg_by_duration_kernel(const float* __restrict__ durations, const float* __restrict__ xs,
                                                               const int64_t* __restrict__ text_lens, const int64_t* __restrict__ feats_lens,
                                                               int T_mel, int T_inp, float* __restrict__ out) {
@@ -107,7 +111,7 @@ __global__ void __launch_bounds__(256) avg_by_duration_kernel(const float* __res
   for (int n = tid; n < T_inp; n += blockDim.x) {
     float v = 0.f;
     if (n < T) {
-      const int s = min(abd_start[n], F), e = min(abd_start[n + 1], F);     // x[start:end] of the length-F slice clamps like numpy
+      const int s = abd_slice_bound(abd_start[n], F), e = abd_slice_bound(abd_start[n + 1], F);     // x[start:end] of the length-F row
       if (e > s) {
         double acc = 0.0;
         for (int j = s; j < e; ++j) acc += (double)x[j];
