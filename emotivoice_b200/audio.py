@@ -1,6 +1,7 @@
 """Host side of the output formats (``JETSGenerator.format_audio``, ``frontdoor.fetch_audio``): which rates and encodings are
 accepted, the resampling ratio, the polyphase filter bank ``ev_format_audio`` runs, the loudness targets and K-weighting
-filter of ``ev_loudness``, and the frame-header rate code of ``ev_flac_encode``.  Pure host code, no CUDA.
+filter of ``ev_loudness``, the ceiling checks, detector bank and fixed constants of ``ev_limit``, and the frame-header rate code
+of ``ev_flac_encode``.  Pure host code, no CUDA.
 
 Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the filter is
 ``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
@@ -81,6 +82,71 @@ def check_loudness(target):
     if not (math.isfinite(t) and LOUDNESS_RANGE[0] <= t <= LOUDNESS_RANGE[1]):
         raise ValueError("loudness must be a finite target in [%g, %g] LUFS, got %r" % (LOUDNESS_RANGE + (target,)))
     return t
+
+
+TRUE_PEAK_RANGE = (-20.0, 0.0)  # dBTP
+
+
+def check_true_peak(ceiling):
+    """A true-peak ceiling -> float dBTP.  Raises ValueError unless it is a finite real number in [-20, 0]."""
+    if isinstance(ceiling, (bool, np.bool_)) or not isinstance(ceiling, (int, float, np.integer, np.floating)):
+        raise ValueError("true_peak must be a ceiling in dBTP, got %r" % (ceiling,))
+    c = float(ceiling)
+    if not (math.isfinite(c) and TRUE_PEAK_RANGE[0] <= c <= TRUE_PEAK_RANGE[1]):
+        raise ValueError("true_peak must be a finite ceiling in [%g, %g] dBTP, got %r" % (TRUE_PEAK_RANGE + (ceiling,)))
+    return c
+
+
+# The true-peak limiter of ev_limit: fixed constants, not options.
+LIMIT_DETECT_RATE = 192000      # the detector oversamples by R = ceil(192000 / sr): 12 at 16 kHz
+LIMIT_LOOKAHEAD_S = 0.005       # look-ahead L: 5 ms, 80 samples at 16 kHz
+LIMIT_RELEASE_DB_PER_S = 60.0   # linear release in dB per second
+LIMIT_GRID = 2.0 ** -32         # ev_limit's envelope grid (dB): the release step is a multiple of it
+
+
+def limit_lookahead(sr):
+    return int(round(LIMIT_LOOKAHEAD_S * sr))
+
+
+def limit_release(sr):
+    """The release per sample (dB), rounded to ev_limit's 2^-32 dB grid so the release scan is exact in fp64."""
+    return round(LIMIT_RELEASE_DB_PER_S / sr / LIMIT_GRID) * LIMIT_GRID
+
+
+def _kaiser_lowpass(half, cutoff):
+    from scipy.signal import firwin
+    return firwin(2 * half + 1, cutoff, window=("kaiser", 5.0))
+
+
+def limit_bank(sr, rate):
+    """The detector of ev_limit for output at ``rate`` Hz from ``sr`` -> (bank (phases, taps) float32, hold M in samples).
+
+    The interpolator oversamples by R = ceil(192000 / sr) and is designed like resample_poly's filter,
+    ``firwin(2 * 10 * R + 1, 1 / R, kaiser 5) * R``.  For a rate below sr it is convolved (at the oversampled rate) with the
+    same-design low-pass at rate / 2, ``firwin(2 * ceil(10 sr / rate) + 1, rate / sr, kaiser 5)``: the down-sampler removes that
+    content, and doing so can raise peaks.  Row p of the bank is phase p's taps h[p + j R], applied as sum_j bank[p][j] x[n + c - j],
+    c = (taps - 1) / 2; the plain interpolator keeps phases 1 .. R - 1 (phase 0 is x[n] itself), the low-passed one all R.
+    M is the larger half-span, in samples at sr, of the detector and of format_audio's resampling filter for that rate."""
+    R = -(-LIMIT_DETECT_RATE // int(sr))
+    h = _kaiser_lowpass(10 * R, 1.0 / R) * R
+    half = 10
+    if rate < sr:
+        lp_half = -(-10 * int(sr) // int(rate))
+        lp = _kaiser_lowpass(lp_half, float(rate) / sr)
+        up = np.zeros((len(lp) - 1) * R + 1)
+        up[::R] = lp
+        h = np.convolve(h, up)
+        half += lp_half
+    taps = 2 * half + 1
+    padded = np.zeros(taps * R)
+    padded[:len(h)] = h
+    bank = padded.reshape(taps, R).T
+    if rate >= sr:
+        bank = bank[1:]
+    g = math.gcd(int(rate), int(sr))
+    up_, down_ = int(rate) // g, int(sr) // g
+    resample_half = -(-10 * max(up_, down_) // up_) if (up_, down_) != (1, 1) else 0
+    return np.ascontiguousarray(bank.astype(np.float32)), max(half, resample_half)
 
 
 def k_weighting(sr):

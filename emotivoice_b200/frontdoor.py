@@ -12,7 +12,7 @@ Pure host code: no CUDA, no torch ops beyond tensor construction.  The style / c
 from the caller (the simbert encoder is out of scope, SURVEY.md s2 row 17).
 
 Prompt side (s8f rank 1): ``PromptEmbeddingCache`` -- batched, cached ``get_style_embedding``.
-Output side (s8f rank 2): ``fetch_audio`` (loudness normalisation, resampling to the client's rate and PCM16 / G.711 encoding of
+Output side (s8f rank 2): ``fetch_audio`` (loudness normalisation, true-peak limiting, resampling to the client's rate and PCM16 / G.711 encoding of
 the valid samples on the GPU + one pinned device->host copy), ``fetch_pcm16`` (the same at 16 kHz PCM16), ``pcm16_to_wav_bytes`` (the 16 kHz mono
 PCM16 RIFF image the front-ends emit) and ``audio_to_wav_bytes`` (the same at any rate, and G.711).
 """
@@ -261,9 +261,10 @@ class MicroBatcher:
     ``max_batch`` counts items.  A joined request is never split across forwards; one with more segments than ``max_batch``
     runs alone.  A forward without a joined request is called exactly as before, with no ``join`` keyword.
 
-    A request that gives ``sample_rate``, ``encoding`` and / or ``loudness`` gets a numpy array in that format instead
-    (``fetch_audio``; the model then needs ``format_audio``).  Requests in different formats share a forward: one output launch
-    (after one loudness measurement, for a format with a ``loudness`` target) and one copy per distinct format.
+    A request that gives ``sample_rate``, ``encoding``, ``loudness`` and / or ``true_peak`` gets a numpy array in that format
+    instead (``fetch_audio``; the model then needs ``format_audio``).  Requests in different formats share a forward: one output
+    launch set (a loudness measurement for a ``loudness`` target, the limiter's passes for a ``true_peak`` ceiling) and one copy
+    per distinct format.
     """
 
     def __init__(self, forward, device="cpu", max_batch=32, max_wait_s=0.005, hop=256):
@@ -278,48 +279,50 @@ class MicroBatcher:
         self._thread.start()
 
     def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0, durations=None,
-               pitch=None, energy=None, sample_rate=None, encoding=None, loudness=None):
+               pitch=None, energy=None, sample_rate=None, encoding=None, loudness=None, true_peak=None):
         """``speed`` > 1 speaks faster (duration_scale = 1 / speed); ``pitch_shift`` in semitones; ``energy_scale``
         multiplies frame energy.  Each is a float or a sequence of ``len(ids)`` values, one per phoneme (a per-phoneme speed
         must lie in [1/16, 16]).  ``durations`` (integer frames), ``pitch`` and ``energy`` (the predictors' normalised units):
         None or ``len(ids)`` values that replace the model's predictions (see ``JETSGenerator.forward``).  ``sample_rate`` /
-        ``encoding`` / ``loudness``: see ``_output_format``.  Invalid values raise ValueError here, so they cannot fail a batch of
-        other requests."""
+        ``encoding`` / ``loudness`` / ``true_peak``: see ``_output_format``.  Invalid values raise ValueError here, so they cannot
+        fail a batch of other requests."""
         ids = np.asarray(ids, dtype=np.int64)
         controls = phoneme_controls(len(ids), speed, pitch_shift, energy_scale)
         given = given_values(len(ids), durations, pitch, energy)
-        fmt = self._output_format(sample_rate, encoding, loudness)
+        fmt = self._output_format(sample_rate, encoding, loudness, true_peak)
         item = (ids, int(speaker_id), style_vec, content_vec, controls) + ((given,) if given else ())
         return self._enqueue([item], False, fmt)
 
     def submit_joined(self, segments, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0,
-                      sample_rate=None, encoding=None, loudness=None):
+                      sample_rate=None, encoding=None, loudness=None, true_peak=None):
         """One long text as ``segments``: a list of phoneme id arrays, e.g. ``split_phonemes`` output put through ``encode``.
         ``style_vec`` / ``content_vec``: one vector for every segment, or a list (or a 2-D array) with one vector per segment,
         for a different prompt per sentence.  ``speed`` / ``pitch_shift`` / ``energy_scale``: one float each, checked as in
         ``submit``.  The future's result is the text's float32 waveform, the segments' mel joined and vocoded as one,
-        trimmed to ``joined_lengths[g] * hop``, or that waveform in the format of ``sample_rate`` / ``encoding`` / ``loudness``
-        (see ``_output_format``).  Raises ValueError here for invalid arguments."""
+        trimmed to ``joined_lengths[g] * hop``, or that waveform in the format of ``sample_rate`` / ``encoding`` / ``loudness`` /
+        ``true_peak`` (see ``_output_format``).  Raises ValueError here for invalid arguments."""
         segs = [np.asarray(s, dtype=np.int64) for s in segments]
         if not segs or any(s.ndim != 1 or s.size == 0 for s in segs):
             raise ValueError("segments must be a non-empty list of non-empty 1-D phoneme id arrays")
         controls = speech_controls(speed, pitch_shift, energy_scale)
         styles = _per_segment("style_vec", style_vec, len(segs))
         contents = _per_segment("content_vec", content_vec, len(segs))
-        fmt = self._output_format(sample_rate, encoding, loudness)
+        fmt = self._output_format(sample_rate, encoding, loudness, true_peak)
         items = [(s, int(speaker_id), st, ct, controls) for s, st, ct in zip(segs, styles, contents)]
         return self._enqueue(items, True, fmt)
 
-    def _output_format(self, sample_rate, encoding, loudness):
-        """A request's output format: None when all three are None (the result is the float32 waveform tensor, as always), else
-        (rate, encoding, loudness) for ``fetch_audio``: the result is then a numpy array at ``sample_rate`` (None: the model's
-        rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None: not normalised).  Raises ValueError for a
-        rate, encoding or loudness target ``format_audio`` does not take."""
-        if sample_rate is None and encoding is None and loudness is None:
+    def _output_format(self, sample_rate, encoding, loudness, true_peak=None):
+        """A request's output format: None when all four are None (the result is the float32 waveform tensor, as always), else
+        (rate, encoding, loudness) for ``fetch_audio``, with true_peak appended when it is given: the result is then a numpy
+        array at ``sample_rate`` (None: the model's rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None:
+        not normalised) and limited to ``true_peak`` dBTP (None: not limited).  Raises ValueError for a rate, encoding, loudness
+        target or ceiling ``format_audio`` does not take."""
+        if sample_rate is None and encoding is None and loudness is None and true_peak is None:
             return None
         encoding = "pcm16" if encoding is None else encoding
         rate, _, _ = audio.plan(sample_rate, encoding, self._sr)
-        return rate, encoding, None if loudness is None else audio.check_loudness(loudness)
+        fmt = (rate, encoding, None if loudness is None else audio.check_loudness(loudness))
+        return fmt if true_peak is None else fmt + (audio.check_true_peak(true_peak),)
 
     def _enqueue(self, items, joined, fmt):
         fut = Future()
@@ -382,14 +385,16 @@ class MicroBatcher:
                 kw["join"] = [g for g, e in enumerate(batch) for _ in e[0]]
             out = self._forward(**kw)
             # request r's output is item r of the forward (group r of a joined one); one format_audio call and one copy
-            # per distinct (rate, encoding, loudness), over the requests that asked for it
+            # per distinct (rate, encoding, loudness[, true_peak]), over the requests that asked for it
             formats = {}
             for r, e in enumerate(batch):
                 if e[3] is not None:
                     formats.setdefault(e[3], []).append(r)
             results = {}
-            for (rate, encoding, loudness), rs in formats.items():
-                results.update(zip(rs, fetch_audio(self._forward, out, rate, encoding, items=rs, hop=self._hop, loudness=loudness)))
+            for fmt, rs in formats.items():
+                extra = {} if len(fmt) < 4 else {"true_peak": fmt[3]}
+                results.update(zip(rs, fetch_audio(self._forward, out, fmt[0], fmt[1], items=rs, hop=self._hop, loudness=fmt[2],
+                                                   **extra)))
             if len(results) < len(batch):
                 wav = out["wav_predictions"]
                 lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
@@ -461,15 +466,18 @@ def audio_to_wav_bytes(samples, sample_rate, encoding="pcm16"):
     return header + data + b"\0" * pad
 
 
-def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None):
+def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
     """Finish one forward in the format a client asked for: ``model.format_audio`` resamples to ``sample_rate`` (None: the
     model's 16 kHz) and encodes ("float32", "pcm16", "mulaw" or "alaw") only the valid samples of each output, packed, on the
     GPU, after normalising each output to ``loudness`` LUFS when that is given (BS.1770-4 integrated loudness, -1 dBFS
-    sample-peak ceiling; see ``format_audio``); then ONE device->host copy of that buffer into pinned memory.  ``out`` is the
+    sample-peak ceiling; see ``format_audio``) and limiting each to ``true_peak`` dBTP when that is given (a look-ahead
+    true-peak limiter, which replaces the sample-peak ceiling); then ONE device->host copy of that buffer into pinned memory.  ``out`` is the
     dict ``model(...)`` returned; ``items`` selects outputs (default: all).  Returns a list of 1-D numpy arrays (float32, int16
     or uint8), one per batch item, or per group of a joined forward.  "flac": each array is the bytes of a complete .flac file
     whose samples are the "pcm16" result.  Invalid arguments raise ValueError before anything is enqueued."""
     extra = {} if loudness is None else {"loudness": loudness}
+    if true_peak is not None:
+        extra["true_peak"] = true_peak
     packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, **extra)
     host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)
     host.copy_(packed, non_blocking=True)

@@ -259,6 +259,7 @@ class _Engine:
         self.call_lock = threading.RLock()      # one forward at a time enqueues on an engine (its workspaces are reused, stream-ordered)
         self._banks = {}              # (up, down) -> device polyphase filter bank of format_audio
         self._kcoef = {}              # sample rate -> K-weighting coefficients of ev_loudness (host float64)
+        self._limit_banks = {}        # (model rate, output rate) -> (device detector bank, hold) of ev_limit
         self.ensure_pe(5000)          # PositionalEncoding max_len=5000 (encoder.py:206)
         self.total_up = int(np.prod([self.cfg.up_rates[i] for i in range(self.cfg.n_ups)]))
 
@@ -465,10 +466,51 @@ class _Engine:
         lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
         return lufs, pk
 
-    def format_audio(self, wav, n_in, items, up, down, encoding, loudness=None, sr=None):
+    def _limit(self, wav, n_in_ptr, items_ptr, k, sr, rate, lufs0, lufs1, target, ceiling, out):
+        """ev_limit of the k listed items into ``out`` (k, L) fp32, pre-gain 10^((target - L) / 20) of each given loudness."""
+        det = self._limit_banks.get((sr, rate))
+        if det is None:
+            bank, hold = audio.limit_bank(sr, rate)
+            det = self._limit_banks[(sr, rate)] = (torch.from_numpy(bank).to(self.device), hold)
+        bank, hold = det
+        L = audio.limit_lookahead(sr)
+        stride = int(wav.stride(0))
+        ws = self._ws("limit", self.lib.ev_limit_workspace_bytes(k, stride, L))
+        _abi.check(self.lib.ev_limit(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, None if lufs0 is None else lufs0.data_ptr(),
+                                     None if lufs1 is None else lufs1.data_ptr(), float(-23.0 if target is None else target),
+                                     float(ceiling), bank.data_ptr(), int(bank.shape[0]), int(bank.shape[1]), L, hold,
+                                     audio.limit_release(sr), out.data_ptr(), int(out.stride(0)), ws.data_ptr(), ws.numel(),
+                                     self._stream()))
+
+    def _limited(self, wav, n_in, items, sr, rate, loudness, ceiling):
+        """The true-peak limited waveforms of the listed items: (len(items), 1, L) fp32 and their valid samples (host list).
+        With a loudness target, two passes: limit x * g1 (g1 = 10^((T - L0) / 20)), measure that result's L1, and limit x * g2
+        from the original samples, g2 = g1 * 10^((T - L1) / 20).  No sync."""
+        k = len(items)
+        n_list = [int(n_in[b]) for b in items]
+        meta, (p_n, p_items, p_nl) = self._meta([n_in, items, n_list])
+        stride = int(wav.stride(0))
+        out = self._ws("limited", 4 * k * stride)[:4 * k * stride].view(torch.float32).view(k, 1, stride)
+        lufs0 = None
+        if loudness is not None:
+            lufs0 = self._loudness(wav, p_n, p_items, k, sr, loudness)[0]
+            self._limit(wav, p_n, p_items, k, sr, rate, lufs0, None, loudness, ceiling, out[:, 0])
+            lufs1 = self._loudness(out, p_nl, None, k, sr, loudness)[0]
+            self._limit(wav, p_n, p_items, k, sr, rate, lufs0, lufs1, loudness, ceiling, out[:, 0])
+        else:
+            self._limit(wav, p_n, p_items, k, sr, rate, None, None, None, ceiling, out[:, 0])
+        return out, n_list, meta
+
+    def format_audio(self, wav, n_in, items, up, down, encoding, loudness=None, sr=None, true_peak=None):
         """ev_format_audio: (B,1,L) fp32 waveform, host per-item valid samples ``n_in`` (B ints <= L) and the listed item indices
         -> (packed device tensor, (len(items)+1,) int64 host offsets).  The filter bank of a ratio is uploaded once per engine.
-        ``loudness`` (LUFS, or None): ev_loudness at ``sr`` Hz first, and its gains go to ev_format_audio_gain."""
+        ``loudness`` (LUFS, or None): ev_loudness at ``sr`` Hz first, and its gains go to ev_format_audio_gain.
+        ``true_peak`` (dBTP, or None): the items are first limited by ``_limited`` (which also applies the loudness gain), and
+        the limited waveforms go through ev_format_audio with no gain."""
+        if true_peak is not None and sum(int(n_in[b]) for b in items) > 0:
+            rate = sr * up // down
+            lim, n_list, meta = self._limited(wav, n_in, items, sr, rate, loudness, true_peak)     # meta: the limiter's device lengths
+            return self.format_audio(lim, n_list, list(range(len(items))), up, down, encoding, None, sr)
         dev = self.device
         bank = None
         if (up, down) != (1, 1):
@@ -496,12 +538,12 @@ class _Engine:
                                                  gain.data_ptr(), self._stream()))
         return packed, offs
 
-    def format_flac(self, wav, n_in, items, up, down, rate, loudness=None, sr=None):
+    def format_flac(self, wav, n_in, items, up, down, rate, loudness=None, sr=None, true_peak=None):
         """``format_audio`` to PCM16 at ``rate`` Hz, then ev_flac_encode -> (uint8 device tensor of the len(items) .flac images
         back to back, (len(items)+1,) int64 host offsets).  The image sizes are known only after encoding: one device->host
         read of the offsets, the call's only sync."""
         lib = self.lib
-        pcm, offs = self.format_audio(wav, n_in, items, up, down, "pcm16", loudness, sr)
+        pcm, offs = self.format_audio(wav, n_in, items, up, down, "pcm16", loudness, sr, true_peak)
         counts = np.ascontiguousarray(np.diff(offs), dtype=np.int64)
         k = len(items)
         bound = sum(int(lib.ev_flac_bound_bytes(int(n))) for n in counts)
@@ -873,7 +915,7 @@ class JETSGenerator(_EngineOwner):
             return eng.measure_loudness(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
 
     @torch.no_grad()
-    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None):
+    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
         """The output of a forward in a client's format, on the GPU: each output's valid samples, resampled to ``sample_rate``
         (None: the model's rate, ``config.sr``, 16000) and encoded, packed back to back.
 
@@ -891,6 +933,15 @@ class JETSGenerator(_EngineOwner):
         gain is the same at every output rate, since resampling is linear.  None: no measurement, and the output is exactly
         as without the argument.
 
+        ``true_peak`` (a ceiling in dBTP, in [-20, 0], or None): a look-ahead limiter holds each output at or below the ceiling
+        in true peak (``ev_limit``, run at the model's rate before resampling).  Its pre-gain is 10^((loudness - L) / 20) with no
+        sample-peak cap (1 without ``loudness`` or where L = -inf).  With ``loudness``, two passes: the limited output is measured
+        again (L1) and the original samples are limited once more under the pre-gain times 10^((loudness - L1) / 20), so the
+        target is reached where limiting took loudness away.  The detector oversamples to 192 kHz (12x at 16 kHz) and, for a
+        rate below the model's, also low-passes as the resampler does; look-ahead 5 ms, linear release 60 dB/s.  The limited
+        waveform is then resampled and encoded with no further gain.  None: the limiter does not run, and the output is exactly
+        as without the argument.
+
         ``encoding="flac"``: each output becomes a complete .flac file image (RFC 9639: mono, 16 bits, 4096-sample blocks) of
         exactly the samples "pcm16" gives, encoded on the GPU by ev_flac_encode; decoding it returns that PCM16 bit for bit.
         The images' sizes exist only after encoding, so this encoding makes ONE device->host read of the len(items) + 1
@@ -903,11 +954,13 @@ class JETSGenerator(_EngineOwner):
         rate, up, down = audio.plan(sample_rate, encoding, sr)
         if loudness is not None:
             loudness = audio.check_loudness(loudness)
+        if true_peak is not None:
+            true_peak = audio.check_true_peak(true_peak)
         wav, n_in, items, eng = self._outputs(out, items, hop)
         if encoding == audio.FLAC:
             if any(n_in[b] < 1 for b in items):
                 raise ValueError("an output with no samples cannot be a FLAC stream (valid samples %s)" % [n_in[b] for b in items])
             with eng.call_lock:
-                return eng.format_flac(wav, n_in, items, up, down, rate, loudness, sr)
+                return eng.format_flac(wav, n_in, items, up, down, rate, loudness, sr, true_peak)
         with eng.call_lock:
-            return eng.format_audio(wav, n_in, items, up, down, encoding, loudness, sr)
+            return eng.format_audio(wav, n_in, items, up, down, encoding, loudness, sr, true_peak)

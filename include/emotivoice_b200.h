@@ -277,6 +277,27 @@ EV_API int ev_loudness(const float* wav, long long item_stride, const int64_t* n
                        const double* kcoef, float target_lufs, float* lufs, float* peak, float* gain, void* ws, size_t ws_bytes,
                        void* stream);
 
+/* True-peak limiter of listed waveform items: holds each item, scaled by its loudness pre-gain, at or below ceiling_dbtp in
+ * true peak, before ev_format_audio resamples and encodes it.  wav / item_stride / n_in / items / n_items as ev_loudness.
+ *   Pre-gain g = 10^((target_lufs - lufs0[k]) / 20) * 10^((target_lufs - lufs1[k]) / 20) in fp64, a factor 1 where its array is
+ *   NULL or its loudness is -inf (lufs0 / lufs1: (n_items) f32 device arrays, ev_loudness's lufs; lufs1 needs lufs0;
+ *   target_lufs in [-70, 0] when lufs0 is given).  ceiling_dbtp in [-20, 0].
+ *   Detector: p[s] = max(|x[s]|, |sum_j bank[ph][j] * x[s + c - j]| over the phases ph), c = (taps - 1) / 2, x zero outside
+ *   [0, n): bank (phases, taps) f32 device array, taps odd (emotivoice_b200.audio.limit_bank).  Required gain r[s] = min(0,
+ *   ceiling - 20 log10(g p[s])) in fp64, at least -1000 dB, rounded down to a multiple of 2^-32 dB.
+ *   Envelope: m[s] = min r over [s - hold, s + lookahead + hold] (r = 0 outside the item), for s from -lookahead; release
+ *   G1[s] = min(m[s], G1[s - 1] + release_db_per_sample) from G1 = 0, computed as an exact fp64 prefix minimum
+ *   (release_db_per_sample in (0, 1], a multiple of 2^-32); attack G[s] = mean of G1 over [s - lookahead, s], so G[s] <= r[s].
+ *   hold >= (taps - 1) / 2, lookahead in [0, 1024].
+ *   out[k * out_stride + s] = fp32(x[s] * g * 10^(G[s] / 20)) for s < n (out_stride >= item_stride); nothing else is written.
+ *   ws: ev_limit_workspace_bytes(n_items, item_stride, lookahead) bytes.  Three launches; an item's output is bitwise the same
+ *   in any batch or order.  No allocation, no sync. */
+EV_API size_t ev_limit_workspace_bytes(int n_items, long long max_n, int lookahead);   /* 0 for arguments out of range */
+EV_API int ev_limit(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items, int sample_rate,
+                    const float* lufs0, const float* lufs1, float target_lufs, float ceiling_dbtp, const float* bank, int phases,
+                    int taps, int lookahead, int hold, double release_db_per_sample, float* out, long long out_stride, void* ws,
+                    size_t ws_bytes, void* stream);
+
 /* FLAC (RFC 9639) file images of int16 items, the lossless compressed response of a TTS server: item k is pcm[pcm_off[k] ..
  * pcm_off[k + 1]) (pcm_off (n_items + 1) i64 DEVICE array, items packed back to back as ev_format_audio writes EV_AUDIO_PCM16),
  * n_samples (n_items) i64 HOST array of the same counts (each in [1, 2^36]; it sizes the grid and the checks below).
