@@ -66,8 +66,7 @@ SIGNATURES = {
     "ev_vocoder": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "ev_join_mel": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "ev_wav_to_pcm16": (_i, [_vp, _vp, _sz, _vp]),
-    "ev_format_audio": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    "ev_format_audio_gain": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "ev_format_audio": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "ev_loudness_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),
     "ev_loudness": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_limit_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),

@@ -7,6 +7,7 @@ Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the
 ``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
 item of n samples gives ``ceil(n * up / down)`` samples.
 """
+import collections
 import math
 
 import numpy as np
@@ -95,6 +96,20 @@ def check_true_peak(ceiling):
     if not (math.isfinite(c) and TRUE_PEAK_RANGE[0] <= c <= TRUE_PEAK_RANGE[1]):
         raise ValueError("true_peak must be a finite ceiling in [%g, %g] dBTP, got %r" % (TRUE_PEAK_RANGE + (ceiling,)))
     return c
+
+
+# A validated output format: the rate and its resampling factors from the source rate, the encoding ("flac" or one of
+# ENCODINGS), the loudness target (LUFS) and the true-peak ceiling (dBTP), each None when not asked for.  Hashable: the
+# MicroBatcher formats all requests of one key with one call.
+OutputFormat = collections.namedtuple("OutputFormat", "rate up down encoding loudness true_peak")
+
+
+def output_format(sample_rate, encoding, loudness, true_peak, source_rate):
+    """The arguments of ``format_audio`` -> ``OutputFormat``, checked by ``plan``, ``check_loudness`` and ``check_true_peak`` in
+    that order.  Raises their ValueError otherwise."""
+    rate, up, down = plan(sample_rate, encoding, source_rate)
+    return OutputFormat(rate, up, down, encoding, None if loudness is None else check_loudness(loudness),
+                        None if true_peak is None else check_true_peak(true_peak))
 
 
 # The true-peak limiter of ev_limit: fixed constants, not options.

@@ -942,19 +942,13 @@ int ev_wav_to_pcm16(const float* wav, int16_t* pcm, size_t n, void* stream) {
   return launch_pcm16(wav, pcm, n, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int ev_format_audio_gain(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
-                         const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
-                         const float* gain, void* stream) {
+int ev_format_audio(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
+                    const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
+                    const float* gain, void* stream) {
   EV_CHECK_ARG(wav && n_in && out_off && out, "ev_format_audio: null argument");
   EV_TRY(use_device_of(wav));
   return launch_audio_out(wav, item_stride, n_in, items, n_items, out_off, bank, up, down, taps_per_phase, encoding, gain, out,
                           reinterpret_cast<cudaStream_t>(stream));
-}
-
-int ev_format_audio(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items, const int64_t* out_off,
-                    const float* bank, int up, int down, int taps_per_phase, int encoding, void* out, void* stream) {
-  return ev_format_audio_gain(wav, item_stride, n_in, items, n_items, out_off, bank, up, down, taps_per_phase, encoding, out, nullptr,
-                              stream);
 }
 
 int ev_op_conv1d(const float* x, const float* w, const float* bias, size_t bias_bstride, const float* res, float* out,

@@ -252,7 +252,7 @@ int launch_conv_post(const float* x, const float* w, const float* bias, const in
                      int L, int C, int K, float slope, float* wav, cudaStream_t st);
 int launch_pcm16(const float* wav, int16_t* pcm, size_t n, cudaStream_t st);
 // resample by up/down (scipy.signal.resample_poly, default filter) + scale by an optional per-item gain + encode the valid samples
-// of listed waveform items, packed (ev_format_audio, ev_format_audio_gain)
+// of listed waveform items, packed (ev_format_audio)
 constexpr int AO_MAX_FACTOR = 1024;
 int launch_audio_out(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
                      const int64_t* out_off, const float* bank, int up, int down, int taps, int encoding, const float* gain, void* out,

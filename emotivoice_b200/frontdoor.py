@@ -313,16 +313,13 @@ class MicroBatcher:
 
     def _output_format(self, sample_rate, encoding, loudness, true_peak=None):
         """A request's output format: None when all four are None (the result is the float32 waveform tensor, as always), else
-        (rate, encoding, loudness) for ``fetch_audio``, with true_peak appended when it is given: the result is then a numpy
-        array at ``sample_rate`` (None: the model's rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None:
-        not normalised) and limited to ``true_peak`` dBTP (None: not limited).  Raises ValueError for a rate, encoding, loudness
-        target or ceiling ``format_audio`` does not take."""
+        the ``audio.OutputFormat`` ``fetch_audio`` is called with: the result is then a numpy array at ``sample_rate`` (None: the
+        model's rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None: not normalised) and limited to
+        ``true_peak`` dBTP (None: not limited).  Raises ValueError for a rate, encoding, loudness target or ceiling
+        ``format_audio`` does not take."""
         if sample_rate is None and encoding is None and loudness is None and true_peak is None:
             return None
-        encoding = "pcm16" if encoding is None else encoding
-        rate, _, _ = audio.plan(sample_rate, encoding, self._sr)
-        fmt = (rate, encoding, None if loudness is None else audio.check_loudness(loudness))
-        return fmt if true_peak is None else fmt + (audio.check_true_peak(true_peak),)
+        return audio.output_format(sample_rate, "pcm16" if encoding is None else encoding, loudness, true_peak, self._sr)
 
     def _enqueue(self, items, joined, fmt):
         fut = Future()
@@ -385,16 +382,15 @@ class MicroBatcher:
                 kw["join"] = [g for g, e in enumerate(batch) for _ in e[0]]
             out = self._forward(**kw)
             # request r's output is item r of the forward (group r of a joined one); one format_audio call and one copy
-            # per distinct (rate, encoding, loudness[, true_peak]), over the requests that asked for it
+            # per distinct OutputFormat, over the requests that asked for it
             formats = {}
             for r, e in enumerate(batch):
                 if e[3] is not None:
                     formats.setdefault(e[3], []).append(r)
             results = {}
-            for fmt, rs in formats.items():
-                extra = {} if len(fmt) < 4 else {"true_peak": fmt[3]}
-                results.update(zip(rs, fetch_audio(self._forward, out, fmt[0], fmt[1], items=rs, hop=self._hop, loudness=fmt[2],
-                                                   **extra)))
+            for f, rs in formats.items():
+                results.update(zip(rs, fetch_audio(self._forward, out, f.rate, f.encoding, items=rs, hop=self._hop, loudness=f.loudness,
+                                                   true_peak=f.true_peak)))
             if len(results) < len(batch):
                 wav = out["wav_predictions"]
                 lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
@@ -475,10 +471,7 @@ def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=
     dict ``model(...)`` returned; ``items`` selects outputs (default: all).  Returns a list of 1-D numpy arrays (float32, int16
     or uint8), one per batch item, or per group of a joined forward.  "flac": each array is the bytes of a complete .flac file
     whose samples are the "pcm16" result.  Invalid arguments raise ValueError before anything is enqueued."""
-    extra = {} if loudness is None else {"loudness": loudness}
-    if true_peak is not None:
-        extra["true_peak"] = true_peak
-    packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, **extra)
+    packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, loudness=loudness, true_peak=true_peak)
     host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)
     host.copy_(packed, non_blocking=True)
     torch.cuda.current_stream(packed.device).synchronize()

@@ -17,13 +17,14 @@ ABI in include/emotivoice_b200.h.  PyTorch provides device memory and the stream
 is no CPU path: calling ``forward`` on CPU tensors raises.
 """
 import ctypes
+import functools
 import threading
 
 import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _abi, audio, packing, synth
+from . import _abi, audio, output, packing, synth
 
 
 class _Holder(nn.Module):
@@ -198,6 +199,21 @@ def _bucket(nbytes):
     return b
 
 
+def _workspace(arena, device, kind, nbytes):
+    """Grow-only workspace arena ``arena``: (stream, kind) -> uint8 buffer: after the largest request has been seen (or
+    `reserve`d) no call allocates device memory any more -- a fresh cudaMalloc in the middle of a forward is a
+    device-synchronising stall of milliseconds.  Reuse across calls is safe because every use is ordered on the stream the
+    buffer belongs to."""
+    key = (torch.cuda.current_stream(device).cuda_stream, kind)
+    t = arena.get(key)
+    if t is None or t.numel() < nbytes:
+        arena.pop(key, None)
+        t = None
+        t = torch.empty((_bucket(nbytes),), dtype=torch.uint8, device=device)
+        arena[key] = t
+    return t
+
+
 def _register(root, dotted, tensor):
     parts = dotted.split(".")
     mod = root
@@ -255,11 +271,10 @@ class _Engine:
         _abi.check(self.lib.ev_bind_weights(self.handle, self.blob.data_ptr(), self.blob.numel(),
                                             ctypes.cast(self.index, ctypes.c_void_p), len(self.index)))
         self.pe = None
-        self._arena = {}              # (stream, kind) -> uint8 workspace, grow-only
+        # the arena does not refer back to the engine, so the output chain can hold it without a reference cycle
+        self._ws = functools.partial(_workspace, {}, self.device)
         self.call_lock = threading.RLock()      # one forward at a time enqueues on an engine (its workspaces are reused, stream-ordered)
-        self._banks = {}              # (up, down) -> device polyphase filter bank of format_audio
-        self._kcoef = {}              # sample rate -> K-weighting coefficients of ev_loudness (host float64)
-        self._limit_banks = {}        # (model rate, output rate) -> (device detector bank, hold) of ev_limit
+        self.output = output.Chain(self.device, self.lib, self._ws)
         self.ensure_pe(5000)          # PositionalEncoding max_len=5000 (encoder.py:206)
         self.total_up = int(np.prod([self.cfg.up_rates[i] for i in range(self.cfg.n_ups)]))
 
@@ -288,19 +303,6 @@ class _Engine:
     # -- calls ------------------------------------------------------------------------
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
-
-    def _ws(self, kind, nbytes):
-        """Grow-only workspace arena, one buffer per (stream, kind): after the largest request has been seen (or `reserve`d) no call
-        allocates device memory any more -- a fresh cudaMalloc in the middle of a forward is a device-synchronising stall of
-        milliseconds.  Reuse across calls is safe because every use is ordered on the stream the buffer belongs to."""
-        key = (self._stream(), kind)
-        t = self._arena.get(key)
-        if t is None or t.numel() < nbytes:
-            self._arena.pop(key, None)
-            t = None
-            t = torch.empty((_bucket(nbytes),), dtype=torch.uint8, device=self.device)
-            self._arena[key] = t
-        return t
 
     def reserve(self, batch, phonemes, frames):
         """Pre-size the arena of the current stream for requests up to (batch, phonemes, frames)."""
@@ -435,130 +437,6 @@ class _Engine:
         _abi.check(self.lib.ev_join_mel(mel.data_ptr(), mel_lens.data_ptr(), group.data_ptr(), B, F, C, G, Fg, joined.data_ptr(),
                                         lens.data_ptr(), self._stream()))
         return joined, lens
-
-    def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
-        """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
-        kc = self._kcoef.get(sr)
-        if kc is None:
-            kc = self._kcoef[sr] = np.ascontiguousarray(audio.k_weighting(sr))
-        res = torch.empty((3, k), dtype=torch.float32, device=self.device)
-        nbytes = self.lib.ev_loudness_workspace_bytes(k, int(wav.stride(0)), sr)
-        ws = self._ws("loudness", nbytes)
-        _abi.check(self.lib.ev_loudness(wav.data_ptr(), int(wav.stride(0)), n_in_ptr, items_ptr, k, sr, kc.ctypes.data, float(target),
-                                        res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(), ws.numel(),
-                                        self._stream()))
-        return res[0], res[1], res[2]
-
-    def _meta(self, arrays):
-        """Host int64 arrays -> one device int64 tensor (one pinned copy) and the device address of each array in it."""
-        meta = torch.from_numpy(np.concatenate([np.asarray(a, np.int64) for a in arrays]))
-        meta = meta.pin_memory().to(self.device, non_blocking=True)
-        ptrs, p = [], meta.data_ptr()
-        for a in arrays:
-            ptrs.append(p)
-            p += 8 * len(a)
-        return meta, ptrs
-
-    def measure_loudness(self, wav, n_in, items, sr):
-        """ev_loudness: (B,1,L) fp32 waveform at ``sr`` Hz, host per-item valid samples and the listed items -> device
-        (lufs, peak) float32 (len(items),)."""
-        meta, (p_n, p_items) = self._meta([n_in, items])
-        lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
-        return lufs, pk
-
-    def _limit(self, wav, n_in_ptr, items_ptr, k, sr, rate, lufs0, lufs1, target, ceiling, out):
-        """ev_limit of the k listed items into ``out`` (k, L) fp32, pre-gain 10^((target - L) / 20) of each given loudness."""
-        det = self._limit_banks.get((sr, rate))
-        if det is None:
-            bank, hold = audio.limit_bank(sr, rate)
-            det = self._limit_banks[(sr, rate)] = (torch.from_numpy(bank).to(self.device), hold)
-        bank, hold = det
-        L = audio.limit_lookahead(sr)
-        stride = int(wav.stride(0))
-        ws = self._ws("limit", self.lib.ev_limit_workspace_bytes(k, stride, L))
-        _abi.check(self.lib.ev_limit(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, None if lufs0 is None else lufs0.data_ptr(),
-                                     None if lufs1 is None else lufs1.data_ptr(), float(-23.0 if target is None else target),
-                                     float(ceiling), bank.data_ptr(), int(bank.shape[0]), int(bank.shape[1]), L, hold,
-                                     audio.limit_release(sr), out.data_ptr(), int(out.stride(0)), ws.data_ptr(), ws.numel(),
-                                     self._stream()))
-
-    def _limited(self, wav, n_in, items, sr, rate, loudness, ceiling):
-        """The true-peak limited waveforms of the listed items: (len(items), 1, L) fp32 and their valid samples (host list).
-        With a loudness target, two passes: limit x * g1 (g1 = 10^((T - L0) / 20)), measure that result's L1, and limit x * g2
-        from the original samples, g2 = g1 * 10^((T - L1) / 20).  No sync."""
-        k = len(items)
-        n_list = [int(n_in[b]) for b in items]
-        meta, (p_n, p_items, p_nl) = self._meta([n_in, items, n_list])
-        stride = int(wav.stride(0))
-        out = self._ws("limited", 4 * k * stride)[:4 * k * stride].view(torch.float32).view(k, 1, stride)
-        lufs0 = None
-        if loudness is not None:
-            lufs0 = self._loudness(wav, p_n, p_items, k, sr, loudness)[0]
-            self._limit(wav, p_n, p_items, k, sr, rate, lufs0, None, loudness, ceiling, out[:, 0])
-            lufs1 = self._loudness(out, p_nl, None, k, sr, loudness)[0]
-            self._limit(wav, p_n, p_items, k, sr, rate, lufs0, lufs1, loudness, ceiling, out[:, 0])
-        else:
-            self._limit(wav, p_n, p_items, k, sr, rate, None, None, None, ceiling, out[:, 0])
-        return out, n_list, meta
-
-    def format_audio(self, wav, n_in, items, up, down, encoding, loudness=None, sr=None, true_peak=None):
-        """ev_format_audio: (B,1,L) fp32 waveform, host per-item valid samples ``n_in`` (B ints <= L) and the listed item indices
-        -> (packed device tensor, (len(items)+1,) int64 host offsets).  The filter bank of a ratio is uploaded once per engine.
-        ``loudness`` (LUFS, or None): ev_loudness at ``sr`` Hz first, and its gains go to ev_format_audio_gain.
-        ``true_peak`` (dBTP, or None): the items are first limited by ``_limited`` (which also applies the loudness gain), and
-        the limited waveforms go through ev_format_audio with no gain."""
-        if true_peak is not None and sum(int(n_in[b]) for b in items) > 0:
-            rate = sr * up // down
-            lim, n_list, meta = self._limited(wav, n_in, items, sr, rate, loudness, true_peak)     # meta: the limiter's device lengths
-            return self.format_audio(lim, n_list, list(range(len(items))), up, down, encoding, None, sr)
-        dev = self.device
-        bank = None
-        if (up, down) != (1, 1):
-            bank = self._banks.get((up, down))
-            if bank is None:
-                bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev)
-                self._banks[(up, down)] = bank
-        offs = audio.packed_offsets(n_in, items, up, down)
-        dtype = {"float32": torch.float32, "pcm16": torch.int16, "mulaw": torch.uint8, "alaw": torch.uint8}[encoding]
-        packed = torch.empty((int(offs[-1]),), dtype=dtype, device=dev)
-        if packed.numel() == 0:
-            return packed, offs
-        k = len(items)
-        meta, (p_n, p_items, p_off) = self._meta([n_in, items, offs[:-1]])
-        if loudness is None:
-            _abi.check(self.lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), p_n, p_items, k, p_off,
-                                                None if bank is None else bank.data_ptr(), up, down,
-                                                0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
-                                                self._stream()))
-            return packed, offs
-        _, _, gain = self._loudness(wav, p_n, p_items, k, sr, loudness)
-        _abi.check(self.lib.ev_format_audio_gain(wav.data_ptr(), int(wav.stride(0)), p_n, p_items, k, p_off,
-                                                 None if bank is None else bank.data_ptr(), up, down,
-                                                 0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
-                                                 gain.data_ptr(), self._stream()))
-        return packed, offs
-
-    def format_flac(self, wav, n_in, items, up, down, rate, loudness=None, sr=None, true_peak=None):
-        """``format_audio`` to PCM16 at ``rate`` Hz, then ev_flac_encode -> (uint8 device tensor of the len(items) .flac images
-        back to back, (len(items)+1,) int64 host offsets).  The image sizes are known only after encoding: one device->host
-        read of the offsets, the call's only sync."""
-        lib = self.lib
-        pcm, offs = self.format_audio(wav, n_in, items, up, down, "pcm16", loudness, sr, true_peak)
-        counts = np.ascontiguousarray(np.diff(offs), dtype=np.int64)
-        k = len(items)
-        bound = sum(int(lib.ev_flac_bound_bytes(int(n))) for n in counts)
-        out = torch.empty((bound,), dtype=torch.uint8, device=self.device)
-        out_off = torch.empty((k + 1,), dtype=torch.int64, device=self.device)
-        pcm_off = torch.from_numpy(offs).pin_memory().to(self.device, non_blocking=True)
-        nbytes = lib.ev_flac_workspace_bytes(k, int(counts.max()))
-        ws = self._ws("flac", nbytes)
-        _abi.check(lib.ev_flac_encode(pcm.data_ptr(), pcm_off.data_ptr(), k, counts.ctypes.data, int(rate), out.data_ptr(), bound,
-                                      out_off.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
-        host = torch.empty((k + 1,), dtype=torch.int64, pin_memory=True)
-        host.copy_(out_off, non_blocking=True)
-        torch.cuda.current_stream(self.device).synchronize()
-        flac_offs = host.numpy().copy()
-        return out[:int(flac_offs[-1])], flac_offs
 
 
 class _EngineOwner(nn.Module):
@@ -912,7 +790,7 @@ class JETSGenerator(_EngineOwner):
         than 400 ms or with no 400 ms block above the gates (silence).  No sync."""
         wav, n_in, items, eng = self._outputs(out, items, hop)
         with eng.call_lock:
-            return eng.measure_loudness(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
+            return eng.output.measure(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
 
     @torch.no_grad()
     def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
@@ -951,16 +829,9 @@ class JETSGenerator(_EngineOwner):
         ``packed[offs[k]:offs[k + 1]]``).  No sync except for "flac": the lengths are the host copies the forward read.
         Invalid arguments raise ValueError before anything is enqueued."""
         sr = int(getattr(self.config, "sr", 16000))
-        rate, up, down = audio.plan(sample_rate, encoding, sr)
-        if loudness is not None:
-            loudness = audio.check_loudness(loudness)
-        if true_peak is not None:
-            true_peak = audio.check_true_peak(true_peak)
+        fmt = audio.output_format(sample_rate, encoding, loudness, true_peak, sr)
         wav, n_in, items, eng = self._outputs(out, items, hop)
-        if encoding == audio.FLAC:
-            if any(n_in[b] < 1 for b in items):
-                raise ValueError("an output with no samples cannot be a FLAC stream (valid samples %s)" % [n_in[b] for b in items])
-            with eng.call_lock:
-                return eng.format_flac(wav, n_in, items, up, down, rate, loudness, sr, true_peak)
+        if encoding == audio.FLAC and any(n_in[b] < 1 for b in items):
+            raise ValueError("an output with no samples cannot be a FLAC stream (valid samples %s)" % [n_in[b] for b in items])
         with eng.call_lock:
-            return eng.format_audio(wav, n_in, items, up, down, encoding, loudness, sr, true_peak)
+            return eng.output.format(wav, n_in, items, fmt, sr)

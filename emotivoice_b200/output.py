@@ -1,0 +1,127 @@
+"""The output chain of one engine: loudness measurement (ev_loudness), true-peak limiting (ev_limit), resampling and encoding
+(ev_format_audio) and FLAC (ev_flac_encode) of a forward's outputs, in that order, with the filter banks and coefficients those
+stages read.  ``JETSGenerator.format_audio`` / ``measure_loudness`` validate their arguments and call it under the engine's lock.
+"""
+import numpy as np
+import torch
+
+from . import _abi, audio
+
+_DTYPES = {"float32": torch.float32, "pcm16": torch.int16, "mulaw": torch.uint8, "alaw": torch.uint8}
+
+
+class Chain:
+    """The output stages of the engine on ``device``; ``ws(kind, nbytes)`` is the engine's workspace arena."""
+
+    def __init__(self, device, lib, ws):
+        self.device, self.lib, self._ws = device, lib, ws
+        self._banks = {}              # (up, down) -> device polyphase filter bank of ev_format_audio
+        self._kcoef = {}              # sample rate -> K-weighting coefficients of ev_loudness (host float64)
+        self._limit_banks = {}        # (model rate, output rate) -> (device detector bank, hold) of ev_limit
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _meta(self, arrays):
+        """Host int64 arrays -> one device int64 tensor (one pinned copy) and the device address of each array in it.  The
+        tensor must stay referenced until the last launch that reads it has been enqueued."""
+        meta = torch.from_numpy(np.concatenate([np.asarray(a, np.int64) for a in arrays]))
+        meta = meta.pin_memory().to(self.device, non_blocking=True)
+        ptrs, p = [], meta.data_ptr()
+        for a in arrays:
+            ptrs.append(p)
+            p += 8 * len(a)
+        return meta, ptrs
+
+    def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
+        """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
+        kc = self._kcoef.get(sr)
+        if kc is None:
+            kc = self._kcoef[sr] = np.ascontiguousarray(audio.k_weighting(sr))
+        res = torch.empty((3, k), dtype=torch.float32, device=self.device)
+        stride = int(wav.stride(0))
+        ws = self._ws("loudness", self.lib.ev_loudness_workspace_bytes(k, stride, sr))
+        _abi.check(self.lib.ev_loudness(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, kc.ctypes.data, float(target),
+                                        res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(), ws.numel(),
+                                        self._stream()))
+        return res[0], res[1], res[2]
+
+    def _limit(self, wav, n_in_ptr, items_ptr, k, sr, rate, lufs0, lufs1, target, ceiling, out):
+        """ev_limit of the k listed items into ``out`` (k, L) fp32, pre-gain 10^((target - L) / 20) of each given loudness."""
+        det = self._limit_banks.get((sr, rate))
+        if det is None:
+            bank, hold = audio.limit_bank(sr, rate)
+            det = self._limit_banks[(sr, rate)] = (torch.from_numpy(bank).to(self.device), hold)
+        bank, hold = det
+        L = audio.limit_lookahead(sr)
+        stride = int(wav.stride(0))
+        ws = self._ws("limit", self.lib.ev_limit_workspace_bytes(k, stride, L))
+        _abi.check(self.lib.ev_limit(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, None if lufs0 is None else lufs0.data_ptr(),
+                                     None if lufs1 is None else lufs1.data_ptr(), float(-23.0 if target is None else target),
+                                     float(ceiling), bank.data_ptr(), int(bank.shape[0]), int(bank.shape[1]), L, hold,
+                                     audio.limit_release(sr), out.data_ptr(), int(out.stride(0)), ws.data_ptr(), ws.numel(),
+                                     self._stream()))
+
+    def measure(self, wav, n_in, items, sr):
+        """ev_loudness: (B,1,L) fp32 waveform at ``sr`` Hz, host per-item valid samples and the listed items -> device
+        (lufs, peak) float32 (len(items),)."""
+        meta, (p_n, p_items) = self._meta([n_in, items])
+        lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
+        return lufs, pk
+
+    def format(self, wav, n_in, items, fmt, sr):
+        """The listed items of a (B,1,L) fp32 waveform at ``sr`` Hz, host valid samples ``n_in`` (B ints <= L), in the
+        ``audio.OutputFormat`` ``fmt`` -> (packed device tensor, (len(items)+1,) int64 host offsets).
+
+        With ``fmt.true_peak``, ev_limit first writes the limited items to the "limited" workspace, which the later stages read:
+        with ``fmt.loudness`` two passes (L0 of the items, limit x * g1, L1 of that result, limit x * g1 * g2; see
+        ``JETSGenerator.format_audio``), else one pass with no pre-gain.  Otherwise with ``fmt.loudness`` one ev_loudness gives
+        the gain of ev_format_audio.  "flac" encodes the PCM16 result and reads its image offsets back: the only sync."""
+        lib, k = self.lib, len(items)
+        encoding = "pcm16" if fmt.encoding == audio.FLAC else fmt.encoding
+        offs = audio.packed_offsets(n_in, items, fmt.up, fmt.down)
+        packed = torch.empty((int(offs[-1]),), dtype=_DTYPES[encoding], device=self.device)
+        if packed.numel() == 0:                  # every listed output is empty (never for "flac"): nothing to launch
+            return packed, offs
+        arrays = [n_in, items, offs]
+        if fmt.true_peak is not None:
+            arrays.append([int(n_in[b]) for b in items])                 # the limited items' lengths, in listed order
+        meta, ptrs = self._meta(arrays)
+        p_n, p_items, p_off = ptrs[:3]
+        src, src_n, src_items, gain = wav, p_n, p_items, None
+        if fmt.true_peak is not None:
+            p_nl = ptrs[3]
+            stride = int(wav.stride(0))
+            lim = self._ws("limited", 4 * k * stride)[:4 * k * stride].view(torch.float32).view(k, stride)
+            lufs0 = lufs1 = None
+            if fmt.loudness is not None:
+                lufs0 = self._loudness(wav, p_n, p_items, k, sr, fmt.loudness)[0]
+                self._limit(wav, p_n, p_items, k, sr, fmt.rate, lufs0, None, fmt.loudness, fmt.true_peak, lim)
+                lufs1 = self._loudness(lim, p_nl, None, k, sr, fmt.loudness)[0]
+            self._limit(wav, p_n, p_items, k, sr, fmt.rate, lufs0, lufs1, fmt.loudness, fmt.true_peak, lim)
+            src, src_n, src_items = lim, p_nl, None
+        elif fmt.loudness is not None:
+            gain = self._loudness(wav, p_n, p_items, k, sr, fmt.loudness)[2]
+        bank = None
+        if (fmt.up, fmt.down) != (1, 1):
+            bank = self._banks.get((fmt.up, fmt.down))
+            if bank is None:
+                bank = self._banks[(fmt.up, fmt.down)] = torch.from_numpy(audio.polyphase_bank(fmt.up, fmt.down)).to(self.device)
+        _abi.check(lib.ev_format_audio(src.data_ptr(), int(src.stride(0)), src_n, src_items, k, p_off,
+                                       None if bank is None else bank.data_ptr(), fmt.up, fmt.down,
+                                       0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),
+                                       None if gain is None else gain.data_ptr(), self._stream()))
+        if fmt.encoding != audio.FLAC:
+            return packed, offs
+        counts = np.ascontiguousarray(np.diff(offs), dtype=np.int64)
+        bound = sum(int(lib.ev_flac_bound_bytes(int(n))) for n in counts)
+        out = torch.empty((bound,), dtype=torch.uint8, device=self.device)
+        out_off = torch.empty((k + 1,), dtype=torch.int64, device=self.device)
+        ws = self._ws("flac", lib.ev_flac_workspace_bytes(k, int(counts.max())))
+        _abi.check(lib.ev_flac_encode(packed.data_ptr(), p_off, k, counts.ctypes.data, int(fmt.rate), out.data_ptr(), bound,
+                                      out_off.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
+        host = torch.empty((k + 1,), dtype=torch.int64, pin_memory=True)
+        host.copy_(out_off, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        flac_offs = host.numpy().copy()
+        return out[:int(flac_offs[-1])], flac_offs

@@ -241,23 +241,19 @@ enum { EV_AUDIO_FLOAT32 = 0, EV_AUDIO_PCM16 = 1, EV_AUDIO_MULAW = 2, EV_AUDIO_AL
  *   10 * max(up, down), with x zero outside [0, n_in[b]): scipy.signal.resample_poly(x[:n_in[b]], up, down) to fp32 accuracy,
  *   one fp32 chain per output in tap order, so an item's output does not depend on the other items of the call.
  *   encoding: EV_AUDIO_*; out holds 4, 2, 1 or 1 byte(s) per sample.
+ *   gain: NULL, or (n_items) f32 per-item gains: listed item k's outputs are then encoded from fp32(y * gain[k]), y the
+ *   resampled sample (at up == down == 1 the sample itself).  gain may be written by the launch just before (ev_loudness).
  *   All arrays are device memory read in stream order (the kernel reads them after the work before it on the stream has
  *   completed); out_off and n_in must describe disjoint output ranges.  No allocation, no sync. */
 EV_API int ev_format_audio(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
                            const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
-                           void* stream);
-/* ev_format_audio with a per-item gain: gain (n_items) f32 device array, or NULL.  Listed item k's outputs are encoded from
- * fp32(y * gain[k]), y the resampled sample ev_format_audio computes (at up == down == 1 the sample itself).  With gain == NULL
- * this is ev_format_audio, bit for bit.  gain is read in stream order, so it may be written by the launch just before
- * (ev_loudness). */
-EV_API int ev_format_audio_gain(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
-                                const int64_t* out_off, const float* bank, int up, int down, int taps_per_phase, int encoding, void* out,
-                                const float* gain, void* stream);
+                           const float* gain, void* stream);
 
 /* Integrated loudness (ITU-R BS.1770-4, one channel) of listed waveform items and the gain that brings each to a target: the
- * server-side loudness normalisation of responses (EBU R128 at -23 LUFS, podcasts at -16), before ev_format_audio_gain encodes
- * them.  Arguments as ev_format_audio: wav items item_stride floats apart, n_in (B) i64 valid samples (at most item_stride;
- * samples at or past n_in[b] are never read), items (n_items) i64 or NULL for 0 .. n_items - 1, 1 <= n_items <= 65535.
+ * server-side loudness normalisation of responses (EBU R128 at -23 LUFS, podcasts at -16), before ev_format_audio applies
+ * the gain and encodes them.  Arguments as ev_format_audio: wav items item_stride floats apart, n_in (B) i64 valid samples (at
+ * most item_stride; samples at or past n_in[b] are never read), items (n_items) i64 or NULL for 0 .. n_items - 1,
+ * 1 <= n_items <= 65535.
  *   sample_rate: the items' rate, a multiple of 10 in [4000, 192000] (100 ms sub-blocks of sample_rate / 10 samples).
  *   kcoef: HOST array of 10 doubles, the K-weighting cascade (b0, b1, b2, a1, a2) of the high shelf, then of the high pass, with
  *   a0 = 1 (emotivoice_b200.audio.k_weighting(sample_rate)).  The cascade runs in fp32 (direct form I) on each 100 ms

@@ -37,6 +37,16 @@ def test_source_rate_is_the_default_and_bad_requests_raise():
             audio.plan(24000, enc, SR)
 
 
+def test_output_format_checks_rate_then_loudness_then_ceiling():
+    assert audio.output_format(48000, "flac", -16, np.float32(-1.0), SR) == audio.OutputFormat(48000, 3, 1, "flac", -16.0, -1.0)
+    assert audio.output_format(None, "pcm16", None, None, SR) == (SR, 1, 1, "pcm16", None, None)
+    assert hash(audio.output_format(8000, "mulaw", -23, None, SR)) == hash(audio.output_format(8000.0, "mulaw", -23.0, None, SR))
+    for args, what in (((3999, "pcm16", 1.0, 1.0), "sample_rate"), ((None, "mp3", 1.0, 1.0), "encoding"),
+                       ((None, "pcm16", 1.0, 1.0), "loudness"), ((None, "pcm16", -23, 1.0), "true_peak")):
+        with pytest.raises(ValueError, match=what):
+            audio.output_format(*args, SR)
+
+
 def _scipy_filter(up, down):
     """resample_poly's own filter (float64, multiplied by up), read back from resample_poly: unit impulses spaced so that no
     output receives two of them, placed so that together they meet every filter tap.  Each such output is one tap times 1.0

@@ -6,6 +6,7 @@ import pytest
 import torch
 from scipy.signal import firwin, resample_poly
 
+from audio_cases import out_dict
 from conftest import GOLDEN, load_golden
 from emotivoice_b200 import _abi, audio, synth
 from emotivoice_b200 import frontdoor as fd
@@ -117,10 +118,6 @@ def _synthetic(lens, seed=0, poison=True):
     return w
 
 
-def _out(w, lens, dev):
-    return {"wav_predictions": torch.from_numpy(w).to(dev), "mel_lengths_host": torch.tensor(lens, dtype=torch.int32)}
-
-
 @pytest.mark.parametrize("rate", [8000, 11025, 24000, 44100, 48000, 192000])
 def test_item_edges_poisoned_padding_and_batch_independence(model, dev, rate):
     _, up, down = audio.plan(rate, "float32", 16000)
@@ -128,12 +125,12 @@ def test_item_edges_poisoned_padding_and_batch_independence(model, dev, rate):
     for t in (256, 512):                  # outputs that end just before, on and just after a tile edge (256 outputs per tile)
         lens += [(t * down) // up + d for d in (-1, 0, 1, 2)]
     w = _synthetic(lens, seed=rate)
-    out = _out(w, lens, dev)
+    out = out_dict(w, lens, dev)
     for enc in ("float32", "pcm16", "mulaw"):
         allv = fd.fetch_audio(model, out, rate, enc, hop=1)
         assert [len(a) for a in allv] == [audio.resampled_length(n, up, down) for n in lens]
         for b, n in enumerate(lens):
-            alone = fd.fetch_audio(model, _out(np.ascontiguousarray(w[b:b + 1, :, :n + 5]), [n], dev), rate, enc, hop=1)[0]
+            alone = fd.fetch_audio(model, out_dict(np.ascontiguousarray(w[b:b + 1, :, :n + 5]), [n], dev), rate, enc, hop=1)[0]
             assert np.array_equal(alone, allv[b]), (enc, b, n)
             if enc == "float32":
                 assert not np.isnan(allv[b]).any()
@@ -185,6 +182,21 @@ def test_microbatcher_mixed_formats_equal_fetch_audio_alone(model, dev):
             assert w.dtype == want.dtype and np.array_equal(w, want), (r, e)
 
 
+def test_launches_per_chain_shape(model, dev):
+    """format_audio enqueues its stages and nothing else: ev_format_audio 1, ev_loudness 2, ev_limit 3 per pass, ev_flac_encode
+    4; no launch when every listed output is empty."""
+    _, out = _engine_out(model, dev)
+    empty = out_dict(np.zeros((2, 1, 64), np.float32), [0, 0], dev)
+    for (loudness, true_peak), n in {(None, None): 1, (-16.0, None): 3, (None, -1.0): 4, (-16.0, -1.0): 11}.items():
+        for enc, extra in (("pcm16", 0), ("flac", 4)):
+            n0 = _abi.launch_count()
+            model.format_audio(out, 24000, enc, loudness=loudness, true_peak=true_peak)
+            assert _abi.launch_count() - n0 == n + extra, (loudness, true_peak, enc)
+        n0 = _abi.launch_count()
+        packed, offs = model.format_audio(empty, 24000, "pcm16", hop=1, loudness=loudness, true_peak=true_peak)
+        assert _abi.launch_count() == n0 and packed.numel() == 0 and offs.tolist() == [0, 0, 0], (loudness, true_peak)
+
+
 def test_invalid_arguments_raise_before_anything_is_enqueued(model, dev, lib):
     _, out = _engine_out(model, dev)
     w = out["wav_predictions"]
@@ -209,7 +221,7 @@ def test_invalid_arguments_raise_before_anything_is_enqueued(model, dev, lib):
     for bk, up, down, taps, enc in bad:
         with pytest.raises(_abi.EvError):
             _abi.check(lib.ev_format_audio(w.data_ptr(), w.stride(0), n_in.data_ptr(), None, 3, off.data_ptr(), bk, up, down, taps,
-                                           enc, dst.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+                                           enc, dst.data_ptr(), None, torch.cuda.current_stream(dev).cuda_stream))
     assert _abi.launch_count() == n0
     got = fd.fetch_audio(model, out, 48000, "pcm16")
     assert [len(a) for a in got] == [3 * int(n) * 256 for n in out["mel_lengths_host"].tolist()]

@@ -181,8 +181,8 @@ def test_microbatcher_groups_flac_with_other_formats(monkeypatch):
 
     calls = []
 
-    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None):
-        calls.append((sample_rate, encoding, loudness, tuple(items)))
+    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
+        calls.append((sample_rate, encoding, loudness, true_peak, tuple(items)))
         return [np.array([len(calls)], audio.NUMPY_DTYPES[encoding]) for _ in items]
 
     monkeypatch.setattr(fd, "fetch_audio", fake_fetch)
@@ -193,7 +193,7 @@ def test_microbatcher_groups_flac_with_other_formats(monkeypatch):
         got = [f.result(timeout=30) for f in futs]
         assert mb.batches_run == 1
     assert forwards == [4]
-    assert sorted(calls, key=str) == sorted([(16000, "flac", None, (0, 3)), (16000, "pcm16", None, (1,)),
-                                             (8000, "mulaw", None, (2,))], key=str)
+    assert sorted(calls, key=str) == sorted([(16000, "flac", None, None, (0, 3)), (16000, "pcm16", None, None, (1,)),
+                                             (8000, "mulaw", None, None, (2,))], key=str)
     assert got[0].dtype == np.uint8 and got[0][0] == got[3][0]
-    assert fd.MicroBatcher._output_format(mb, 48000, "flac", -16) == (48000, "flac", -16.0)
+    assert fd.MicroBatcher._output_format(mb, 48000, "flac", -16) == audio.OutputFormat(48000, 3, 1, "flac", -16.0, None)

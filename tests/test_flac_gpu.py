@@ -12,31 +12,15 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT, load_golden
+from audio_cases import SR, engine_outputs
+from conftest import ROOT
 from emotivoice_b200 import _abi, synth
 from emotivoice_b200 import frontdoor as fd
 from oracle import flac_oracle as F
 from test_flac import signals
 
 pytestmark = pytest.mark.gpu
-SR = 16000
-KEYS = ("inputs_ling", "input_lengths", "inputs_speaker", "inputs_style_embedding", "inputs_content_embedding")
 RATES = [8000, 16000, 24000, 44100, 48000, 127625]
-_cache = {}
-
-
-def _engine_outputs(model, dev):
-    """name -> the forward's output dict, for b1_t100, b3_padded and the joined paragraph."""
-    if not _cache:
-        for name in ("b1_t100", "b3_padded"):
-            g = load_golden(name)
-            _cache[name] = model(**{k: g[k].to(dev) for k in KEYS})
-        g = load_golden("joined_paragraph")
-        ends = np.cumsum(g["seg_lens"].numpy())
-        segs = [g["ids"].numpy()[e - n:e] for e, n in zip(ends, g["seg_lens"].tolist())]
-        batch = fd.collate([(s, int(spk), st.numpy(), ct.numpy()) for s, spk, st, ct in zip(segs, g["speakers"], g["style"], g["content"])])
-        _cache["paragraph"] = model(**{k: batch[k].to(dev) for k in KEYS}, join=[0] * len(segs))
-    return _cache
 
 
 def abi_flac(lib, dev, items, rate):
@@ -67,7 +51,7 @@ def _check(img, pcm, rate, what):
 @pytest.mark.parametrize("loudness", [None, -16.0])
 @pytest.mark.parametrize("rate", RATES)
 def test_engine_outputs_equal_the_oracle(model, dev, rate, loudness):
-    for name, out in _engine_outputs(model, dev).items():
+    for name, (out, _) in engine_outputs(model, dev).items():
         imgs = fd.fetch_audio(model, out, rate, "flac", loudness=loudness)
         pcms = fd.fetch_audio(model, out, rate, "pcm16", loudness=loudness)
         assert len(imgs) == len(pcms)
@@ -145,7 +129,7 @@ def test_same_bytes_with_pdl_off(tmp_path):
 
 
 def test_invalid_arguments(model, lib, dev):
-    out = _engine_outputs(model, dev)["b3_padded"]
+    out, _ = engine_outputs(model, dev)["b3_padded"]
     torch.cuda.synchronize()
     n0 = _abi.launch_count()
     for kw in (dict(sample_rate=3999), dict(sample_rate=44100.5), dict(items=[3]), dict(loudness=1.0), dict(encoding="FLAC")):
@@ -205,7 +189,7 @@ def test_third_party_decoder_when_installed(model, dev, tmp_path):
     tool = shutil.which("flac") or shutil.which("ffmpeg")
     if tool is None:
         pytest.skip("no flac or ffmpeg binary on this machine")
-    out = _engine_outputs(model, dev)["b1_t100"]
+    out, _ = engine_outputs(model, dev)["b1_t100"]
     img = fd.fetch_audio(model, out, 24000, "flac")[0]
     pcm = fd.fetch_audio(model, out, 24000, "pcm16")[0]
     src, dst = tmp_path / "a.flac", tmp_path / "a.raw"

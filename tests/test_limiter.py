@@ -144,8 +144,8 @@ def test_microbatcher_formats_once_per_key_with_ceilings(monkeypatch):
 
     calls = []
 
-    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, **kw):
-        calls.append((sample_rate, encoding, loudness, kw.get("true_peak", "absent"), tuple(items)))
+    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
+        calls.append((sample_rate, encoding, loudness, true_peak, tuple(items)))
         return [np.array([len(calls)]) for _ in items]
 
     monkeypatch.setattr(fd, "fetch_audio", fake_fetch)
@@ -161,9 +161,9 @@ def test_microbatcher_formats_once_per_key_with_ceilings(monkeypatch):
         futs = [mb.submit(np.array([1, 2, 3]), 0, z, z, **kw) for kw in reqs]
         got = [f.result(timeout=30) for f in futs]
         assert mb.batches_run == 1
-    assert sorted(calls, key=str) == sorted([(16000, "pcm16", -16.0, -1.0, (0, 1)), (16000, "pcm16", -16.0, "absent", (2,)),
+    assert sorted(calls, key=str) == sorted([(16000, "pcm16", -16.0, -1.0, (0, 1)), (16000, "pcm16", -16.0, None, (2,)),
                                              (16000, "pcm16", None, -2.0, (3,)), (8000, "mulaw", -16.0, -3.0, (4,))], key=str)
     assert got[0][0] == got[1][0] and isinstance(got[5], torch.Tensor)
-    assert fd.MicroBatcher._output_format(mb, None, None, -23, -1) == (16000, "pcm16", -23.0, -1.0)
-    assert fd.MicroBatcher._output_format(mb, None, None, None, -1) == (16000, "pcm16", None, -1.0)
-    assert fd.MicroBatcher._output_format(mb, None, None, -23, None) == (16000, "pcm16", -23.0)
+    assert fd.MicroBatcher._output_format(mb, None, None, -23, -1) == audio.OutputFormat(16000, 1, 1, "pcm16", -23.0, -1.0)
+    assert fd.MicroBatcher._output_format(mb, None, None, None, -1) == audio.OutputFormat(16000, 1, 1, "pcm16", None, -1.0)
+    assert fd.MicroBatcher._output_format(mb, None, None, -23, None) == audio.OutputFormat(16000, 1, 1, "pcm16", -23.0, None)

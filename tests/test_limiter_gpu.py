@@ -27,15 +27,14 @@ import numpy as np
 import pytest
 import torch
 
+from audio_cases import SR, abi_limit, abi_loudness, engine_outputs, out_dict, padded_batch, ten_minutes
 from conftest import ROOT
 from emotivoice_b200 import _abi, audio, synth
 from emotivoice_b200 import frontdoor as fd
 from oracle import flac_oracle, limiter_oracle as O, loudness_oracle
 from test_limiter import sine_45, voiced
-from test_loudness_gpu import _batch, _engine_outputs, _out, abi_loudness, ten_minutes
 
 pytestmark = pytest.mark.gpu
-SR = 16000
 RATES = {16000: (1, 1), 22050: (441, 320), 24000: (3, 2), 44100: (441, 160), 48000: (3, 1), 8000: (1, 2), 11025: (441, 640)}
 MARGIN = 0.05
 RESAMPLED_EDGE, EDGE_S = 0.2, 0.002
@@ -51,27 +50,6 @@ def synthetic_items():
            "voiced12": voiced(12.0), "voiced16": voiced(16.0, seed=1), "voiced20": voiced(20.0, seed=2),
            "silence": np.zeros(2 * SR, np.float32), "short": voiced(16.0, seed=3)[:5000]}
     return sig
-
-
-def abi_limit(lib, dev, w, lens, rate, ceiling, lufs0=None, lufs1=None, target=-23.0, items=None):
-    """ev_limit straight through the ABI -> host (k, stride) float32."""
-    wt = torch.from_numpy(w).to(dev) if isinstance(w, np.ndarray) else w
-    n_in = torch.tensor(lens, dtype=torch.int64, device=dev)
-    k = len(lens) if items is None else len(items)
-    it = None if items is None else torch.tensor(items, dtype=torch.int64, device=dev)
-    bank, hold = audio.limit_bank(SR, rate)
-    bank = torch.from_numpy(bank).to(dev)
-    L = audio.limit_lookahead(SR)
-    out = torch.full((k, wt.stride(0)), np.nan, dtype=torch.float32, device=dev)
-    nb = lib.ev_limit_workspace_bytes(k, wt.stride(0), L)
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-    l0 = None if lufs0 is None else torch.from_numpy(np.asarray(lufs0, np.float32)).to(dev)
-    l1 = None if lufs1 is None else torch.from_numpy(np.asarray(lufs1, np.float32)).to(dev)
-    _abi.check(lib.ev_limit(wt.data_ptr(), wt.stride(0), n_in.data_ptr(), None if it is None else it.data_ptr(), k, SR,
-                            None if l0 is None else l0.data_ptr(), None if l1 is None else l1.data_ptr(), target, ceiling,
-                            bank.data_ptr(), bank.shape[0], bank.shape[1], L, hold, audio.limit_release(SR), out.data_ptr(),
-                            out.stride(0), ws.data_ptr(), nb, torch.cuda.current_stream(dev).cuda_stream))
-    return out.cpu().numpy()
 
 
 def _compare(y, x, g, yo, Go, name):
@@ -98,7 +76,7 @@ def _two_pass_abi(lib, dev, w, lens, rate, ceiling, target):
 @pytest.mark.parametrize("rate", [16000, 8000])
 def test_synthetic_items_match_the_oracle(model, lib, dev, rate):
     sig = synthetic_items()
-    w, lens = _batch(list(sig.values()))
+    w, lens = padded_batch(list(sig.values()))
     for C, target in ((-1.0, None), (-1.0, -16.0), (-3.0, -23.0)):
         if target is None:
             y = abi_limit(lib, dev, w, lens, rate, C)
@@ -114,13 +92,13 @@ def test_synthetic_items_match_the_oracle(model, lib, dev, rate):
             yo, Go, _ = O.limit(x, SR, rate, C, g2)
             _compare(y2[b, :lens[b]], x, g2, yo, Go, (name, rate, C, target, 2))
             if rate == SR:                                 # format_audio at the model's rate is the ABI chain, bit for bit
-                want = fd.fetch_audio(model, _out(w, lens, dev), None, "float32", items=[b], hop=1, loudness=target, true_peak=C)[0]
+                want = fd.fetch_audio(model, out_dict(w, lens, dev), None, "float32", items=[b], hop=1, loudness=target, true_peak=C)[0]
                 assert np.array_equal(want.view(np.int32), y2[b, :lens[b]].view(np.int32)), name
 
 
 def test_ten_minutes_matches_the_oracle(lib, dev):
     x = ten_minutes() * np.float32(8.0)            # loud enough that limiting runs all along the item
-    w, lens = _batch([x])
+    w, lens = padded_batch([x])
     y = abi_limit(lib, dev, w, lens, SR, -1.0)
     yo, Go, _ = O.limit(x, SR, SR, -1.0, 1.0, fast=True)
     _compare(y[0, :lens[0]], x, 1.0, yo, Go, "ten_minutes")
@@ -129,7 +107,7 @@ def test_ten_minutes_matches_the_oracle(lib, dev):
 
 def test_engine_outputs_match_the_oracle(model, lib, dev):
     for name in ("b1_t100", "b3_padded"):
-        out, xs = _engine_outputs(model, dev)[name]
+        out, xs = engine_outputs(model, dev)[name]
         w = out["wav_predictions"].cpu().numpy()
         lens = [len(x) for x in xs]
         y1, y2, L0, L1 = _two_pass_abi(lib, dev, w, lens, SR, -1.0, -14.0)
@@ -153,9 +131,9 @@ def _excess(y, rate, C):
 
 def test_true_peak_bound_at_every_rate(model, dev):
     sig = synthetic_items()
-    out_e, xs = _engine_outputs(model, dev)["b3_padded"]
-    w, lens = _batch(list(sig.values()))
-    out = _out(w, lens, dev)
+    out_e, xs = engine_outputs(model, dev)["b3_padded"]
+    w, lens = padded_batch(list(sig.values()))
+    out = out_dict(w, lens, dev)
     worst, bad = {}, []
     for C in (-1.0, -3.0):
         for rate in RATES:
@@ -193,8 +171,8 @@ def test_true_peak_bound_at_every_rate(model, dev):
 def test_loudness_targets_are_reached(model, dev, plr):
     import torchaudio.functional as F
     x = voiced(plr, seconds=6.0, seed=int(plr))
-    w, lens = _batch([x])
-    out = _out(w, lens, dev)
+    w, lens = padded_batch([x])
+    out = out_dict(w, lens, dev)
     for target in (-23.0, -16.0, -14.0, -10.0):
         y = fd.fetch_audio(model, out, None, "float32", hop=1, loudness=target, true_peak=-1.0)[0]
         Ly = loudness_oracle.integrated_loudness(y.astype(np.float64), SR)
@@ -212,11 +190,11 @@ def test_loudness_targets_are_reached(model, dev, plr):
 
 def test_neutral_case_is_the_uncapped_gain(model, lib, dev):
     x = voiced(16.0, seed=5) * np.float32(0.05)
-    w, lens = _batch([x])
+    w, lens = padded_batch([x])
     L0 = abi_loudness(lib, dev, w, lens)[0][0]
     g = O.pregain(-30.0, L0)
     assert 20 * np.log10(g * O.detect(x, SR, SR).max()) < -1.5          # nothing to limit
-    y = fd.fetch_audio(model, _out(w, lens, dev), None, "float32", hop=1, loudness=-30.0, true_peak=-1.0)[0]
+    y = fd.fetch_audio(model, out_dict(w, lens, dev), None, "float32", hop=1, loudness=-30.0, true_peak=-1.0)[0]
     y2 = abi_limit(lib, dev, w, lens, SR, -1.0, [L0], [L0], -30.0)[0]
     sel = np.abs(x) > 1e-4
     ratio = y[sel].astype(np.float64) / x[sel]
@@ -226,21 +204,21 @@ def test_neutral_case_is_the_uncapped_gain(model, lib, dev):
 
 def test_batch_and_order_independence(model, lib, dev):
     sig = list(synthetic_items().values())
-    w, lens = _batch(sig)
+    w, lens = padded_batch(sig)
     order = list(range(len(sig)))[::-1]
     full = _two_pass_abi(lib, dev, w, lens, SR, -1.0, -16.0)[1]
     rev = abi_limit(lib, dev, w, lens, SR, -2.0, items=order)
     fwd = abi_limit(lib, dev, w, lens, SR, -2.0)
-    out = _out(w, lens, dev)
+    out = out_dict(w, lens, dev)
     enc_all = {fmt: fd.fetch_audio(model, out, *fmt, hop=1, loudness=-16.0, true_peak=-1.0) for fmt in ((8000, "mulaw"), (None, "float32"),
                                                                                                        (24000, "flac"))}
     for b, x in enumerate(sig):
-        wb, lb = _batch([x])
+        wb, lb = padded_batch([x])
         alone = _two_pass_abi(lib, dev, wb, lb, SR, -1.0, -16.0)[1]
         assert np.array_equal(alone[0, :lb[0]].view(np.int32), full[b, :lens[b]].view(np.int32)), b
         assert np.array_equal(rev[order.index(b), :lens[b]].view(np.int32), fwd[b, :lens[b]].view(np.int32)), b
         for fmt, allv in enc_all.items():
-            one = fd.fetch_audio(model, _out(wb, lb, dev), *fmt, hop=1, loudness=-16.0, true_peak=-1.0)[0]
+            one = fd.fetch_audio(model, out_dict(wb, lb, dev), *fmt, hop=1, loudness=-16.0, true_peak=-1.0)[0]
             assert np.array_equal(one.view(np.uint8), allv[b].view(np.uint8)), (fmt, b)
 
 
@@ -251,7 +229,7 @@ def pdl_dump(path):
     lib = _abi.load()
     dev = torch.device("cuda:0")
     sig = synthetic_items()
-    w, lens = _batch([sig[k] for k in ("sine_45", "voiced16", "short", "silence")])
+    w, lens = padded_batch([sig[k] for k in ("sine_45", "voiced16", "short", "silence")])
     y1, y2, _, _ = _two_pass_abi(lib, dev, w, lens, 8000, -1.0, -16.0)
     np.savez(path, y1=np.nan_to_num(y1), y2=np.nan_to_num(y2))
 
@@ -289,7 +267,7 @@ def test_microbatcher_mixed_ceilings_equal_fetch_audio_alone(model, dev):
 
 
 def test_invalid_arguments_raise_before_anything_is_enqueued(model, lib, dev):
-    out, xs = _engine_outputs(model, dev)["b3_padded"]
+    out, xs = engine_outputs(model, dev)["b3_padded"]
     torch.cuda.synchronize()
     n0 = _abi.launch_count()
     for bad in (float("nan"), float("inf"), 1.0, -21.0, True, "-1"):

@@ -142,8 +142,8 @@ def test_microbatcher_measures_and_formats_once_per_key(monkeypatch):
 
     calls = []
 
-    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None):
-        calls.append((sample_rate, encoding, loudness, tuple(items)))
+    def fake_fetch(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
+        calls.append((sample_rate, encoding, loudness, true_peak, tuple(items)))
         return [np.array([sample_rate or 0, len(calls)]) for _ in items]
 
     monkeypatch.setattr(fd, "fetch_audio", fake_fetch)
@@ -159,10 +159,10 @@ def test_microbatcher_measures_and_formats_once_per_key(monkeypatch):
         futs = [mb.submit(np.array([1, 2, 3]), 0, z, z, **kw) for kw in reqs]
         got = [f.result(timeout=30) for f in futs]
         assert mb.batches_run == 1
-    assert sorted(calls, key=str) == sorted([(16000, "pcm16", -23.0, (0, 2)), (8000, "mulaw", -16.0, (1,)),
-                                             (24000, "pcm16", -23.0, (3,))], key=str)
+    assert sorted(calls, key=str) == sorted([(16000, "pcm16", -23.0, None, (0, 2)), (8000, "mulaw", -16.0, None, (1,)),
+                                             (24000, "pcm16", -23.0, None, (3,))], key=str)
     assert isinstance(got[4], torch.Tensor)
     assert got[0][1] == got[2][1]                   # one call served both -23 LUFS requests at 16 kHz PCM16
-    assert fd.MicroBatcher._output_format(mb, None, None, -23) == (16000, "pcm16", -23.0)
+    assert fd.MicroBatcher._output_format(mb, None, None, -23) == audio.OutputFormat(16000, 1, 1, "pcm16", -23.0, None)
     assert fd.MicroBatcher._output_format(mb, None, None, None) is None
-    assert fd.MicroBatcher._output_format(mb, None, "alaw", None) == (16000, "alaw", None)
+    assert fd.MicroBatcher._output_format(mb, None, "alaw", None) == audio.OutputFormat(16000, 1, 1, "alaw", None, None)

@@ -1,7 +1,8 @@
 """Loudness normalisation on the GPU (``JETSGenerator.measure_loudness``, ``format_audio(loudness=...)``, ev_loudness and
-ev_format_audio_gain): integrated loudness and peak against the fp64 BS.1770-4 oracle on the engine's outputs and on synthetic
-items with NaN past their lengths, batch independence, the gain identity of every encoding, the normalised result, no change
-without a target (and with EV_PDL=0), mixed targets in one MicroBatcher forward, and argument errors."""
+the gain of ev_format_audio): integrated loudness and peak against the fp64 BS.1770-4 oracle on the engine's outputs and on
+synthetic items with NaN past their lengths, batch independence, the gain identity of every encoding, the normalised result, no
+change without a target or under unit gains (and with EV_PDL=0), mixed targets in one MicroBatcher forward, and argument
+errors."""
 import os
 import subprocess
 import sys
@@ -10,17 +11,15 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, ROOT, load_golden
+from audio_cases import SR, abi_loudness, engine_outputs, out_dict, padded_batch, ten_minutes
+from conftest import GOLDEN, ROOT
 from emotivoice_b200 import _abi, audio, synth
 from emotivoice_b200 import frontdoor as fd
 from oracle import loudness_oracle as O
 
 pytestmark = pytest.mark.gpu
-SR = 16000
-KEYS = ("inputs_ling", "input_lengths", "inputs_speaker", "inputs_style_embedding", "inputs_content_embedding")
 DL = 1e-3                   # LU
 CEILING = 10.0 ** (-1.0 / 20.0)
-_cache = {}
 
 
 def _sine(dbfs, seconds, f):
@@ -51,14 +50,6 @@ def synthetic_items():
     return {k: v.astype(np.float32) for k, v in sig.items()}
 
 
-def ten_minutes():
-    """A 10-minute item: noise whose level moves slowly over 8 dB."""
-    n = 600 * SR
-    t = np.arange(n) / SR
-    env = 10.0 ** ((-30.0 + 4.0 * np.sin(2 * np.pi * t / 47.0)) / 20.0)
-    return np.clip(env * np.random.default_rng(8).standard_normal(n), -1.0, 1.0).astype(np.float32)
-
-
 def gate_margin(x):
     """Smallest distance (LU) of a block's loudness to the absolute or relative gate (inf without blocks)."""
     _, l, rel = O.gating(np.asarray(x, np.float64), SR)
@@ -75,36 +66,6 @@ def _oracle(x, target):
     return L, pk, O.gain(L, pk, target)
 
 
-def _batch(signals, poison=True):
-    """(B, 1, L) float32 device tensor, NaN past each item's length, and the lengths."""
-    lens = [len(s) for s in signals]
-    w = np.full((len(signals), 1, max(lens) + 37), np.nan if poison else 0.0, dtype=np.float32)
-    for b, s in enumerate(signals):
-        w[b, 0, :len(s)] = s
-    return w, lens
-
-
-def abi_loudness(lib, dev, w, lens, items=None, target=-23.0):
-    """ev_loudness straight through the ABI -> host (lufs, peak, gain) float32 arrays."""
-    wt = torch.from_numpy(w).to(dev)
-    n_in = torch.tensor(lens, dtype=torch.int64, device=dev)
-    k = len(lens) if items is None else len(items)
-    it = None if items is None else torch.tensor(items, dtype=torch.int64, device=dev)
-    res = torch.empty((3, k), dtype=torch.float32, device=dev)
-    kc = audio.k_weighting(SR)
-    nb = lib.ev_loudness_workspace_bytes(k, wt.stride(0), SR)
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-    _abi.check(lib.ev_loudness(wt.data_ptr(), wt.stride(0), n_in.data_ptr(), None if it is None else it.data_ptr(), k, SR,
-                               kc.ctypes.data, target, res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(), nb,
-                               torch.cuda.current_stream(dev).cuda_stream))
-    r = res.cpu().numpy()
-    return r[0], r[1], r[2]
-
-
-def _out(w, lens, dev):
-    return {"wav_predictions": torch.from_numpy(w).to(dev), "mel_lengths_host": torch.tensor(lens, dtype=torch.int32)}
-
-
 def _check(L, pk, x, name):
     Lo, po, _ = _oracle(x, -23.0)
     assert pk == np.float32(po), (name, pk, po)
@@ -115,66 +76,48 @@ def _check(L, pk, x, name):
         assert L == -np.inf, (name, L)
 
 
-def _engine_outputs(model, dev):
-    """name -> (out, waveforms as host arrays) for b1_t100, b3_padded and the joined paragraph."""
-    if not _cache:
-        for name in ("b1_t100", "b3_padded"):
-            g = load_golden(name)
-            out = model(**{k: g[k].to(dev) for k in KEYS})
-            wav = out["wav_predictions"].cpu().numpy()
-            _cache[name] = (out, [wav[b, 0, :int(n) * 256] for b, n in enumerate(out["mel_lengths_host"].tolist())])
-        g = load_golden("joined_paragraph")
-        ends = np.cumsum(g["seg_lens"].numpy())
-        segs = [g["ids"].numpy()[e - n:e] for e, n in zip(ends, g["seg_lens"].tolist())]
-        batch = fd.collate([(s, int(spk), st.numpy(), ct.numpy()) for s, spk, st, ct in zip(segs, g["speakers"], g["style"], g["content"])])
-        out = model(**{k: batch[k].to(dev) for k in KEYS}, join=[0] * len(segs))
-        wav = out["wav_predictions"].cpu().numpy()
-        _cache["paragraph"] = (out, [wav[0, 0, :int(out["joined_lengths_host"][0]) * 256]])
-    return _cache
-
-
 def test_engine_outputs_match_the_oracle(model, dev, lib):
-    for name, (out, xs) in _engine_outputs(model, dev).items():
+    for name, (out, xs) in engine_outputs(model, dev).items():
         lufs, pk = model.measure_loudness(out)
         assert lufs.dtype == torch.float32 and lufs.device == dev and lufs.shape == (len(xs),)
         lufs, pk = lufs.cpu().numpy(), pk.cpu().numpy()
         for b, x in enumerate(xs):
             _check(lufs[b], pk[b], x, (name, b))
         print(name, "lufs", lufs.tolist(), "peak", pk.tolist())
-    lufs, pk = model.measure_loudness(_engine_outputs(model, dev)["b3_padded"][0], items=[2, 0])
-    whole = model.measure_loudness(_engine_outputs(model, dev)["b3_padded"][0])
+    lufs, pk = model.measure_loudness(engine_outputs(model, dev)["b3_padded"][0], items=[2, 0])
+    whole = model.measure_loudness(engine_outputs(model, dev)["b3_padded"][0])
     assert torch.equal(lufs, whole[0][[2, 0]]) and torch.equal(pk, whole[1][[2, 0]])
 
 
 def test_synthetic_items_match_the_oracle(lib, dev):
     sig = synthetic_items()
-    w, lens = _batch(list(sig.values()))
+    w, lens = padded_batch(list(sig.values()))
     lufs, pk, _ = abi_loudness(lib, dev, w, lens)
     for b, (name, x) in enumerate(sig.items()):
         _check(lufs[b], pk[b], x, name)
     assert lufs[list(sig).index("n6399")] == -np.inf and lufs[list(sig).index("silence")] == -np.inf
     assert np.isfinite(lufs[list(sig).index("n6400")])
     x = ten_minutes()
-    w, lens = _batch([x])
+    w, lens = padded_batch([x])
     lufs, pk, _ = abi_loudness(lib, dev, w, lens)
     _check(lufs[0], pk[0], x, "ten_minutes")
 
 
 def test_batch_independence(model, lib, dev):
     sig = list(synthetic_items().values())
-    w, lens = _batch(sig)
+    w, lens = padded_batch(sig)
     full = abi_loudness(lib, dev, w, lens, target=-20.0)
     order = list(range(len(sig)))[::-1]
     rev = abi_loudness(lib, dev, w, lens, items=order, target=-20.0)
-    out = _out(w, lens, dev)
+    out = out_dict(w, lens, dev)
     enc_all = {fmt: fd.fetch_audio(model, out, *fmt, hop=1, loudness=-20.0) for fmt in ((8000, "mulaw"), (None, "float32"))}
     for b, x in enumerate(sig):
-        wb, lb = _batch([x])
+        wb, lb = padded_batch([x])
         alone = abi_loudness(lib, dev, wb, lb, target=-20.0)
         for a, f, r in zip(alone, full, rev):
             assert a.view(np.int32)[0] == f.view(np.int32)[b] == r.view(np.int32)[order.index(b)], b
         for fmt, allv in enc_all.items():
-            one = fd.fetch_audio(model, _out(wb, lb, dev), *fmt, hop=1, loudness=-20.0)[0]
+            one = fd.fetch_audio(model, out_dict(wb, lb, dev), *fmt, hop=1, loudness=-20.0)[0]
             assert np.array_equal(one.view(np.uint8), allv[b].view(np.uint8)), (fmt, b)
 
 
@@ -185,7 +128,7 @@ def _g711():
 
 @pytest.mark.parametrize("target", [-30.0, -16.0])
 def test_gain_identity_and_result(model, lib, dev, target):
-    out, xs = _engine_outputs(model, dev)["b1_t100"]
+    out, xs = engine_outputs(model, dev)["b1_t100"]
     x = xs[0]
     w = out["wav_predictions"].cpu().numpy()
     _, _, g = abi_loudness(lib, dev, w, [len(x)], target=target)
@@ -213,8 +156,8 @@ def test_gain_identity_and_result(model, lib, dev, target):
 
 def test_silence_and_short_items_are_left_as_they_are(model, dev):
     sig = synthetic_items()
-    w, lens = _batch([sig["silence"], sig["n6399"], sig["n6400"]])
-    out = _out(w, lens, dev)
+    w, lens = padded_batch([sig["silence"], sig["n6399"], sig["n6400"]])
+    out = out_dict(w, lens, dev)
     for fmt in ((None, "float32"), (24000, "pcm16")):
         plain = fd.fetch_audio(model, out, *fmt, hop=1)
         norm = fd.fetch_audio(model, out, *fmt, hop=1, loudness=-23.0)
@@ -230,7 +173,7 @@ def pdl_dump(path):
     lib = _abi.load()
     dev = torch.device("cuda:0")
     sig = synthetic_items()
-    w, lens = _batch([sig[k] for k in ("tone_997_m20", "noise_m40", "n32777", "silence")])
+    w, lens = padded_batch([sig[k] for k in ("tone_997_m20", "noise_m40", "n32777", "silence")])
     lufs, pk, g = abi_loudness(lib, dev, w, lens, target=-18.0)
     wt = torch.from_numpy(w).to(dev)
     n_in = torch.tensor(lens, dtype=torch.int64, device=dev)
@@ -239,13 +182,13 @@ def pdl_dump(path):
     bank = torch.from_numpy(audio.polyphase_bank(3, 2)).to(dev)
     gain = torch.from_numpy(g).to(dev)
     dst = torch.empty(int(offs[-1]), dtype=torch.float32, device=dev)
-    _abi.check(lib.ev_format_audio_gain(wt.data_ptr(), wt.stride(0), n_in.data_ptr(), None, len(lens), off.data_ptr(), bank.data_ptr(),
-                                        3, 2, bank.shape[1], 0, dst.data_ptr(), gain.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    _abi.check(lib.ev_format_audio(wt.data_ptr(), wt.stride(0), n_in.data_ptr(), None, len(lens), off.data_ptr(), bank.data_ptr(),
+                                   3, 2, bank.shape[1], 0, dst.data_ptr(), gain.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
     np.savez(path, lufs=lufs, peak=pk, gain=g, out=dst.cpu().numpy())
 
 
 def test_no_change_without_a_target_and_with_pdl_off(model, lib, dev, tmp_path):
-    out, xs = _engine_outputs(model, dev)["b3_padded"]
+    out, xs = engine_outputs(model, dev)["b3_padded"]
     w = out["wav_predictions"]
     n_in = torch.tensor([len(x) for x in xs], dtype=torch.int64, device=dev)
     st = torch.cuda.current_stream(dev).cuda_stream
@@ -256,10 +199,11 @@ def test_no_change_without_a_target_and_with_pdl_off(model, lib, dev, tmp_path):
         it = torch.tensor([2, 0, 1], dtype=torch.int64, device=dev)
         a = torch.full((int(offs[-1]) * 4,), 7, dtype=torch.uint8, device=dev)
         b = a.clone()
+        ones = torch.ones(3, dtype=torch.float32, device=dev)
         args = (w.data_ptr(), w.stride(0), n_in.data_ptr(), it.data_ptr(), 3, off.data_ptr(), None if bank is None else bank.data_ptr(),
                 up, down, 0 if bank is None else bank.shape[1], enc)
-        _abi.check(lib.ev_format_audio(*args, a.data_ptr(), st))
-        _abi.check(lib.ev_format_audio_gain(*args, b.data_ptr(), None, st))
+        _abi.check(lib.ev_format_audio(*args, a.data_ptr(), None, st))
+        _abi.check(lib.ev_format_audio(*args, b.data_ptr(), ones.data_ptr(), st))       # fp32(y * 1) == y
         assert torch.equal(a, b), (up, down, enc)
     here = str(tmp_path / "pdl_on.npz")
     pdl_dump(here)
@@ -293,7 +237,7 @@ def test_microbatcher_mixed_targets_equal_fetch_audio_alone(model, dev):
 
 
 def test_invalid_arguments_raise_before_anything_is_enqueued(model, lib, dev):
-    out, xs = _engine_outputs(model, dev)["b3_padded"]
+    out, xs = engine_outputs(model, dev)["b3_padded"]
     torch.cuda.synchronize()
     n0 = _abi.launch_count()
     for bad in (float("nan"), float("inf"), 1.0, -71.0, True, "-23"):
