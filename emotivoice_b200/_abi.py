@@ -75,6 +75,9 @@ SIGNATURES = {
     "ev_flac_bound_bytes": (_sz, [ctypes.c_longlong]),
     "ev_flac_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
     "ev_flac_encode": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "ev_watermark_embed": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _i, _u64, _vp, ctypes.c_longlong, _vp]),
+    "ev_watermark_detect_workspace_bytes": (_sz, [_i]),
+    "ev_watermark_detect": (_i, [_vp, ctypes.c_longlong, _vp, _i, _u64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ev_launch_count": (_u64, []),
     "ev_op_conv1d": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp]),
     "ev_op_conv1d_tc": (_i, [_vp, _vp, _i, _vp, _sz, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _f, _i, _i, _f, _vp, _sz, _vp]),

@@ -1,7 +1,7 @@
 """Host side of the output formats (``JETSGenerator.format_audio``, ``frontdoor.fetch_audio``): which rates and encodings are
 accepted, the resampling ratio, the polyphase filter bank ``ev_format_audio`` runs, the loudness targets and K-weighting
 filter of ``ev_loudness``, the ceiling checks, detector bank and fixed constants of ``ev_limit``, and the frame-header rate code
-of ``ev_flac_encode``.  Pure host code, no CUDA.
+of ``ev_flac_encode``, and the watermark's constants and key check.  Pure host code, no CUDA.
 
 Resampling is ``scipy.signal.resample_poly(x, up, down)`` with its defaults: the filter is
 ``firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up``, input outside the item is zero, and an
@@ -98,18 +98,53 @@ def check_true_peak(ceiling):
     return c
 
 
-# A validated output format: the rate and its resampling factors from the source rate, the encoding ("flac" or one of
-# ENCODINGS), the loudness target (LUFS) and the true-peak ceiling (dBTP), each None when not asked for.  Hashable: the
-# MicroBatcher formats all requests of one key with one call.
-OutputFormat = collections.namedtuple("OutputFormat", "rate up down encoding loudness true_peak")
+def check_watermark(key):
+    """A watermark key -> int.  Raises ValueError unless it is an integer (not a bool) in [1, 2^63 - 1]."""
+    if isinstance(key, (bool, np.bool_)) or not isinstance(key, (int, np.integer)):
+        raise ValueError("watermark must be an integer key, got %r" % (key,))
+    if not WATERMARK_KEY_RANGE[0] <= int(key) <= WATERMARK_KEY_RANGE[1]:
+        raise ValueError("watermark must be a key in [1, 2^63 - 1], got %r" % (key,))
+    return int(key)
 
 
-def output_format(sample_rate, encoding, loudness, true_peak, source_rate):
-    """The arguments of ``format_audio`` -> ``OutputFormat``, checked by ``plan``, ``check_loudness`` and ``check_true_peak`` in
-    that order.  Raises their ValueError otherwise."""
+_FIELDS = ("rate", "up", "down", "encoding", "loudness", "true_peak", "watermark")
+
+
+class OutputFormat(tuple):
+    """A validated output format: the rate and its resampling factors from the source rate, the encoding ("flac" or one of
+    ENCODINGS), the loudness target (LUFS), the true-peak ceiling (dBTP) and the watermark key, each None when not asked for.
+    Hashable: the MicroBatcher formats all requests of one key with one call.  Without a watermark it is the six-tuple of the
+    first six fields, so it equals the formats (and tuples) made before the mark existed; with one it has seven."""
+    __slots__ = ()
+
+    def __new__(cls, rate, up, down, encoding, loudness, true_peak, watermark=None):
+        fields = (rate, up, down, encoding, loudness, true_peak)
+        return tuple.__new__(cls, fields if watermark is None else fields + (watermark,))
+
+    def __repr__(self):
+        return "OutputFormat(%s)" % ", ".join("%s=%r" % (f, getattr(self, f)) for f in _FIELDS)
+
+    def __getnewargs__(self):
+        return tuple(self)
+
+
+for _i, _f in enumerate(_FIELDS):
+    setattr(OutputFormat, _f, property(lambda self, i=_i: self[i] if i < len(self) else None))
+
+
+def output_format(sample_rate, encoding, loudness, true_peak, source_rate, *, watermark=None):
+    """The arguments of ``format_audio`` -> ``OutputFormat``, checked by ``plan``, ``check_loudness``, ``check_true_peak`` and
+    ``check_watermark`` in that order; a watermark also needs an output rate of at least 8000 Hz, where its band still fits.
+    Raises their ValueError otherwise."""
     rate, up, down = plan(sample_rate, encoding, source_rate)
-    return OutputFormat(rate, up, down, encoding, None if loudness is None else check_loudness(loudness),
-                        None if true_peak is None else check_true_peak(true_peak))
+    loudness = None if loudness is None else check_loudness(loudness)
+    true_peak = None if true_peak is None else check_true_peak(true_peak)
+    if watermark is not None:
+        watermark = check_watermark(watermark)
+        if rate < WATERMARK_MIN_RATE:
+            raise ValueError("a watermark needs an output rate of at least %d Hz (its band reaches 3.4 kHz), got %d"
+                             % (WATERMARK_MIN_RATE, rate))
+    return OutputFormat(rate, up, down, encoding, loudness, true_peak, watermark)
 
 
 # The true-peak limiter of ev_limit: fixed constants, not options.
@@ -162,6 +197,18 @@ def limit_bank(sr, rate):
     up_, down_ = int(rate) // g, int(sr) // g
     resample_half = -(-10 * max(up_, down_) // up_) if (up_, down_) != (1, 1) else 0
     return np.ascontiguousarray(bank.astype(np.float32)), max(half, resample_half)
+
+
+# The watermark of ev_watermark_embed / ev_watermark_detect (emotivoice_b200.watermark): fixed constants, not options.  They
+# hold at the model's rate, 16 kHz.
+WATERMARK_N = 1024              # MCLT frame (sine window); bins of 15.625 Hz, bin k centred at (k + 1/2) 15.625 Hz
+WATERMARK_HOP = 512             # frame j covers samples [(j - 1) hop, (j + 1) hop), j = 0 .. ceil(n / hop)
+WATERMARK_BAND = (19, 218)      # bins 19..217: about 300-3400 Hz, inside 8 kHz telephony and the resampler's passband
+WATERMARK_PERIOD = 64           # P: the pattern repeats every 64 frames (about 2 s)
+WATERMARK_ALPHA = 10.0 ** (-20.0 / 20.0) / math.sqrt(2.0)   # the mark 20 dB under the host's in-band energy (E[C^2] = M^2 / 2)
+WATERMARK_DETECT_Z = 7.0        # detection threshold (see emotivoice_b200.watermark)
+WATERMARK_MIN_RATE = 8000       # output rates below this cut into the band
+WATERMARK_KEY_RANGE = (1, 2 ** 63 - 1)
 
 
 def k_weighting(sr):

@@ -8,12 +8,14 @@
 // One CTA per (item, tile of kTile frames).  The tile's input span is staged in shared memory once, with the reflect padding
 // applied in the index map; nothing at or past n_samples[b] is read.  Each warp transforms one frame at a time: the 1024 real
 // samples are taken as 512 complex pairs z[n] = w[2n] x[2n] + i w[2n+1] x[2n+1], transformed by three radix-8 Stockham stages
-// in shared memory (fp32 FFMA, twiddles from a host table built in fp64), and split into bins 0..512 of the real transform:
+// in shared memory (stockham.cuh: fp32 FFMA, twiddles from a host table built in fp64), and split into bins 0..512 of the
+// real transform:
 //   X[k] = E[k] + W_1024^k O[k],  E = (Z[k] + conj Z[512-k]) / 2,  O = (Z[k] - conj Z[512-k]) / 2i.
 // The epilogue (magnitude, energy, mel bands, log) runs in the same warp; results leave through a per-tile buffer so the
 // channels-first mel rows are stored along time.  Every output is computed from its own item's samples in a fixed order, so a
 // batch is bitwise its items' single-item calls.
 #include "ev_common.cuh"
+#include "stockham.cuh"
 
 namespace ev {
 
@@ -41,63 +43,6 @@ struct FeatsParams {
   float* energy;             // (B, F) or null
   int32_t* status;           // or null
 };
-
-__device__ __forceinline__ int bpad(int i) { return i + (i >> 3); }
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
-__device__ __forceinline__ void bfly(float2& a, float2& b) {
-  const float2 t = a;
-  a = make_float2(t.x + b.x, t.y + b.y);
-  b = make_float2(t.x - b.x, t.y - b.y);
-}
-
-// In-register 8-point DFT (forward, e^{-i}), radix-2 decimation in frequency: bin k ends in v[bitrev3(k)].
-__device__ __forceinline__ void fft8(float2 (&v)[8]) {
-  constexpr float s = 0.70710678118654752440f;
-  bfly(v[0], v[4]); bfly(v[1], v[5]); bfly(v[2], v[6]); bfly(v[3], v[7]);
-  v[5] = make_float2((v[5].x + v[5].y) * s, (v[5].y - v[5].x) * s);      // * W8^1
-  v[6] = make_float2(v[6].y, -v[6].x);                                  // * W8^2 = -i
-  v[7] = make_float2((v[7].y - v[7].x) * s, -(v[7].x + v[7].y) * s);     // * W8^3
-  bfly(v[0], v[2]); bfly(v[1], v[3]); bfly(v[4], v[6]); bfly(v[5], v[7]);
-  v[3] = make_float2(v[3].y, -v[3].x);
-  v[7] = make_float2(v[7].y, -v[7].x);
-  bfly(v[0], v[1]); bfly(v[2], v[3]); bfly(v[4], v[5]); bfly(v[6], v[7]);
-}
-
-__device__ __forceinline__ int brev3(int k) { return ((k & 1) << 2) | (k & 2) | ((k >> 2) & 1); }
-
-// Stockham radix-8 stage of the 512-point FFT, NS = 8^stage: butterfly j reads v[r] = in[j + 64 r] * W_{8 NS}^{r (j % NS)} and
-// writes bin r of its 8-point DFT to out[(j / NS) * 8 NS + j % NS + r NS].  Every lane holds its two butterflies in registers
-// between the reads and the writes, so in and out may be the same buffer.
-template <int NS>
-__device__ __forceinline__ void stockham_store(float2 (&v)[2][8], float2* buf, int lane) {
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    const int j = lane + 32 * q;
-    const int d = (j / NS) * NS * 8 + j % NS;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) buf[bpad(d + r * NS)] = v[q][brev3(r)];
-  }
-}
-
-template <int NS>
-__device__ __forceinline__ void stockham_stage(float2* buf, const float2* tw, int lane) {
-  float2 v[2][8];
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    const int j = lane + 32 * q;
-    const int k = j % NS;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) v[q][r] = buf[bpad(j + 64 * r)];
-#pragma unroll
-    for (int r = 1; r < 8; ++r) v[q][r] = cmul(v[q][r], tw[2 * r * k * (kHalf / (8 * NS))]);   // W_512^m = W_1024^2m
-    fft8(v[q]);
-  }
-  __syncwarp();
-  stockham_store<NS>(v, buf, lane);
-  __syncwarp();
-}
 
 __global__ void __launch_bounds__(kWarps * 32) stft_feats_kernel(const FeatsParams p) {
   pdl_entry();

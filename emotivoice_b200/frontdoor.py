@@ -279,47 +279,49 @@ class MicroBatcher:
         self._thread.start()
 
     def submit(self, ids, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0, durations=None,
-               pitch=None, energy=None, sample_rate=None, encoding=None, loudness=None, true_peak=None):
+               pitch=None, energy=None, sample_rate=None, encoding=None, loudness=None, true_peak=None, watermark=None):
         """``speed`` > 1 speaks faster (duration_scale = 1 / speed); ``pitch_shift`` in semitones; ``energy_scale``
         multiplies frame energy.  Each is a float or a sequence of ``len(ids)`` values, one per phoneme (a per-phoneme speed
         must lie in [1/16, 16]).  ``durations`` (integer frames), ``pitch`` and ``energy`` (the predictors' normalised units):
         None or ``len(ids)`` values that replace the model's predictions (see ``JETSGenerator.forward``).  ``sample_rate`` /
-        ``encoding`` / ``loudness`` / ``true_peak``: see ``_output_format``.  Invalid values raise ValueError here, so they cannot
+        ``encoding`` / ``loudness`` / ``true_peak`` / ``watermark``: see ``_output_format``.  Invalid values raise ValueError here, so they cannot
         fail a batch of other requests."""
         ids = np.asarray(ids, dtype=np.int64)
         controls = phoneme_controls(len(ids), speed, pitch_shift, energy_scale)
         given = given_values(len(ids), durations, pitch, energy)
-        fmt = self._output_format(sample_rate, encoding, loudness, true_peak)
+        fmt = self._output_format(sample_rate, encoding, loudness, true_peak, watermark)
         item = (ids, int(speaker_id), style_vec, content_vec, controls) + ((given,) if given else ())
         return self._enqueue([item], False, fmt)
 
     def submit_joined(self, segments, speaker_id, style_vec, content_vec, speed=1.0, pitch_shift=0.0, energy_scale=1.0,
-                      sample_rate=None, encoding=None, loudness=None, true_peak=None):
+                      sample_rate=None, encoding=None, loudness=None, true_peak=None, watermark=None):
         """One long text as ``segments``: a list of phoneme id arrays, e.g. ``split_phonemes`` output put through ``encode``.
         ``style_vec`` / ``content_vec``: one vector for every segment, or a list (or a 2-D array) with one vector per segment,
         for a different prompt per sentence.  ``speed`` / ``pitch_shift`` / ``energy_scale``: one float each, checked as in
         ``submit``.  The future's result is the text's float32 waveform, the segments' mel joined and vocoded as one,
         trimmed to ``joined_lengths[g] * hop``, or that waveform in the format of ``sample_rate`` / ``encoding`` / ``loudness`` /
-        ``true_peak`` (see ``_output_format``).  Raises ValueError here for invalid arguments."""
+        ``true_peak`` / ``watermark`` (see ``_output_format``).  Raises ValueError here for invalid arguments."""
         segs = [np.asarray(s, dtype=np.int64) for s in segments]
         if not segs or any(s.ndim != 1 or s.size == 0 for s in segs):
             raise ValueError("segments must be a non-empty list of non-empty 1-D phoneme id arrays")
         controls = speech_controls(speed, pitch_shift, energy_scale)
         styles = _per_segment("style_vec", style_vec, len(segs))
         contents = _per_segment("content_vec", content_vec, len(segs))
-        fmt = self._output_format(sample_rate, encoding, loudness, true_peak)
+        fmt = self._output_format(sample_rate, encoding, loudness, true_peak, watermark)
         items = [(s, int(speaker_id), st, ct, controls) for s, st, ct in zip(segs, styles, contents)]
         return self._enqueue(items, True, fmt)
 
-    def _output_format(self, sample_rate, encoding, loudness, true_peak=None):
-        """A request's output format: None when all four are None (the result is the float32 waveform tensor, as always), else
+    def _output_format(self, sample_rate, encoding, loudness, true_peak=None, watermark=None):
+        """A request's output format: None when all five are None (the result is the float32 waveform tensor, as always), else
         the ``audio.OutputFormat`` ``fetch_audio`` is called with: the result is then a numpy array at ``sample_rate`` (None: the
-        model's rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None: not normalised) and limited to
-        ``true_peak`` dBTP (None: not limited).  Raises ValueError for a rate, encoding, loudness target or ceiling
-        ``format_audio`` does not take."""
-        if sample_rate is None and encoding is None and loudness is None and true_peak is None:
+        model's rate) in ``encoding`` (None: "pcm16"), normalised to ``loudness`` LUFS (None: not normalised), limited to
+        ``true_peak`` dBTP (None: not limited) and marked with the key ``watermark`` (None: not marked).  Requests with different
+        keys have different formats, so each key gets its own ``fetch_audio`` call.  Raises ValueError for a rate, encoding,
+        loudness target, ceiling or key ``format_audio`` does not take."""
+        if sample_rate is None and encoding is None and loudness is None and true_peak is None and watermark is None:
             return None
-        return audio.output_format(sample_rate, "pcm16" if encoding is None else encoding, loudness, true_peak, self._sr)
+        return audio.output_format(sample_rate, "pcm16" if encoding is None else encoding, loudness, true_peak, self._sr,
+                                   watermark=watermark)
 
     def _enqueue(self, items, joined, fmt):
         fut = Future()
@@ -389,8 +391,9 @@ class MicroBatcher:
                     formats.setdefault(e[3], []).append(r)
             results = {}
             for f, rs in formats.items():
+                mark = {} if f.watermark is None else {"watermark": f.watermark}     # only asked of fetch_audio when used
                 results.update(zip(rs, fetch_audio(self._forward, out, f.rate, f.encoding, items=rs, hop=self._hop, loudness=f.loudness,
-                                                   true_peak=f.true_peak)))
+                                                   true_peak=f.true_peak, **mark)))
             if len(results) < len(batch):
                 wav = out["wav_predictions"]
                 lens = out.get("joined_lengths_host", out.get("joined_lengths")) if joined else out.get("mel_lengths")
@@ -462,16 +465,19 @@ def audio_to_wav_bytes(samples, sample_rate, encoding="pcm16"):
     return header + data + b"\0" * pad
 
 
-def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
+def fetch_audio(model, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None,
+                watermark=None):
     """Finish one forward in the format a client asked for: ``model.format_audio`` resamples to ``sample_rate`` (None: the
     model's 16 kHz) and encodes ("float32", "pcm16", "mulaw" or "alaw") only the valid samples of each output, packed, on the
     GPU, after normalising each output to ``loudness`` LUFS when that is given (BS.1770-4 integrated loudness, -1 dBFS
     sample-peak ceiling; see ``format_audio``) and limiting each to ``true_peak`` dBTP when that is given (a look-ahead
-    true-peak limiter, which replaces the sample-peak ceiling); then ONE device->host copy of that buffer into pinned memory.  ``out`` is the
+    true-peak limiter, which replaces the sample-peak ceiling), each marked with the key ``watermark`` when that is given
+    (``emotivoice_b200.watermark.detect`` finds the mark); then ONE device->host copy of that buffer into pinned memory.  ``out`` is the
     dict ``model(...)`` returned; ``items`` selects outputs (default: all).  Returns a list of 1-D numpy arrays (float32, int16
     or uint8), one per batch item, or per group of a joined forward.  "flac": each array is the bytes of a complete .flac file
     whose samples are the "pcm16" result.  Invalid arguments raise ValueError before anything is enqueued."""
-    packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, loudness=loudness, true_peak=true_peak)
+    packed, offs = model.format_audio(out, sample_rate, encoding, items=items, hop=hop, loudness=loudness, true_peak=true_peak,
+                                      watermark=watermark)
     host = torch.empty(packed.shape, dtype=packed.dtype, pin_memory=True)
     host.copy_(packed, non_blocking=True)
     torch.cuda.current_stream(packed.device).synchronize()

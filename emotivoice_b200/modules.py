@@ -793,7 +793,8 @@ class JETSGenerator(_EngineOwner):
             return eng.output.measure(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
 
     @torch.no_grad()
-    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None):
+    def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None,
+                     watermark=None):
         """The output of a forward in a client's format, on the GPU: each output's valid samples, resampled to ``sample_rate``
         (None: the model's rate, ``config.sr``, 16000) and encoded, packed back to back.
 
@@ -820,6 +821,13 @@ class JETSGenerator(_EngineOwner):
         waveform is then resampled and encoded with no further gain.  None: the limiter does not run, and the output is exactly
         as without the argument.
 
+        ``watermark`` (an integer key in [1, 2^63 - 1], or None): before anything else, each output gets a keyed mark that
+        ``emotivoice_b200.watermark.detect`` finds again (``ev_watermark_embed``, at the model's rate; see ``audio`` for its
+        constants): in each 1024-sample MCLT frame, bins of about 300-3400 Hz are changed by a keyed +-1 pattern 20 dB under
+        their own magnitude.  Loudness, the limiter, resampling and encoding then process the marked output, so their targets
+        hold for what is delivered.  Needs an output rate of at least 8000 Hz.  None: the output is exactly as without the
+        argument.
+
         ``encoding="flac"``: each output becomes a complete .flac file image (RFC 9639: mono, 16 bits, 4096-sample blocks) of
         exactly the samples "pcm16" gives, encoded on the GPU by ev_flac_encode; decoding it returns that PCM16 bit for bit.
         The images' sizes exist only after encoding, so this encoding makes ONE device->host read of the len(items) + 1
@@ -829,7 +837,7 @@ class JETSGenerator(_EngineOwner):
         ``packed[offs[k]:offs[k + 1]]``).  No sync except for "flac": the lengths are the host copies the forward read.
         Invalid arguments raise ValueError before anything is enqueued."""
         sr = int(getattr(self.config, "sr", 16000))
-        fmt = audio.output_format(sample_rate, encoding, loudness, true_peak, sr)
+        fmt = audio.output_format(sample_rate, encoding, loudness, true_peak, sr, watermark=watermark)
         wav, n_in, items, eng = self._outputs(out, items, hop)
         if encoding == audio.FLAC and any(n_in[b] < 1 for b in items):
             raise ValueError("an output with no samples cannot be a FLAC stream (valid samples %s)" % [n_in[b] for b in items])

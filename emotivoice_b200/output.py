@@ -1,6 +1,6 @@
-"""The output chain of one engine: loudness measurement (ev_loudness), true-peak limiting (ev_limit), resampling and encoding
-(ev_format_audio) and FLAC (ev_flac_encode) of a forward's outputs, in that order, with the filter banks and coefficients those
-stages read.  ``JETSGenerator.format_audio`` / ``measure_loudness`` validate their arguments and call it under the engine's lock.
+"""The output chain of one engine: the watermark (ev_watermark_embed), loudness measurement (ev_loudness), true-peak limiting
+(ev_limit), resampling and encoding (ev_format_audio) and FLAC (ev_flac_encode) of a forward's outputs, in that order, with
+the filter banks and coefficients those stages read.  ``JETSGenerator.format_audio`` / ``measure_loudness`` validate their arguments and call it under the engine's lock.
 """
 import numpy as np
 import torch
@@ -73,7 +73,9 @@ class Chain:
         """The listed items of a (B,1,L) fp32 waveform at ``sr`` Hz, host valid samples ``n_in`` (B ints <= L), in the
         ``audio.OutputFormat`` ``fmt`` -> (packed device tensor, (len(items)+1,) int64 host offsets).
 
-        With ``fmt.true_peak``, ev_limit first writes the limited items to the "limited" workspace, which the later stages read:
+        With ``fmt.watermark``, ev_watermark_embed first writes the marked items to the "marked" workspace, and every later
+        stage reads that instead of ``wav``, so loudness targets and the ceiling hold for what is delivered.
+        With ``fmt.true_peak``, ev_limit then writes the limited items to the "limited" workspace, which the later stages read:
         with ``fmt.loudness`` two passes (L0 of the items, limit x * g1, L1 of that result, limit x * g1 * g2; see
         ``JETSGenerator.format_audio``), else one pass with no pre-gain.  Otherwise with ``fmt.loudness`` one ev_loudness gives
         the gain of ev_format_audio.  "flac" encodes the PCM16 result and reads its image offsets back: the only sync."""
@@ -84,24 +86,29 @@ class Chain:
         if packed.numel() == 0:                  # every listed output is empty (never for "flac"): nothing to launch
             return packed, offs
         arrays = [n_in, items, offs]
-        if fmt.true_peak is not None:
-            arrays.append([int(n_in[b]) for b in items])                 # the limited items' lengths, in listed order
+        if fmt.true_peak is not None or fmt.watermark is not None:
+            arrays.append([int(n_in[b]) for b in items])                 # the limited / marked items' lengths, in listed order
         meta, ptrs = self._meta(arrays)
         p_n, p_items, p_off = ptrs[:3]
         src, src_n, src_items, gain = wav, p_n, p_items, None
+        stride = int(wav.stride(0))
+        if fmt.watermark is not None:
+            marked = self._ws("marked", 4 * k * stride)[:4 * k * stride].view(torch.float32).view(k, stride)
+            _abi.check(lib.ev_watermark_embed(wav.data_ptr(), stride, p_n, p_items, k, sr, fmt.watermark, marked.data_ptr(), stride,
+                                              self._stream()))
+            src, src_n, src_items = marked, ptrs[3], None
         if fmt.true_peak is not None:
             p_nl = ptrs[3]
-            stride = int(wav.stride(0))
             lim = self._ws("limited", 4 * k * stride)[:4 * k * stride].view(torch.float32).view(k, stride)
             lufs0 = lufs1 = None
             if fmt.loudness is not None:
-                lufs0 = self._loudness(wav, p_n, p_items, k, sr, fmt.loudness)[0]
-                self._limit(wav, p_n, p_items, k, sr, fmt.rate, lufs0, None, fmt.loudness, fmt.true_peak, lim)
+                lufs0 = self._loudness(src, src_n, src_items, k, sr, fmt.loudness)[0]
+                self._limit(src, src_n, src_items, k, sr, fmt.rate, lufs0, None, fmt.loudness, fmt.true_peak, lim)
                 lufs1 = self._loudness(lim, p_nl, None, k, sr, fmt.loudness)[0]
-            self._limit(wav, p_n, p_items, k, sr, fmt.rate, lufs0, lufs1, fmt.loudness, fmt.true_peak, lim)
+            self._limit(src, src_n, src_items, k, sr, fmt.rate, lufs0, lufs1, fmt.loudness, fmt.true_peak, lim)
             src, src_n, src_items = lim, p_nl, None
         elif fmt.loudness is not None:
-            gain = self._loudness(wav, p_n, p_items, k, sr, fmt.loudness)[2]
+            gain = self._loudness(src, src_n, src_items, k, sr, fmt.loudness)[2]
         bank = None
         if (fmt.up, fmt.down) != (1, 1):
             bank = self._banks.get((fmt.up, fmt.down))

@@ -1,0 +1,96 @@
+"""Finds the watermark ``format_audio(watermark=KEY)`` embeds: ``detect(wav, sample_rate, key)`` answers "does this recording
+carry the mark of this key?" for each recording of a batch, on the GPU (``ev_watermark_detect``).
+
+The mark carries no payload.  At 16 kHz, in MCLT frames of 1024 samples (hop 512, sine window), each MDCT coefficient C of
+bins 19..217 (about 300-3400 Hz) of frame j was changed by alpha * M * s(key, j mod 64, k), M the MCLT magnitude and s = +-1
+a keyed pattern (``audio.WATERMARK_*``).  The detector analyses the recording on the grid shifted by tau samples for every tau
+in [0, 512), takes u = C / M in the band (skipping cells with M = 0), folds the frames modulo 64 into b[tau, r, k], and for
+every frame phase m0 in [0, 64) computes
+
+    z(tau, m0) = sum_{r,k} s(key, (r + m0) mod 64, k) b[tau, r, k] / sqrt(sum_{r,k} b[tau, r, k]^2).
+
+It reports the largest z of each recording and its (tau, m0): for a recording that starts c samples into a marked output,
+tau = -c mod 512 and m0 = ((c + tau) / 512) mod 64.
+
+False positives.  Take a recording and a key chosen independently of it, and model the pattern as an ideal keyed PRF: the
+signs s(key, ., .) are then independent fair +-1 given b, and for a fixed (tau, m0) they multiply 64 * 199 distinct cells of
+b.  The numerator is a Rademacher sum sum_i s_i b_i, and Hoeffding's inequality gives P(sum_i s_i b_i >= t ||b||) <=
+exp(-t^2 / 2), with no Gaussian assumption and whatever the recording.  A union over the 512 * 64 = 32768 hypotheses gives
+P(max z >= t) <= 32768 exp(-t^2 / 2); at t = DETECT_Z = 7.0 that is 32768 * e^-24.5 = 7.6e-7 per (recording, key).  SplitMix64
+is not a cryptographic PRF, so the bound is for keys chosen without knowledge of the recording.
+
+Silence (every cell M = 0) gives z = 0.
+"""
+import torch
+
+from . import _abi, audio
+
+DETECT_Z = audio.WATERMARK_DETECT_Z
+SR = 16000
+
+
+def _to_device(values, dev):
+    """Host integers -> a device int64 tensor through pinned memory, without a sync."""
+    return torch.tensor(values, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+
+
+def _resample_to_16k(wav, lens, rate, dev, lib):
+    """The (B, L) recordings at ``rate`` -> (B, L16) float32 at 16 kHz through ev_format_audio's float32 path (each row's
+    valid samples resampled as ``scipy.signal.resample_poly`` does), and the lengths at 16 kHz."""
+    _, up, down = audio.plan(SR, "float32", rate)
+    B, L = wav.shape
+    lens16 = [audio.resampled_length(n, up, down) for n in lens]
+    out = torch.empty((B, audio.resampled_length(L, up, down)), dtype=torch.float32, device=dev)
+    meta = _to_device(lens + [b * out.stride(0) for b in range(B)], dev)        # n_in, then where each row starts in out
+    bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev, non_blocking=True)
+    _abi.check(lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), meta.data_ptr(), None, B, meta.data_ptr() + 8 * B,
+                                   bank.data_ptr(), up, down, int(bank.shape[1]), audio.ENCODINGS["float32"], out.data_ptr(),
+                                   None, torch.cuda.current_stream(dev).cuda_stream))
+    return out, lens16
+
+
+@torch.no_grad()
+def detect(wav, sample_rate, key, lengths=None):
+    """Searches each recording for the mark of ``key``.
+
+    ``wav``: a CUDA (B, L) float32 tensor, one recording per row.  ``sample_rate``: their rate in Hz, at least 8000; a rate
+    other than 16 kHz is first resampled to 16 kHz by ``ev_format_audio`` (the rates ``audio.plan`` accepts).  ``key``: an
+    integer in [1, 2^63 - 1].  ``lengths``: the valid samples of each row (a sequence or a CPU tensor of B integers in [0, L]);
+    None: every row is L samples.
+
+    Returns (z float32, offset int32, phase int32) device tensors of shape (B,): the largest z of each recording and its grid
+    offset tau and frame phase m0.  z >= DETECT_Z means the mark is present (see the module docstring for the bound).  No
+    sync.  Invalid arguments raise ValueError before anything is enqueued."""
+    if not (isinstance(wav, torch.Tensor) and wav.dim() == 2 and wav.dtype == torch.float32 and wav.is_cuda):
+        raise ValueError("wav must be a CUDA (B, L) float32 tensor")
+    B, L = int(wav.shape[0]), int(wav.shape[1])
+    if not 1 <= B <= 65535 or L < 1:
+        raise ValueError("wav must hold 1 to 65535 recordings of at least one sample, got shape %s" % (tuple(wav.shape),))
+    rate = audio.plan(sample_rate, "float32", SR)[0]
+    if rate < audio.WATERMARK_MIN_RATE:
+        raise ValueError("the mark's band needs a rate of at least %d Hz, got %d" % (audio.WATERMARK_MIN_RATE, rate))
+    key = audio.check_watermark(key)
+    if lengths is None:
+        lens = [L] * B
+    else:
+        if torch.is_tensor(lengths):
+            if lengths.device.type != "cpu":
+                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
+            lengths = lengths.tolist()
+        lens = [int(v) for v in lengths]
+        if len(lens) != B or any(n < 0 or n > L for n in lens):
+            raise ValueError("lengths must be %d integers in [0, %d], got %s" % (B, L, lens))
+    lib = _abi.load()
+    dev = wav.device
+    wav = wav.contiguous()
+    if rate != SR:
+        wav, lens = _resample_to_16k(wav, lens, rate, dev, lib)
+    n = _to_device(lens, dev)
+    z = torch.empty((B,), dtype=torch.float32, device=dev)
+    offset = torch.empty((B,), dtype=torch.int32, device=dev)
+    phase = torch.empty((B,), dtype=torch.int32, device=dev)
+    nb = int(lib.ev_watermark_detect_workspace_bytes(B))
+    ws = torch.empty((nb,), dtype=torch.uint8, device=dev)
+    _abi.check(lib.ev_watermark_detect(wav.data_ptr(), int(wav.stride(0)), n.data_ptr(), B, key, z.data_ptr(), offset.data_ptr(),
+                                       phase.data_ptr(), ws.data_ptr(), nb, torch.cuda.current_stream(dev).cuda_stream))
+    return z, offset, phase

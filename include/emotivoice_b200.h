@@ -313,6 +313,30 @@ EV_API size_t ev_flac_workspace_bytes(int n_items, long long max_n);          /*
 EV_API int ev_flac_encode(const int16_t* pcm, const int64_t* pcm_off, int n_items, const int64_t* n_samples, int sample_rate,
                           uint8_t* out, size_t out_bytes, int64_t* out_off, void* ws, size_t ws_bytes, void* stream);
 
+/* Keyed zero-bit watermark of listed 16 kHz waveform items, a machine-readable mark that the output is synthetic
+ * (emotivoice_b200.audio holds the definition; oracle/watermark_oracle.py restates it in fp64).  The MCLT of frames of 1024
+ * samples, hop 512, sine window, frame j over samples [(j - 1) 512, (j + 1) 512) for j = 0 .. ceil(n / 512), zero outside the
+ * item: each MDCT coefficient C of bins 19..217 (300-3400 Hz) gets alpha * M * s(key, j mod 64, k), M = sqrt(C^2 + S^2) the
+ * MCLT magnitude, alpha = 10^(-20/20) / sqrt(2), s = +-1 from SplitMix64's output function; y = x + the overlap-added IMDCT
+ * of that change.  Silent stretches stay silent and nothing is added outside the band.
+ *   wav / item_stride / n_in / items / n_items as ev_loudness.  sample_rate must be 16000.  key in [1, 2^63 - 1].
+ *   out[k * out_stride + s] = y[s] for s < n (out_stride >= item_stride; out must not overlap wav); nothing else is written.
+ * One launch; each output is bitwise the same in any batch or order.  No allocation, no sync. */
+EV_API int ev_watermark_embed(const float* wav, long long item_stride, const int64_t* n_in, const int64_t* items, int n_items,
+                              int sample_rate, uint64_t key, float* out, long long out_stride, void* stream);
+
+/* The detector of ev_watermark_embed's mark in 16 kHz items: item k is wav[k * item_stride ..], n (n_items) i64 device array
+ * of its valid samples (clamped to [0, item_stride]).  For each grid offset tau in [0, 512) and frame phase m0 in [0, 64): the
+ * MCLT on frames shifted by tau samples, u = C / M in the band (cells with M = 0 skipped), b[r, k] = sum of u over frames
+ * j = r mod 64, z = sum_{r,k} s(key, (r + m0) mod 64, k) b[r, k] / sqrt(sum b^2) (0 when b is all zero).
+ *   z (n_items) f32, offset / phase (n_items) i32: the largest z of each item and its (tau, m0), the first in (tau, m0) order on
+ *   ties.  ws: ev_watermark_detect_workspace_bytes(n_items) bytes; afterwards it holds each item's best z per tau ((n_items, 512)
+ *   f32) and that z's m0 ((n_items, 512) i32).  Two launches; each result depends only on its own item.
+ *   No allocation, no sync. */
+EV_API size_t ev_watermark_detect_workspace_bytes(int n_items);                  /* 0 for arguments out of range */
+EV_API int ev_watermark_detect(const float* wav, long long item_stride, const int64_t* n, int n_items, uint64_t key, float* z,
+                               int32_t* offset, int32_t* phase, void* ws, size_t ws_bytes, void* stream);
+
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
 EV_API uint64_t ev_launch_count(void);
