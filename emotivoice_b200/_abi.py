@@ -72,6 +72,8 @@ SIGNATURES = {
     "ev_limit_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),
     "ev_limit": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _i, _i, _vp, _vp, _f, _f, _vp, _i, _i, _i, _i, ctypes.c_double, _vp,
                       ctypes.c_longlong, _vp, _sz, _vp]),
+    "ev_meter_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),
+    "ev_meter": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, ctypes.c_longlong, _vp, _sz, _vp]),
     "ev_flac_bound_bytes": (_sz, [ctypes.c_longlong]),
     "ev_flac_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
     "ev_flac_encode": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _vp, _sz, _vp]),

@@ -199,6 +199,21 @@ def limit_bank(sr, rate):
     return np.ascontiguousarray(bank.astype(np.float32)), max(half, resample_half)
 
 
+def true_peak_bank(sr):
+    """The true-peak detector of ev_meter at ``sr`` Hz -> (R, 21) float32, R = ceil(192000 / sr): every phase of the
+    limiter's interpolator ``firwin(2 * 10 * R + 1, 1 / R, kaiser 5) * R``, row p = h[p + j R], phase 0 included, so the
+    detector reads exactly the samples of ``resample_poly(x, R, 1)`` and |x|.  ``limit_bank(sr, sr)`` is rows 1 .. R - 1: the
+    limiter takes |x[n]| for phase 0, but the filter's centre tap is 1 + 6.7e-4 (firwin's unit-gain scaling), so phase 0
+    reads up to 0.0059 dB above |x[n]|.  None at R = 1 (192 kHz), where resample_poly returns x itself."""
+    R = -(-LIMIT_DETECT_RATE // int(sr))
+    if R == 1:
+        return None
+    h = _kaiser_lowpass(10 * R, 1.0 / R) * R
+    padded = np.zeros(21 * R)
+    padded[:len(h)] = h
+    return np.ascontiguousarray(padded.reshape(21, R).T.astype(np.float32))
+
+
 # The watermark of ev_watermark_embed / ev_watermark_detect (emotivoice_b200.watermark): fixed constants, not options.  They
 # hold at the model's rate, 16 kHz.
 WATERMARK_N = 1024              # MCLT frame (sine window); bins of 15.625 Hz, bin k centred at (k + 1/2) 15.625 Hz

@@ -263,6 +263,20 @@ int launch_join_mel(const float* mel, const int32_t* mel_lens, const int32_t* gr
                     int32_t* group_lens, cudaStream_t st);
 void preload_voc_kernels();
 
+// ---------------------------------------------------------------------------------
+// loudness stages of ev_loudness (loudness_kernels.cu), which ev_meter runs too
+// ---------------------------------------------------------------------------------
+long long loud_max_sub(long long max_n, int sample_rate);      // 100 ms sub-blocks of an item of max_n samples (the last partial)
+bool loud_grid_ok(long long max_n, int sample_rate);           // the sub-block grid of max_n fits a launch
+int restart_warmup(const double* kcoef);                       // W of the K-weighting restart, or -1 (unstable / too slow)
+// energy / peak (n_items, loud_max_sub(item_stride)) of every sub-block; item b at wav + start[b] (start NULL: b * item_stride),
+// n_in[b] valid samples clamped to item_stride
+int launch_loud_subblock(const float* wav, long long item_stride, const int64_t* start, const int64_t* n_in, const int64_t* items,
+                         int n_items, int sample_rate, const double* kcoef, int W, double* energy, float* peak, cudaStream_t st);
+// gated integrated loudness, sample peak and normalisation gain of each item from those sub-blocks
+int launch_loud_gate(long long item_stride, const int64_t* n_in, const int64_t* items, int n_items, int sample_rate,
+                     const double* energy, const float* peak, double target, float* lufs, float* peak_out, float* gain, cudaStream_t st);
+
 __device__ __forceinline__ float act_apply(float v, int act, float slope) {
   switch (act) {
     case EV_ACT_LRELU: return v > 0.f ? v : v * slope;

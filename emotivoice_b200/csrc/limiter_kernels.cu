@@ -2,7 +2,7 @@
 // pre-gain g, at or below a ceiling C in dBTP.  Everything runs at the items' own rate; per item of n valid samples:
 //   detector   p[s] = max(|x[s]|, |sum_j bank[ph][j] * x[s + c - j]| over the bank's phases), c = (taps - 1) / 2, x zero outside
 //              [0, n): the oversampled (interpolated, and for a lower output rate also low-passed) waveform around s.  fp32, one
-//              chain per value in tap order.
+//              chain per value in tap order (tp_detect, true_peak.cuh, which ev_meter's true peak runs too).
 //   required   r[s] = min(0, C - 20 log10(g p[s])) in fp64, clamped at -1000 dB and rounded DOWN to the grid Q = 2^-32 dB; 0 outside
 //              the item.
 //   hold       m[s] = min r over [s - M, s + L + M] (look-ahead L, hold M), for s in [-L, n).
@@ -22,6 +22,7 @@
 #include <math.h>
 
 #include "ev_common.cuh"
+#include "true_peak.cuh"
 
 namespace ev {
 
@@ -83,14 +84,7 @@ __global__ void __launch_bounds__(LM_THREADS) lim_detect_kernel(const float* __r
     const long long s = r0 + q;
     double r = 0.0;
     if (s >= 0 && s < n) {
-      const float* xc = xs + q + 2 * c;                       // xc[-j] = x[s + c - j]
-      float p = fabsf(xs[q + c]);
-      for (int ph = 0; ph < phases; ++ph) {
-        const float* h = hs + ph * taps;
-        float acc = 0.f;
-        for (int j = 0; j < taps; ++j) acc = fmaf(h[j], xc[-j], acc);
-        p = fmaxf(p, fabsf(acc));
-      }
+      const float p = tp_detect(xs + q, hs, phases, taps);      // xs[q + c] = x[s]
       const double gp = g * (double)p;
       if (gp > 0.0) r = fmax(fmin(0.0, ceiling - 20.0 * log10(gp)), LM_FLOOR_DB);
       if (!(r == r)) r = LM_FLOOR_DB;                          // a NaN sample: as loud as can be

@@ -8,7 +8,8 @@
 // which decays as the largest pole radius r of the cascade, is below W * r^W <= 1e-10; no state is carried between sub-blocks,
 // so a sub-block's result depends only on its item's samples and the rate.  The 32 sub-blocks of a warp are consecutive: the
 // warp stages 32 samples of each lane's span at a time in shared memory with coalesced loads.  Samples at or past n_in[b] are
-// never read; a last, partial sub-block only gives its peak.
+// never read; a last, partial sub-block only gives its peak.  Item b starts at wav + b * item_stride, or at wav + start[b]
+// when ev_meter passes the items' start offsets (item_stride is then the longest item's length, which bounds n_in).
 // loud_gate_kernel: one CTA per listed item.  Gating blocks are four consecutive sub-blocks (400 ms, 75 % overlap); block
 // loudness l = -0.691 + 10 log10(mean square), the absolute gate keeps l > -70, the relative gate l > (loudness of those) - 10,
 // and L is the loudness of the blocks that pass both.  Sums are fp64 in a fixed order (thread t takes blocks t, t + T, ...,
@@ -32,6 +33,7 @@ struct KCoef {
 };
 
 __global__ void __launch_bounds__(LD_THREADS) loud_subblock_kernel(const float* __restrict__ wav, long long item_stride,
+                                                                   const int64_t* __restrict__ start,
                                                                    const int64_t* __restrict__ n_in, const int64_t* __restrict__ items,
                                                                    int S, int W, long long max_sub, KCoef c,
                                                                    double* __restrict__ energy, float* __restrict__ peak) {
@@ -44,7 +46,7 @@ __global__ void __launch_bounds__(LD_THREADS) loud_subblock_kernel(const float* 
   const long long j0 = ((long long)blockIdx.x * LD_WARPS + warp) * 32;
   if (j0 >= n_sub) return;                                    // whole warps only
   const long long j = j0 + lane;
-  const float* x = wav + b * item_stride;
+  const float* x = wav + (start ? start[b] : b * item_stride);
   float (*buf)[33] = stage[warp];
   float sx1 = 0.f, sx2 = 0.f, sy1 = 0.f, sy2 = 0.f, hy1 = 0.f, hy2 = 0.f;
   double acc = 0.0;
@@ -156,7 +158,7 @@ static double pole_radius(double a1, double a2) {
 }
 
 // W: the smallest multiple of 32 with W * r^W <= LD_TRANSIENT, or -1 (unstable cascade, or W above LD_MAX_WARMUP)
-static int restart_warmup(const double* kc) {
+int restart_warmup(const double* kc) {
   const double r = fmax(pole_radius(kc[3], kc[4]), pole_radius(kc[8], kc[9]));
   if (!(r < 1.0)) return -1;
   if (r == 0.0) return 32;
@@ -165,7 +167,26 @@ static int restart_warmup(const double* kc) {
   return -1;
 }
 
-static long long loud_max_sub(long long max_n, int sample_rate) { return (max_n + sample_rate / 10 - 1) / (sample_rate / 10); }
+long long loud_max_sub(long long max_n, int sample_rate) { return (max_n + sample_rate / 10 - 1) / (sample_rate / 10); }
+
+bool loud_grid_ok(long long max_n, int sample_rate) { return (loud_max_sub(max_n, sample_rate) + LD_THREADS - 1) / LD_THREADS <= 0x7fffffffll; }
+
+int launch_loud_subblock(const float* wav, long long item_stride, const int64_t* start, const int64_t* n_in, const int64_t* items,
+                         int n_items, int sample_rate, const double* kcoef, int W, double* energy, float* peak, cudaStream_t st) {
+  const long long max_sub = loud_max_sub(item_stride, sample_rate);
+  KCoef c;
+  c.s0 = (float)kcoef[0]; c.s1 = (float)kcoef[1]; c.s2 = (float)kcoef[2]; c.sa1 = (float)kcoef[3]; c.sa2 = (float)kcoef[4];
+  c.h0 = (float)kcoef[5]; c.h1 = (float)kcoef[6]; c.h2 = (float)kcoef[7]; c.ha1 = (float)kcoef[8]; c.ha2 = (float)kcoef[9];
+  const long long gx = (max_sub + LD_THREADS - 1) / LD_THREADS;
+  return launch("loud_subblock_kernel", loud_subblock_kernel, dim3((unsigned)gx, n_items), LD_THREADS, 0, st, wav, item_stride, start,
+                n_in, items, sample_rate / 10, W, max_sub, c, energy, peak);
+}
+
+int launch_loud_gate(long long item_stride, const int64_t* n_in, const int64_t* items, int n_items, int sample_rate,
+                     const double* energy, const float* peak, double target, float* lufs, float* peak_out, float* gain, cudaStream_t st) {
+  return launch("loud_gate_kernel", loud_gate_kernel, dim3(n_items), LG_THREADS, 0, st, item_stride, n_in, items, sample_rate / 10,
+                loud_max_sub(item_stride, sample_rate), energy, peak, target, lufs, peak_out, gain);
+}
 
 static size_t loud_ws_bytes(int n_items, long long max_n, int sample_rate) {
   const size_t cells = (size_t)n_items * (size_t)loud_max_sub(max_n, sample_rate);
@@ -203,19 +224,12 @@ int ev_loudness(const float* wav, long long item_stride, const int64_t* n_in, co
   EV_CHECK_ARG(ws_bytes >= need, "ev_loudness: workspace of %zu bytes, %zu needed", ws_bytes, need);
   EV_TRY(use_device_of(wav));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int S = sample_rate / 10;
   const long long max_sub = loud_max_sub(item_stride, sample_rate);
+  EV_CHECK_ARG(loud_grid_ok(item_stride, sample_rate), "ev_loudness: item_stride=%lld is too long", item_stride);
   double* energy = static_cast<double*>(ws);
   float* pks = reinterpret_cast<float*>(energy + (size_t)n_items * max_sub);
-  KCoef c;
-  c.s0 = (float)kcoef[0]; c.s1 = (float)kcoef[1]; c.s2 = (float)kcoef[2]; c.sa1 = (float)kcoef[3]; c.sa2 = (float)kcoef[4];
-  c.h0 = (float)kcoef[5]; c.h1 = (float)kcoef[6]; c.h2 = (float)kcoef[7]; c.ha1 = (float)kcoef[8]; c.ha2 = (float)kcoef[9];
-  const long long gx = (max_sub + LD_THREADS - 1) / LD_THREADS;
-  EV_CHECK_ARG(gx <= 0x7fffffffll, "ev_loudness: item_stride=%lld is too long", item_stride);
-  EV_TRY(launch("loud_subblock_kernel", loud_subblock_kernel, dim3((unsigned)gx, n_items), LD_THREADS, 0, st, wav, item_stride, n_in,
-                items, S, W, max_sub, c, energy, pks));
-  return launch("loud_gate_kernel", loud_gate_kernel, dim3(n_items), LG_THREADS, 0, st, item_stride, n_in, items, S, max_sub,
-                (const double*)energy, (const float*)pks, (double)target_lufs, lufs, peak, gain);
+  EV_TRY(launch_loud_subblock(wav, item_stride, nullptr, n_in, items, n_items, sample_rate, kcoef, W, energy, pks, st));
+  return launch_loud_gate(item_stride, n_in, items, n_items, sample_rate, energy, pks, (double)target_lufs, lufs, peak, gain, st);
 }
 
 }  // extern "C"

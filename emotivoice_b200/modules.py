@@ -25,6 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import _abi, audio, output, packing, synth
+from .loudness import check_rate as check_meter_rate
 
 
 class _Holder(nn.Module):
@@ -791,6 +792,27 @@ class JETSGenerator(_EngineOwner):
         wav, n_in, items, eng = self._outputs(out, items, hop)
         with eng.call_lock:
             return eng.output.measure(wav, n_in, items, int(getattr(self.config, "sr", 16000)))
+
+    @torch.no_grad()
+    def meter(self, out, sample_rate=None, items=None, hop=None, loudness=None, true_peak=None, watermark=None, series=False):
+        """The loudness meter (EBU R128; ``emotivoice_b200.loudness`` holds the definitions) of exactly what
+        ``format_audio(out, sample_rate, "float32", items, hop, loudness, true_peak, watermark)`` delivers: the chain's float32
+        stage runs as it would there, then ``ev_meter`` reads its packed outputs in place, at the output rate.  Lets a server
+        check the integrated loudness, true peak, maximum momentary and short-term loudness and loudness range of its
+        responses.  The output rate must also be a multiple of 10 Hz (100 ms sub-blocks).  ``series``: also return the
+        momentary and short-term series.
+
+        Returns a ``loudness.Meter`` of device tensors, one value per listed output.  No sync; invalid arguments raise
+        ValueError before anything is enqueued."""
+        sr = int(getattr(self.config, "sr", 16000))
+        fmt = audio.output_format(sample_rate, "float32", loudness, true_peak, sr, watermark=watermark)
+        check_meter_rate(fmt.rate)
+        if not isinstance(series, (bool, np.bool_)):
+            raise ValueError("series must be True or False, got %r" % (series,))
+        wav, n_in, items, eng = self._outputs(out, items, hop)
+        with eng.call_lock:
+            packed, offs = eng.output.format(wav, n_in, items, fmt, sr)
+            return eng.output.meter(packed, offs, fmt.rate, bool(series))
 
     @torch.no_grad()
     def format_audio(self, out, sample_rate=None, encoding="pcm16", items=None, hop=None, loudness=None, true_peak=None,

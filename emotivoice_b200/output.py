@@ -1,11 +1,12 @@
 """The output chain of one engine: the watermark (ev_watermark_embed), loudness measurement (ev_loudness), true-peak limiting
 (ev_limit), resampling and encoding (ev_format_audio) and FLAC (ev_flac_encode) of a forward's outputs, in that order, with
-the filter banks and coefficients those stages read.  ``JETSGenerator.format_audio`` / ``measure_loudness`` validate their arguments and call it under the engine's lock.
+the filter banks and coefficients those stages read, and the loudness meter (ev_meter) of what it delivers.
+``JETSGenerator.format_audio`` / ``measure_loudness`` / ``meter`` validate their arguments and call it under the engine's lock.
 """
 import numpy as np
 import torch
 
-from . import _abi, audio
+from . import _abi, audio, loudness
 
 _DTYPES = {"float32": torch.float32, "pcm16": torch.int16, "mulaw": torch.uint8, "alaw": torch.uint8}
 
@@ -33,11 +34,15 @@ class Chain:
             p += 8 * len(a)
         return meta, ptrs
 
-    def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
-        """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
+    def _k_weighting(self, sr):
         kc = self._kcoef.get(sr)
         if kc is None:
             kc = self._kcoef[sr] = np.ascontiguousarray(audio.k_weighting(sr))
+        return kc
+
+    def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
+        """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
+        kc = self._k_weighting(sr)
         res = torch.empty((3, k), dtype=torch.float32, device=self.device)
         stride = int(wav.stride(0))
         ws = self._ws("loudness", self.lib.ev_loudness_workspace_bytes(k, stride, sr))
@@ -68,6 +73,17 @@ class Chain:
         meta, (p_n, p_items) = self._meta([n_in, items])
         lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
         return lufs, pk
+
+    def meter(self, packed, offs, rate, series):
+        """ev_meter of the outputs ``format`` packed as float32 at ``rate`` Hz (a multiple of 10), output k at
+        packed[offs[k]:offs[k + 1]] -> ``loudness.Meter``.  No sync."""
+        lens = np.diff(offs).tolist()
+        meta, (p_meta,) = self._meta([np.concatenate([offs[:-1], lens])])
+        if packed.numel() == 0:                  # every output is empty: ev_meter reads no sample, but needs an address
+            packed = torch.empty((1,), dtype=torch.float32, device=self.device)
+        return loudness.enqueue(self.lib, packed.data_ptr(), p_meta, lens, rate, self.device, self._stream(),
+                                lambda nb: self._ws("meter", nb), series, loudness.detector_bank(rate, self.device),
+                                self._k_weighting(rate))
 
     def format(self, wav, n_in, items, fmt, sr):
         """The listed items of a (B,1,L) fp32 waveform at ``sr`` Hz, host valid samples ``n_in`` (B ints <= L), in the

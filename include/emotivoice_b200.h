@@ -294,6 +294,34 @@ EV_API int ev_limit(const float* wav, long long item_stride, const int64_t* n_in
                     int taps, int lookahead, int hold, double release_db_per_sample, float* out, long long out_stride, void* ws,
                     size_t ws_bytes, void* stream);
 
+/* Loudness meter (EBU R128: ITU-R BS.1770-4 and EBU Tech 3342, one channel) of waveform items, for checking what a server
+ * delivers and measuring recordings: item k is the n[k] samples at wav + start[k] (start, n: (n_items) i64 DEVICE arrays, so a
+ * (B, L) batch and ev_format_audio's packed EV_AUDIO_FLOAT32 outputs are both read in place), n_host (n_items) i64 HOST array
+ * of the same counts (>= 0; it sizes the grid, the workspace and the series; a device count is clamped to the largest of them).
+ * 1 <= n_items <= 65535.  sample_rate: a multiple of 10 in [4000, 192000]; kcoef: as ev_loudness (HOST, 10 doubles).
+ *   Sub-blocks: ev_loudness's, 100 ms of S = sample_rate / 10 samples, K-weighted, sum of squares e[j]; only the n / S full
+ *   ones count.  Loudness of a mean square z: -0.691 + 10 log10(z).
+ *   momentary M[j] of (((e[j] + e[j+1]) + e[j+2]) + e[j+3]) / (4 S), j < n / S - 3: ev_loudness's gating blocks, ungated (10 Hz).
+ *   short-term S[j] of (e[j] + ... + e[j+29], left to right) / (30 S), j < n / S - 29 (3 s windows, 10 Hz).
+ *   LRA (EBU Tech 3342): the short-term values S > -70; of those the values S > 10 log10(mean of 10^(S/10)) - 20 (the mean
+ *   taken over the mean squares in fp64, in a fixed order); of the m left, sorted ascending, v[round(0.95 (m - 1))] -
+ *   v[round(0.10 (m - 1))], round half away from zero, each v the exact element (a radix select); NaN when m = 0.
+ *   True peak: 20 log10 of max p[s] over the item, p ev_limit's detector (max of |x[s]| and |sum_j bank[ph][j] x[s + c - j]|,
+ *   c = (taps - 1) / 2, x zero outside [0, n)) with bank (phases, taps) f32 device array, taps odd: emotivoice_b200.audio.
+ *   true_peak_bank(sample_rate), all R = ceil(192000 / sample_rate) phases of the limiter's interpolator, so p reads exactly
+ *   scipy.signal.resample_poly(x, R, 1) and |x|; phases may be 0 (bank NULL; 192 kHz).
+ *   results (6, n_items) f32 device, row r for item k at results[r * n_items + k]: 0 integrated loudness I (bitwise
+ *   ev_loudness's lufs), 1 LRA (LU), 2 max M, 3 max S (-inf for an empty or silent series), 4 true peak (dBTP, -inf for
+ *   silence), 5 sample peak max |x| (linear, ev_loudness's peak).
+ *   momentary / short_term: NULL, or (n_items, series_stride) f32 device arrays, series_stride >= (max n_host) / S: row k holds
+ *   M (S) of item k, then NaN to the end of the row.
+ *   ws: ev_meter_workspace_bytes(n_items, max n_host, sample_rate) bytes.  Four launches; each item's results are bitwise the
+ *   same in any batch or order.  No allocation, no sync. */
+EV_API size_t ev_meter_workspace_bytes(int n_items, long long max_n, int sample_rate);   /* 0 for arguments out of range */
+EV_API int ev_meter(const float* wav, const int64_t* start, const int64_t* n, const int64_t* n_host, int n_items, int sample_rate,
+                    const double* kcoef, const float* bank, int phases, int taps, float* results, float* momentary, float* short_term,
+                    long long series_stride, void* ws, size_t ws_bytes, void* stream);
+
 /* FLAC (RFC 9639) file images of int16 items, the lossless compressed response of a TTS server: item k is pcm[pcm_off[k] ..
  * pcm_off[k + 1]) (pcm_off (n_items + 1) i64 DEVICE array, items packed back to back as ev_format_audio writes EV_AUDIO_PCM16),
  * n_samples (n_items) i64 HOST array of the same counts (each in [1, 2^36]; it sizes the grid and the checks below).
