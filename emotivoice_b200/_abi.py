@@ -74,6 +74,9 @@ SIGNATURES = {
                       ctypes.c_longlong, _vp, _sz, _vp]),
     "ev_meter_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i]),
     "ev_meter": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, ctypes.c_longlong, _vp, _sz, _vp]),
+    "ev_eval_workspace_bytes": (_sz, [_i, _i, _i]),
+    "ev_eval_compare": (_i, [_vp, _vp, ctypes.c_longlong, _vp, _i, _vp, _vp, ctypes.c_longlong, _vp, _i, _i, _vp, _vp, _vp, _vp,
+                             ctypes.c_longlong, _vp, _sz, _vp]),
     "ev_flac_bound_bytes": (_sz, [ctypes.c_longlong]),
     "ev_flac_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
     "ev_flac_encode": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _vp, _sz, _vp]),

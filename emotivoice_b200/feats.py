@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _abi
+from . import _abi, audio
 
 N_FFT = 1024
 _MAX_MELS = 128
@@ -112,6 +112,16 @@ _DEV_CACHE = {}
 _BANDS = {}      # mel_spectrogram_torch's band tables per (sampling_rate, num_mels, fmin, fmax, device), like its mel_basis dict
 
 
+def device_ints(values, dev):
+    """Host integers -> a device int64 tensor through pinned memory, without a sync."""
+    return torch.tensor(values, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+
+
+def upload(a, dev):
+    """A host array -> a device tensor through pinned memory, without a sync."""
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+
+
 def _on_device(key, make, dev):
     k = (key, str(dev))
     t = _DEV_CACHE.get(k)
@@ -189,7 +199,7 @@ def stft_features(y, pad, hop, window, mag_eps, bands=None, energy=False, length
         mel = torch.empty((B, n_mels, F), dtype=torch.float32, device=dev)
     if energy:
         out_e = torch.empty((B, F), dtype=torch.float32, device=dev)
-    ns = None if lengths is None else torch.tensor(ls, dtype=torch.int64).to(dev)
+    ns = None if lengths is None else device_ints(ls, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev) if check_range else None
     win = window.detach().to(device=dev, dtype=torch.float32).contiguous()
     tw = _on_device("twiddles", twiddles, dev)
@@ -199,6 +209,23 @@ def stft_features(y, pad, hop, window, mag_eps, bands=None, energy=False, length
                                     None if out_e is None else out_e.data_ptr(), None if status is None else status.data_ptr(),
                                     torch.cuda.current_stream(dev).cuda_stream))
     return mel, out_e, status
+
+
+def resample(wav, lens, rate, target):
+    """Contiguous CUDA (B, L) float32 recordings at ``rate`` -> ((B, L') float32 at ``target`` Hz, the lengths at ``target``),
+    through ev_format_audio's float32 path: each row's valid samples resampled as ``scipy.signal.resample_poly`` does.  The
+    rates must be ones ``audio.plan`` accepts; a row is not written past its own valid samples.  No sync."""
+    _, up, down = audio.plan(target, "float32", rate)
+    B, L = wav.shape
+    dev = wav.device
+    lens_out = [audio.resampled_length(n, up, down) for n in lens]
+    out = torch.empty((B, audio.resampled_length(L, up, down)), dtype=torch.float32, device=dev)
+    meta = device_ints(list(lens) + [b * out.stride(0) for b in range(B)], dev)  # n_in, then where each row starts in out
+    bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev, non_blocking=True)
+    _abi.check(_abi.load().ev_format_audio(wav.data_ptr(), int(wav.stride(0)), meta.data_ptr(), None, B, meta.data_ptr() + 8 * B,
+                                           bank.data_ptr(), up, down, int(bank.shape[1]), audio.ENCODINGS["float32"], out.data_ptr(),
+                                           None, torch.cuda.current_stream(dev).cuda_stream))
+    return out, lens_out
 
 
 class TacotronSTFT(nn.Module):
@@ -359,7 +386,7 @@ def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=Fals
     if nbytes == 0:
         raise ValueError("ev_pitch rejects B=%d N=%d sr=%d hop=%d" % (B, N, int(sr), int(hop)))
     ws = torch.empty((nbytes + 15) // 16 * 2, dtype=torch.float64, device=dev)
-    ns = None if lengths is None else torch.tensor(ls, dtype=torch.int64).to(dev)
+    ns = None if lengths is None else device_ints(ls, dev)
     out = torch.empty((B, F), dtype=torch.float64, device=dev)
     f0 = torch.empty((B, F), dtype=torch.float64, device=dev) if raw else None
     flags = (_PITCH_CONTINUOUS if continuous else 0) | (_PITCH_LOG if log else 0)

@@ -23,30 +23,10 @@ Silence (every cell M = 0) gives z = 0.
 """
 import torch
 
-from . import _abi, audio
+from . import _abi, audio, feats
 
 DETECT_Z = audio.WATERMARK_DETECT_Z
 SR = 16000
-
-
-def _to_device(values, dev):
-    """Host integers -> a device int64 tensor through pinned memory, without a sync."""
-    return torch.tensor(values, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
-
-
-def _resample_to_16k(wav, lens, rate, dev, lib):
-    """The (B, L) recordings at ``rate`` -> (B, L16) float32 at 16 kHz through ev_format_audio's float32 path (each row's
-    valid samples resampled as ``scipy.signal.resample_poly`` does), and the lengths at 16 kHz."""
-    _, up, down = audio.plan(SR, "float32", rate)
-    B, L = wav.shape
-    lens16 = [audio.resampled_length(n, up, down) for n in lens]
-    out = torch.empty((B, audio.resampled_length(L, up, down)), dtype=torch.float32, device=dev)
-    meta = _to_device(lens + [b * out.stride(0) for b in range(B)], dev)        # n_in, then where each row starts in out
-    bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev, non_blocking=True)
-    _abi.check(lib.ev_format_audio(wav.data_ptr(), int(wav.stride(0)), meta.data_ptr(), None, B, meta.data_ptr() + 8 * B,
-                                   bank.data_ptr(), up, down, int(bank.shape[1]), audio.ENCODINGS["float32"], out.data_ptr(),
-                                   None, torch.cuda.current_stream(dev).cuda_stream))
-    return out, lens16
 
 
 @torch.no_grad()
@@ -84,8 +64,8 @@ def detect(wav, sample_rate, key, lengths=None):
     dev = wav.device
     wav = wav.contiguous()
     if rate != SR:
-        wav, lens = _resample_to_16k(wav, lens, rate, dev, lib)
-    n = _to_device(lens, dev)
+        wav, lens = feats.resample(wav, lens, rate, SR)
+    n = feats.device_ints(lens, dev)
     z = torch.empty((B,), dtype=torch.float32, device=dev)
     offset = torch.empty((B,), dtype=torch.int32, device=dev)
     phase = torch.empty((B,), dtype=torch.int32, device=dev)

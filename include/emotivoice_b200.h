@@ -365,6 +365,31 @@ EV_API size_t ev_watermark_detect_workspace_bytes(int n_items);                 
 EV_API int ev_watermark_detect(const float* wav, long long item_stride, const int64_t* n, int n_items, uint64_t key, float* z,
                                int32_t* offset, int32_t* phase, void* ws, size_t ws_bytes, void* stream);
 
+/* Objective comparison of syntheses with recordings: cepstral distance after dynamic time warping (DTW), F0 error and voicing
+ * error along the warping path.  Pair k compares N = n_syn[k] syn frames with M = n_ref[k] ref frames (n_syn, n_ref: (n_items)
+ * i32 DEVICE arrays, clamped to [1, max_n] and [1, max_m]; max_n, max_m in [1, 4096] are HOST maxima, they size the grid and
+ * the workspace).  1 <= n_items <= 65535.
+ *   mel_syn (n_items, 80, syn_frames) f32 log-mels (ln of the mel magnitude), f0_syn (n_items, syn_frames) f64 F0 in Hz, 0 or
+ *   less for unvoiced; syn_frames >= max_n; likewise mel_ref, f0_ref, ref_frames >= max_m.  Frames past a pair's N and M are
+ *   never read.  table (24, 80) f64 DEVICE: row k - 1 holds cos(pi k (m + 1/2) / 80), m = 0..79.
+ *   c_k[f] = (sum_m fp64(L[m, f]) * table[k - 1][m], ascending m) / 80, k = 1..24; d(i, j) = sqrt(sum_k (c_k[i] - c'_k[j])^2),
+ *   ascending k; every product, sum, difference, quotient and square root rounded on its own (no FMA).
+ *   D(0,0) = d(0,0), D(i,j) = d(i,j) + min(D(i-1,j-1), D(i-1,j), D(i,j-1)) over the predecessors that exist, ties to the
+ *   first in that order; the path: the backtrack from (N-1, M-1) to (0,0), P pairs, max(N, M) <= P <= N + M - 1.
+ *   stats (3, n_items) f64 DEVICE, row r for pair k at stats[r * n_items + k]: 0 mcd = (10 sqrt(2) / ln 10) (D(N-1, M-1) / P)
+ *   in dB (D(N-1, M-1) is the sum of d along the path in path order); 1 f0_rmse = sqrt(E / V) in cents, E the sum in path
+ *   order of (1200 log2(f_syn / f_ref))^2 over the V pairs voiced on both sides (NaN when V = 0); 2 vuv_error = (pairs whose
+ *   voicing differs) / P.  counts (2, n_items) i32 DEVICE: 0 V, 1 P.
+ *   path: NULL, or (n_items, path_stride, 2) i32 DEVICE, path_stride >= max_n + max_m - 1: row k holds the P pairs (syn frame,
+ *   ref frame) from (0,0), then -1 to the end of the row.
+ *   ws: ev_eval_workspace_bytes(n_items, max_n, max_m) bytes (9 max_n max_m bytes per pair, plus the cepstra).  Three launches;
+ *   each pair's results are bitwise the same in any batch or order.  No allocation, no sync. */
+EV_API size_t ev_eval_workspace_bytes(int n_items, int max_n, int max_m);            /* 0 for arguments out of range */
+EV_API int ev_eval_compare(const float* mel_syn, const double* f0_syn, long long syn_frames, const int32_t* n_syn, int max_n,
+                           const float* mel_ref, const double* f0_ref, long long ref_frames, const int32_t* n_ref, int max_m,
+                           int n_items, const double* table, double* stats, int32_t* counts, int32_t* path, long long path_stride,
+                           void* ws, size_t ws_bytes, void* stream);
+
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
 EV_API uint64_t ev_launch_count(void);
