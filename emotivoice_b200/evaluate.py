@@ -45,7 +45,7 @@ import collections
 import numpy as np
 import torch
 
-from . import _abi, audio, feats
+from . import _abi, audio, feats, recordings
 
 SR = 16000
 HOP = 256
@@ -60,9 +60,6 @@ Comparison.__doc__ = """Per-pair results of ``compare`` (device tensors of shape
 each pair's own path, P_max = max(N) + max(M) - 1 over the batch (the longest synthesis and the longest recording may be in
 different rows); None unless asked for."""
 
-_STFT = {}                      # device -> (window, bands) of TacotronSTFT(1024, 256, 1024, 80, 16000, 0, 8000)
-_TABLE = {}                     # device -> the (24, 80) cosine table
-
 
 def cos_table():
     """(24, 80) float64: row k - 1 holds cos(pi k (m + 1/2) / 80), m = 0..79."""
@@ -71,47 +68,11 @@ def cos_table():
     return np.cos(np.pi * k * (m + 0.5) / N_MELS)
 
 
-def _device_table(dev):
-    key = str(dev)
-    if key not in _TABLE:
-        _TABLE[key] = feats.upload(cos_table(), dev)
-    return _TABLE[key]
-
-
-def _stft(dev):
-    key = str(dev)
-    if key not in _STFT:
-        stft = feats.TacotronSTFT(1024, HOP, 1024, N_MELS, SR, 0.0, 8000.0)
-        bands, weights = feats.band_table(stft.mel_basis.numpy())
-        _STFT[key] = (feats.upload(stft.window.numpy(), dev), (feats.upload(bands, dev), feats.upload(weights, dev)))
-    return _STFT[key]
-
-
-def _check_wav(x, name):
-    if not (isinstance(x, torch.Tensor) and x.dim() == 2 and x.dtype == torch.float32 and x.is_cuda):
-        raise ValueError("%s must be a CUDA (B, L) float32 tensor" % name)
-    if not 1 <= x.shape[0] <= 65535 or x.shape[1] < 1:
-        raise ValueError("%s must hold 1 to 65535 recordings of at least one sample, got shape %s" % (name, tuple(x.shape)))
-
-
-def _check_lengths(lengths, B, L, name):
-    if lengths is None:
-        return [L] * B
-    if torch.is_tensor(lengths):
-        if lengths.device.type != "cpu":
-            raise ValueError("%s must be host integers (a sequence or a CPU tensor)" % name)
-        lengths = lengths.tolist()
-    if isinstance(lengths, (str, bytes)) or any(isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) for v in lengths):
-        raise ValueError("%s must be %d integers in [0, %d], got %r" % (name, B, L, lengths))
-    lens = [int(v) for v in lengths]
-    if len(lens) != B or any(n < 0 or n > L for n in lens):
-        raise ValueError("%s must be %d integers in [0, %d], got %s" % (name, B, L, lens))
-    return lens
-
-
 def _features(wav, lens):
-    """16 kHz (B, L) items -> (log-mel (B, 80, F) float32, F0 (B, F) float64), frames per item n // 256 + 1."""
-    window, bands = _stft(wav.device)
+    """16 kHz (B, L) items -> (log-mel (B, 80, F) float32, F0 (B, F) float64), frames per item n // 256 + 1: the mel of
+    TacotronSTFT(1024, 256, 1024, 80, 16000, 0, 8000) without its range check."""
+    bands = feats.mel_bands(SR, N_MELS, 0.0, 8000.0, wav.device)
+    window = feats.scipy_hann(wav.device)
     mel, _, _ = feats.stft_features(wav, 1024 // 2, HOP, window, 0.0, bands=bands, lengths=lens, check_range=False)
     f0 = feats.pitch_track(wav, SR, HOP, continuous=False, lengths=lens)
     assert mel.shape[2] == f0.shape[1] == wav.shape[1] // HOP + 1, (tuple(mel.shape), tuple(f0.shape))
@@ -131,16 +92,16 @@ def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, ret
     Returns a ``Comparison`` of device tensors, with no host sync.  The workspace grows with B max(N) max(M): batch long
     test sets in chunks of similar lengths (module docstring).  Invalid arguments raise ValueError before anything is
     enqueued."""
-    _check_wav(syn, "syn")
-    _check_wav(ref, "ref")
+    syn = recordings.recording_batch(syn, "syn")
+    ref = recordings.recording_batch(ref, "ref")
     B = int(syn.shape[0])
     if int(ref.shape[0]) != B:
         raise ValueError("syn and ref must hold the same number of recordings, got %d and %d" % (B, int(ref.shape[0])))
     if syn.device != ref.device:
         raise ValueError("syn and ref must be on the same device")
     rate, up, down = audio.plan(sample_rate, "float32", SR)
-    ls = _check_lengths(syn_lengths, B, int(syn.shape[1]), "syn_lengths")
-    lr = _check_lengths(ref_lengths, B, int(ref.shape[1]), "ref_lengths")
+    ls = recordings.host_lengths(syn_lengths, B, int(syn.shape[1]), "syn_lengths")
+    lr = recordings.host_lengths(ref_lengths, B, int(ref.shape[1]), "ref_lengths")
     if rate != SR:                                # up / down take 16 kHz to the rate, so the way back is down / up
         ls16 = [audio.resampled_length(n, down, up) for n in ls]
         lr16 = [audio.resampled_length(n, down, up) for n in lr]
@@ -155,16 +116,15 @@ def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, ret
         raise ValueError("return_path must be True or False, got %r" % (return_path,))
     lib = _abi.load()
     dev = syn.device
-    syn, ref = syn.contiguous(), ref.contiguous()
     if rate != SR:
-        syn, ls = feats.resample(syn, ls, rate, SR)
-        ref, lr = feats.resample(ref, lr, rate, SR)
+        syn, ls = recordings.resample(syn, ls, rate, SR)
+        ref, lr = recordings.resample(ref, lr, rate, SR)
     assert ls == ls16 and lr == lr16
     mel_s, f0_s = _features(syn, ls)
     mel_r, f0_r = _features(ref, lr)
     ns = [n // HOP + 1 for n in ls]
     nr = [n // HOP + 1 for n in lr]
-    counts_in = torch.tensor(ns + nr, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    counts_in, (p_ns, p_nr) = recordings.upload([ns, nr], dev, np.int32)
     max_n, max_m = max(ns), max(nr)
     stats = torch.empty((3, B), dtype=torch.float64, device=dev)
     counts = torch.empty((2, B), dtype=torch.int32, device=dev)
@@ -172,9 +132,10 @@ def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, ret
     path = torch.empty((B, p_max, 2), dtype=torch.int32, device=dev) if return_path else None
     nb = int(lib.ev_eval_workspace_bytes(B, max_n, max_m))
     ws = torch.empty((nb,), dtype=torch.uint8, device=dev)
-    _abi.check(lib.ev_eval_compare(mel_s.data_ptr(), f0_s.data_ptr(), int(mel_s.shape[2]), counts_in.data_ptr(), max_n,
-                                   mel_r.data_ptr(), f0_r.data_ptr(), int(mel_r.shape[2]), counts_in.data_ptr() + 4 * B, max_m, B,
-                                   _device_table(dev).data_ptr(), stats.data_ptr(), counts.data_ptr(),
+    table = recordings.device_table("cos_table", cos_table, dev)
+    _abi.check(lib.ev_eval_compare(mel_s.data_ptr(), f0_s.data_ptr(), int(mel_s.shape[2]), p_ns, max_n,
+                                   mel_r.data_ptr(), f0_r.data_ptr(), int(mel_r.shape[2]), p_nr, max_m, B,
+                                   table.data_ptr(), stats.data_ptr(), counts.data_ptr(),
                                    None if path is None else path.data_ptr(), p_max, ws.data_ptr(), nb,
                                    torch.cuda.current_stream(dev).cuda_stream))
     return Comparison(stats[0], stats[1], stats[2], counts[0], counts[1], path)

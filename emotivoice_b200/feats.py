@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _abi, audio
+from . import _abi, recordings
 
 N_FFT = 1024
 _MAX_MELS = 128
@@ -108,29 +108,6 @@ def twiddles():
     return np.stack([np.cos(a), -np.sin(a)], axis=1).astype(np.float32)
 
 
-_DEV_CACHE = {}
-_BANDS = {}      # mel_spectrogram_torch's band tables per (sampling_rate, num_mels, fmin, fmax, device), like its mel_basis dict
-
-
-def device_ints(values, dev):
-    """Host integers -> a device int64 tensor through pinned memory, without a sync."""
-    return torch.tensor(values, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
-
-
-def upload(a, dev):
-    """A host array -> a device tensor through pinned memory, without a sync."""
-    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
-
-
-def _on_device(key, make, dev):
-    k = (key, str(dev))
-    t = _DEV_CACHE.get(k)
-    if t is None:
-        t = torch.from_numpy(np.ascontiguousarray(make())).to(dev)
-        _DEV_CACHE[k] = t
-    return t
-
-
 def n_frames(n, pad, hop):
     """Frames of an n-sample item reflect-padded by pad at both ends (conv1d / stft with center=False)."""
     return (int(n) + 2 * int(pad) - N_FFT) // int(hop) + 1
@@ -148,20 +125,8 @@ def _check_fft(n_fft, win_length):
 
 
 def _lengths(y, lengths, pad):
-    """Host item lengths (a sequence or a CPU tensor; None: every row is N samples), checked like F.pad(reflect) would."""
-    B, N = y.shape
-    if lengths is None:
-        ls = [N] * B
-    else:
-        if torch.is_tensor(lengths):
-            if lengths.device.type != "cpu":
-                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
-            lengths = lengths.tolist()
-        ls = [int(v) for v in lengths]
-        if len(ls) != B:
-            raise ValueError("%d lengths for %d items" % (len(ls), B))
-        if any(v > N for v in ls):
-            raise ValueError("a length exceeds the %d samples of a row" % N)
+    """Host item lengths (``recordings.host_lengths``), checked like F.pad(reflect) would."""
+    ls = recordings.host_lengths(lengths, *y.shape)
     for v in ls:
         if v <= pad:
             raise RuntimeError("an item of %d samples is not longer than the reflect padding %d" % (v, pad))
@@ -170,12 +135,30 @@ def _lengths(y, lengths, pad):
     return ls
 
 
-def device_bands(basis, dev):
-    """band_table of a dense basis as device tensors (bands, weights)."""
-    bt, bw = band_table(basis.detach().cpu().numpy() if torch.is_tensor(basis) else basis)
+def _checked_band_table(basis):
+    bt, bw = band_table(basis)
     if bt.shape[0] > _MAX_MELS:
         raise ValueError("%d mel bands are not supported: at most %d" % (bt.shape[0], _MAX_MELS))
+    return bt, bw
+
+
+def device_bands(basis, dev):
+    """band_table of a dense basis as device tensors (bands, weights)."""
+    bt, bw = _checked_band_table(basis.detach().cpu().numpy() if torch.is_tensor(basis) else basis)
     return torch.from_numpy(bt).to(dev), torch.from_numpy(bw).to(dev)
+
+
+def mel_bands(sampling_rate, num_mels, fmin, fmax, dev):
+    """device_bands of mel_filterbank(sampling_rate, 1024, num_mels, fmin, fmax), made once per device like the reference's
+    mel_basis dict."""
+    key = ("mel_bands", int(sampling_rate), int(num_mels), float(fmin), None if fmax is None else float(fmax))
+    return recordings.device_table(key, lambda: _checked_band_table(
+        mel_filterbank(sr=sampling_rate, n_fft=N_FFT, n_mels=num_mels, fmin=fmin, fmax=fmax)), dev)
+
+
+def scipy_hann(dev):
+    """hann_window_scipy() on dev, made once per device."""
+    return recordings.device_table("scipy_hann", hann_window_scipy, dev)
 
 
 def stft_features(y, pad, hop, window, mag_eps, bands=None, energy=False, lengths=None, check_range=False):
@@ -199,33 +182,16 @@ def stft_features(y, pad, hop, window, mag_eps, bands=None, energy=False, length
         mel = torch.empty((B, n_mels, F), dtype=torch.float32, device=dev)
     if energy:
         out_e = torch.empty((B, F), dtype=torch.float32, device=dev)
-    ns = None if lengths is None else device_ints(ls, dev)
+    ns = None if lengths is None else recordings.upload([ls], dev)[0]
     status = torch.zeros(1, dtype=torch.int32, device=dev) if check_range else None
     win = window.detach().to(device=dev, dtype=torch.float32).contiguous()
-    tw = _on_device("twiddles", twiddles, dev)
+    tw = recordings.device_table("twiddles", twiddles, dev)
     _abi.check(lib.ev_stft_features(x.data_ptr(), N, None if ns is None else ns.data_ptr(), B, int(pad), int(hop), F, win.data_ptr(),
                                     tw.data_ptr(), float(mag_eps), None if bands is None else bands.data_ptr(),
                                     None if band_w is None else band_w.data_ptr(), n_mels, None if mel is None else mel.data_ptr(),
                                     None if out_e is None else out_e.data_ptr(), None if status is None else status.data_ptr(),
                                     torch.cuda.current_stream(dev).cuda_stream))
     return mel, out_e, status
-
-
-def resample(wav, lens, rate, target):
-    """Contiguous CUDA (B, L) float32 recordings at ``rate`` -> ((B, L') float32 at ``target`` Hz, the lengths at ``target``),
-    through ev_format_audio's float32 path: each row's valid samples resampled as ``scipy.signal.resample_poly`` does.  The
-    rates must be ones ``audio.plan`` accepts; a row is not written past its own valid samples.  No sync."""
-    _, up, down = audio.plan(target, "float32", rate)
-    B, L = wav.shape
-    dev = wav.device
-    lens_out = [audio.resampled_length(n, up, down) for n in lens]
-    out = torch.empty((B, audio.resampled_length(L, up, down)), dtype=torch.float32, device=dev)
-    meta = device_ints(list(lens) + [b * out.stride(0) for b in range(B)], dev)  # n_in, then where each row starts in out
-    bank = torch.from_numpy(audio.polyphase_bank(up, down)).to(dev, non_blocking=True)
-    _abi.check(_abi.load().ev_format_audio(wav.data_ptr(), int(wav.stride(0)), meta.data_ptr(), None, B, meta.data_ptr() + 8 * B,
-                                           bank.data_ptr(), up, down, int(bank.shape[1]), audio.ENCODINGS["float32"], out.data_ptr(),
-                                           None, torch.cuda.current_stream(dev).cuda_stream))
-    return out, lens_out
 
 
 class TacotronSTFT(nn.Module):
@@ -268,11 +234,8 @@ def mel_spectrogram_torch(y, n_fft, num_mels, sampling_rate, hop_size, win_size,
     if center:
         raise ValueError("mel_spectrogram_torch: center=True is not supported, only the reference's center=False")
     dev = y.device
-    key = (int(sampling_rate), int(num_mels), float(fmin), None if fmax is None else float(fmax), str(dev))
-    bands = _BANDS.get(key)
-    if bands is None:
-        bands = _BANDS[key] = device_bands(mel_filterbank(sr=sampling_rate, n_fft=n_fft, n_mels=num_mels, fmin=fmin, fmax=fmax), dev)
-    window = _on_device("torch_hann", lambda: torch.hann_window(N_FFT).numpy(), dev)
+    bands = mel_bands(sampling_rate, num_mels, fmin, fmax, dev)
+    window = recordings.device_table("torch_hann", lambda: torch.hann_window(N_FFT).numpy(), dev)
     mel, _, _ = stft_features(y, (N_FFT - int(hop_size)) // 2, hop_size, window, 1e-6, bands=bands, lengths=lengths)
     return mel
 
@@ -300,9 +263,7 @@ class Energy:
             raise ValueError("pad_mode %r is not supported: only 'reflect'" % (pad_mode,))
 
     def _calculate_energy(self, wav, lengths=None):
-        dev = wav.device
-        window = _on_device("scipy_hann", hann_window_scipy, dev)
-        _, e, _ = stft_features(wav, N_FFT // 2, self.hop_length, window, 0.0, energy=True, lengths=lengths)
+        _, e, _ = stft_features(wav, N_FFT // 2, self.hop_length, scipy_hann(wav.device), 0.0, energy=True, lengths=lengths)
         return e
 
     def get_energy(self, wav, use_token_averaged_energy=True, duration=None, lengths=None):
@@ -362,18 +323,7 @@ def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=Fals
     if wav.dtype not in (torch.float32, torch.float64):
         raise ValueError("wav must be float32 or float64, got %s" % wav.dtype)
     B, N = wav.shape
-    if lengths is None:
-        ls = [N] * B
-    else:
-        if torch.is_tensor(lengths):
-            if lengths.device.type != "cpu":
-                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
-            lengths = lengths.tolist()
-        ls = [int(v) for v in lengths]
-        if len(ls) != B:
-            raise ValueError("%d lengths for %d items" % (len(ls), B))
-        if any(v > N for v in ls):
-            raise ValueError("a length exceeds the %d samples of a row" % N)
+    ls = recordings.host_lengths(lengths, B, N)
     m = pitch_min_samples(sr)
     if any(v < m for v in ls):
         raise ValueError("an item of %d samples is too short to filter: at least %d at %d Hz" % (min(ls), m, int(sr)))
@@ -386,7 +336,7 @@ def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=Fals
     if nbytes == 0:
         raise ValueError("ev_pitch rejects B=%d N=%d sr=%d hop=%d" % (B, N, int(sr), int(hop)))
     ws = torch.empty((nbytes + 15) // 16 * 2, dtype=torch.float64, device=dev)
-    ns = None if lengths is None else device_ints(ls, dev)
+    ns = None if lengths is None else recordings.upload([ls], dev)[0]
     out = torch.empty((B, F), dtype=torch.float64, device=dev)
     f0 = torch.empty((B, F), dtype=torch.float64, device=dev) if raw else None
     flags = (_PITCH_CONTINUOUS if continuous else 0) | (_PITCH_LOG if log else 0)

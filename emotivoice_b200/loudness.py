@@ -30,14 +30,12 @@ import collections
 import numpy as np
 import torch
 
-from . import _abi, audio
+from . import _abi, audio, recordings
 
 Meter = collections.namedtuple("Meter", "integrated loudness_range max_momentary max_short_term true_peak sample_peak momentary short_term")
 Meter.__doc__ = """Per-recording results of ``meter`` (device float32 tensors of shape (B,)): integrated (LUFS), loudness_range
 (LU), max_momentary and max_short_term (LUFS), true_peak (dBTP), sample_peak (linear); momentary and short_term: (B, K)
 series at 10 Hz when asked for (row b holds NaN past its own values), else None."""
-
-_banks = {}                     # (device, rate) -> device detector bank of the true peak, or None (no phases at 192 kHz)
 
 
 def check_rate(sample_rate):
@@ -51,30 +49,31 @@ def check_rate(sample_rate):
     return rate
 
 
-def detector_bank(rate, dev):
-    """``audio.true_peak_bank(rate)`` on ``dev`` (cached), or None at 192 kHz."""
-    key = (str(dev), rate)
-    if key not in _banks:
-        bank = audio.true_peak_bank(rate)
-        _banks[key] = None if bank is None else torch.from_numpy(bank).pin_memory().to(dev, non_blocking=True)
-    return _banks[key]
+def k_weighting(rate):
+    """``audio.k_weighting(rate)`` as a host float64 tensor, made once per rate: ev_loudness and ev_meter read it by address."""
+    return recordings.device_table(("k_weighting", rate), lambda: audio.k_weighting(rate), "cpu")
 
 
-def enqueue(lib, base, meta_ptr, lens, rate, dev, stream, ws, series, bank, kcoef):
+def enqueue(base, meta_ptr, lens, rate, ws, series):
     """ev_meter of the items at base + start[k] (``meta_ptr``: device i64 start offsets followed by the lengths; ``lens``: host
-    lengths) -> Meter.  ``ws(nbytes)`` returns a device workspace of at least nbytes.  Arguments must already be valid."""
+    lengths) -> Meter.  ``ws(nbytes)`` returns a workspace of at least nbytes on the items' device.  Arguments must already
+    be valid."""
+    lib = _abi.load()
     k = len(lens)
+    nb = int(lib.ev_meter_workspace_bytes(k, max(lens), rate))
+    w = ws(nb)
+    dev = w.device
     res = torch.empty((6, k), dtype=torch.float32, device=dev)
     cols = max(lens) // (rate // 10)
     ser = torch.empty((2, k, cols), dtype=torch.float32, device=dev) if series else None
-    nb = int(lib.ev_meter_workspace_bytes(k, max(lens), rate))
-    w = ws(nb)
     n_host = np.ascontiguousarray(lens, dtype=np.int64)
+    bank = recordings.device_table(("true_peak_bank", rate), lambda: audio.true_peak_bank(rate), dev)   # None at 192 kHz
     phases, taps = (0, 21) if bank is None else (int(bank.shape[0]), int(bank.shape[1]))
-    _abi.check(lib.ev_meter(base, meta_ptr, meta_ptr + 8 * k, n_host.ctypes.data, k, rate, kcoef.ctypes.data,
+    _abi.check(lib.ev_meter(base, meta_ptr, meta_ptr + 8 * k, n_host.ctypes.data, k, rate, k_weighting(rate).data_ptr(),
                             None if bank is None else bank.data_ptr(), phases, taps, res.data_ptr(),
                             None if ser is None or ser.numel() == 0 else ser[0].data_ptr(),
-                            None if ser is None or ser.numel() == 0 else ser[1].data_ptr(), cols, w.data_ptr(), nb, stream))
+                            None if ser is None or ser.numel() == 0 else ser[1].data_ptr(), cols, w.data_ptr(), nb,
+                            torch.cuda.current_stream(dev).cuda_stream))
     mom = st = None
     if series:
         mom, st = ser[0][:, :max(0, cols - 3)], ser[1][:, :max(0, cols - 29)]
@@ -92,33 +91,12 @@ def meter(wav, sample_rate, lengths=None, series=False):
 
     Returns a ``Meter`` of device tensors.  Four launches, no sync; invalid arguments raise ValueError before anything is
     enqueued."""
-    if not (isinstance(wav, torch.Tensor) and wav.dim() == 2 and wav.dtype == torch.float32 and wav.is_cuda):
-        raise ValueError("wav must be a CUDA (B, L) float32 tensor")
-    B, L = int(wav.shape[0]), int(wav.shape[1])
-    if not 1 <= B <= 65535 or L < 1:
-        raise ValueError("wav must hold 1 to 65535 recordings of at least one sample, got shape %s" % (tuple(wav.shape),))
+    wav = recordings.recording_batch(wav)
+    B, L = wav.shape
     rate = check_rate(sample_rate)
-    if lengths is None:
-        lens = [L] * B
-    else:
-        if torch.is_tensor(lengths):
-            if lengths.device.type != "cpu":
-                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
-            lengths = lengths.tolist()
-        if isinstance(lengths, (str, bytes)) or any(isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer))
-                                                     for v in lengths):
-            raise ValueError("lengths must be %d integers in [0, %d], got %r" % (B, L, lengths))
-        lens = [int(v) for v in lengths]
-        if len(lens) != B or any(n < 0 or n > L for n in lens):
-            raise ValueError("lengths must be %d integers in [0, %d], got %s" % (B, L, lens))
+    lens = recordings.host_lengths(lengths, B, L)
     if not isinstance(series, (bool, np.bool_)):
         raise ValueError("series must be True or False, got %r" % (series,))
-    lib = _abi.load()
     dev = wav.device
-    if wav.stride(1) != 1:
-        wav = wav.contiguous()
-    stride = int(wav.stride(0))
-    meta = torch.tensor([b * stride for b in range(B)] + lens, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
-    return enqueue(lib, wav.data_ptr(), meta.data_ptr(), lens, rate, dev, torch.cuda.current_stream(dev).cuda_stream,
-                   lambda nb: torch.empty((nb,), dtype=torch.uint8, device=dev), bool(series), detector_bank(rate, dev),
-                   np.ascontiguousarray(audio.k_weighting(rate)))
+    meta, (p_meta, _) = recordings.upload([[b * wav.stride(0) for b in range(B)], lens], dev)     # start offsets, then lengths
+    return enqueue(wav.data_ptr(), p_meta, lens, rate, lambda nb: torch.empty((nb,), dtype=torch.uint8, device=dev), bool(series))

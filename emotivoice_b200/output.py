@@ -6,7 +6,7 @@ the filter banks and coefficients those stages read, and the loudness meter (ev_
 import numpy as np
 import torch
 
-from . import _abi, audio, loudness
+from . import _abi, audio, loudness, recordings
 
 _DTYPES = {"float32": torch.float32, "pcm16": torch.int16, "mulaw": torch.uint8, "alaw": torch.uint8}
 
@@ -16,48 +16,23 @@ class Chain:
 
     def __init__(self, device, lib, ws):
         self.device, self.lib, self._ws = device, lib, ws
-        self._banks = {}              # (up, down) -> device polyphase filter bank of ev_format_audio
-        self._kcoef = {}              # sample rate -> K-weighting coefficients of ev_loudness (host float64)
-        self._limit_banks = {}        # (model rate, output rate) -> (device detector bank, hold) of ev_limit
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
 
-    def _meta(self, arrays):
-        """Host int64 arrays -> one device int64 tensor (one pinned copy) and the device address of each array in it.  The
-        tensor must stay referenced until the last launch that reads it has been enqueued."""
-        meta = torch.from_numpy(np.concatenate([np.asarray(a, np.int64) for a in arrays]))
-        meta = meta.pin_memory().to(self.device, non_blocking=True)
-        ptrs, p = [], meta.data_ptr()
-        for a in arrays:
-            ptrs.append(p)
-            p += 8 * len(a)
-        return meta, ptrs
-
-    def _k_weighting(self, sr):
-        kc = self._kcoef.get(sr)
-        if kc is None:
-            kc = self._kcoef[sr] = np.ascontiguousarray(audio.k_weighting(sr))
-        return kc
-
     def _loudness(self, wav, n_in_ptr, items_ptr, k, sr, target):
         """ev_loudness of the k listed items (device i64 n_in / items pointers) -> device (lufs, peak, gain) float32 (k,)."""
-        kc = self._k_weighting(sr)
         res = torch.empty((3, k), dtype=torch.float32, device=self.device)
         stride = int(wav.stride(0))
         ws = self._ws("loudness", self.lib.ev_loudness_workspace_bytes(k, stride, sr))
-        _abi.check(self.lib.ev_loudness(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, kc.ctypes.data, float(target),
-                                        res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(), ws.numel(),
-                                        self._stream()))
+        _abi.check(self.lib.ev_loudness(wav.data_ptr(), stride, n_in_ptr, items_ptr, k, sr, loudness.k_weighting(sr).data_ptr(),
+                                        float(target), res[0].data_ptr(), res[1].data_ptr(), res[2].data_ptr(), ws.data_ptr(),
+                                        ws.numel(), self._stream()))
         return res[0], res[1], res[2]
 
     def _limit(self, wav, n_in_ptr, items_ptr, k, sr, rate, lufs0, lufs1, target, ceiling, out):
         """ev_limit of the k listed items into ``out`` (k, L) fp32, pre-gain 10^((target - L) / 20) of each given loudness."""
-        det = self._limit_banks.get((sr, rate))
-        if det is None:
-            bank, hold = audio.limit_bank(sr, rate)
-            det = self._limit_banks[(sr, rate)] = (torch.from_numpy(bank).to(self.device), hold)
-        bank, hold = det
+        bank, hold = recordings.device_table(("limit_bank", sr, rate), lambda: audio.limit_bank(sr, rate), self.device)
         L = audio.limit_lookahead(sr)
         stride = int(wav.stride(0))
         ws = self._ws("limit", self.lib.ev_limit_workspace_bytes(k, stride, L))
@@ -70,7 +45,7 @@ class Chain:
     def measure(self, wav, n_in, items, sr):
         """ev_loudness: (B,1,L) fp32 waveform at ``sr`` Hz, host per-item valid samples and the listed items -> device
         (lufs, peak) float32 (len(items),)."""
-        meta, (p_n, p_items) = self._meta([n_in, items])
+        meta, (p_n, p_items) = recordings.upload([n_in, items], self.device)
         lufs, pk, _ = self._loudness(wav, p_n, p_items, len(items), sr, -23.0)      # any valid target: the gain is not used
         return lufs, pk
 
@@ -78,12 +53,10 @@ class Chain:
         """ev_meter of the outputs ``format`` packed as float32 at ``rate`` Hz (a multiple of 10), output k at
         packed[offs[k]:offs[k + 1]] -> ``loudness.Meter``.  No sync."""
         lens = np.diff(offs).tolist()
-        meta, (p_meta,) = self._meta([np.concatenate([offs[:-1], lens])])
+        meta, (p_meta, _) = recordings.upload([offs[:-1], lens], self.device)
         if packed.numel() == 0:                  # every output is empty: ev_meter reads no sample, but needs an address
             packed = torch.empty((1,), dtype=torch.float32, device=self.device)
-        return loudness.enqueue(self.lib, packed.data_ptr(), p_meta, lens, rate, self.device, self._stream(),
-                                lambda nb: self._ws("meter", nb), series, loudness.detector_bank(rate, self.device),
-                                self._k_weighting(rate))
+        return loudness.enqueue(packed.data_ptr(), p_meta, lens, rate, lambda nb: self._ws("meter", nb), series)
 
     def format(self, wav, n_in, items, fmt, sr):
         """The listed items of a (B,1,L) fp32 waveform at ``sr`` Hz, host valid samples ``n_in`` (B ints <= L), in the
@@ -104,7 +77,7 @@ class Chain:
         arrays = [n_in, items, offs]
         if fmt.true_peak is not None or fmt.watermark is not None:
             arrays.append([int(n_in[b]) for b in items])                 # the limited / marked items' lengths, in listed order
-        meta, ptrs = self._meta(arrays)
+        meta, ptrs = recordings.upload(arrays, self.device)
         p_n, p_items, p_off = ptrs[:3]
         src, src_n, src_items, gain = wav, p_n, p_items, None
         stride = int(wav.stride(0))
@@ -127,9 +100,7 @@ class Chain:
             gain = self._loudness(src, src_n, src_items, k, sr, fmt.loudness)[2]
         bank = None
         if (fmt.up, fmt.down) != (1, 1):
-            bank = self._banks.get((fmt.up, fmt.down))
-            if bank is None:
-                bank = self._banks[(fmt.up, fmt.down)] = torch.from_numpy(audio.polyphase_bank(fmt.up, fmt.down)).to(self.device)
+            bank = recordings.polyphase_bank(fmt.up, fmt.down, self.device)
         _abi.check(lib.ev_format_audio(src.data_ptr(), int(src.stride(0)), src_n, src_items, k, p_off,
                                        None if bank is None else bank.data_ptr(), fmt.up, fmt.down,
                                        0 if bank is None else int(bank.shape[1]), audio.ENCODINGS[encoding], packed.data_ptr(),

@@ -23,7 +23,7 @@ Silence (every cell M = 0) gives z = 0.
 """
 import torch
 
-from . import _abi, audio, feats
+from . import _abi, audio, recordings
 
 DETECT_Z = audio.WATERMARK_DETECT_Z
 SR = 16000
@@ -41,31 +41,18 @@ def detect(wav, sample_rate, key, lengths=None):
     Returns (z float32, offset int32, phase int32) device tensors of shape (B,): the largest z of each recording and its grid
     offset tau and frame phase m0.  z >= DETECT_Z means the mark is present (see the module docstring for the bound).  No
     sync.  Invalid arguments raise ValueError before anything is enqueued."""
-    if not (isinstance(wav, torch.Tensor) and wav.dim() == 2 and wav.dtype == torch.float32 and wav.is_cuda):
-        raise ValueError("wav must be a CUDA (B, L) float32 tensor")
-    B, L = int(wav.shape[0]), int(wav.shape[1])
-    if not 1 <= B <= 65535 or L < 1:
-        raise ValueError("wav must hold 1 to 65535 recordings of at least one sample, got shape %s" % (tuple(wav.shape),))
+    wav = recordings.recording_batch(wav)
+    B, L = wav.shape
     rate = audio.plan(sample_rate, "float32", SR)[0]
     if rate < audio.WATERMARK_MIN_RATE:
         raise ValueError("the mark's band needs a rate of at least %d Hz, got %d" % (audio.WATERMARK_MIN_RATE, rate))
     key = audio.check_watermark(key)
-    if lengths is None:
-        lens = [L] * B
-    else:
-        if torch.is_tensor(lengths):
-            if lengths.device.type != "cpu":
-                raise ValueError("lengths must be host integers (a sequence or a CPU tensor)")
-            lengths = lengths.tolist()
-        lens = [int(v) for v in lengths]
-        if len(lens) != B or any(n < 0 or n > L for n in lens):
-            raise ValueError("lengths must be %d integers in [0, %d], got %s" % (B, L, lens))
+    lens = recordings.host_lengths(lengths, B, L)
     lib = _abi.load()
     dev = wav.device
-    wav = wav.contiguous()
     if rate != SR:
-        wav, lens = feats.resample(wav, lens, rate, SR)
-    n = feats.device_ints(lens, dev)
+        wav, lens = recordings.resample(wav, lens, rate, SR)
+    n = recordings.upload([lens], dev)[0]
     z = torch.empty((B,), dtype=torch.float32, device=dev)
     offset = torch.empty((B,), dtype=torch.int32, device=dev)
     phase = torch.empty((B,), dtype=torch.int32, device=dev)

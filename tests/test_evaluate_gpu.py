@@ -17,7 +17,7 @@ from scipy.signal import lfilter, resample_poly
 
 from audio_cases import KEYS
 from conftest import ROOT, load_golden
-from emotivoice_b200 import _abi, evaluate, feats
+from emotivoice_b200 import _abi, evaluate, feats, recordings
 from oracle import eval_oracle as O
 from test_audio_format_gpu import _check_float32, _reference
 
@@ -236,7 +236,7 @@ def test_speech_against_itself_half_gain_and_a_semitone_up(dev):
     w_ref = _rows([x, half, up], dev)
     n = [len(x)] * 3
     N = len(x) // 256 + 1
-    floor = feats.stft_features(w_ref, 512, 256, evaluate._stft(dev)[0], 0.0, bands=evaluate._stft(dev)[1], lengths=n)[0]
+    floor = feats.stft_features(w_ref, 512, 256, feats.scipy_hann(dev), 0.0, bands=feats.mel_bands(SR, 80, 0.0, 8000.0, dev), lengths=n)[0]
     assert float(floor[1, :, :N].min()) > math.log(1e-5) + 1.0   # half the gain keeps every band clear of the clamp
     c = _host(evaluate.compare(w_syn, w_ref, syn_lengths=n, ref_lengths=n, return_path=True))
     print("itself: mcd %g vuv %g f0 %g" % (c["mcd"][0], c["vuv_error"][0], c["f0_rmse"][0]))
@@ -273,8 +273,8 @@ def test_48k_input_gives_the_bits_of_its_16k_resampling(dev):
     s48, r48 = _rows(xs, dev), _rows(ys, dev)
     ls, lr = [len(x) for x in xs], [len(y) for y in ys]
     a = _host(evaluate.compare(s48, r48, sample_rate=48000, syn_lengths=ls, ref_lengths=lr, return_path=True))
-    s16, ls16 = feats.resample(s48.contiguous(), ls, 48000, SR)
-    r16, lr16 = feats.resample(r48.contiguous(), lr, 48000, SR)
+    s16, ls16 = recordings.resample(s48.contiguous(), ls, 48000, SR)
+    r16, lr16 = recordings.resample(r48.contiguous(), lr, 48000, SR)
     b = _host(evaluate.compare(s16, r16, syn_lengths=ls16, ref_lengths=lr16, return_path=True))
     for k in a:
         assert a[k].tobytes() == b[k].tobytes(), k
@@ -288,7 +288,7 @@ def test_48k_input_against_scipy_resampling_to_16k(dev):
     s48, r48 = _rows(xs, dev), _rows(ys, dev)
     ls, lr = [len(x) for x in xs], [len(y) for y in ys]
     for sig, t48, lens in ((xs, s48, ls), (ys, r48, lr)):
-        got, lens16 = feats.resample(t48.contiguous(), lens, 48000, SR)
+        got, lens16 = recordings.resample(t48.contiguous(), lens, 48000, SR)
         got = got.cpu().numpy()
         for b, x in enumerate(sig):
             y64, m = _reference(x, 1, 3)
@@ -373,7 +373,7 @@ def test_launch_counts_and_argument_errors(lib, dev):
     evaluate.compare(syn, ref, syn_lengths=ls, ref_lengths=lr)                  # warm the caches
     torch.cuda.synchronize()
     n0 = _abi.launch_count()
-    feats.stft_features(syn, 512, 256, evaluate._stft(dev)[0], 0.0, bands=evaluate._stft(dev)[1], lengths=ls)
+    feats.stft_features(syn, 512, 256, feats.scipy_hann(dev), 0.0, bands=feats.mel_bands(SR, 80, 0.0, 8000.0, dev), lengths=ls)
     n_stft = _abi.launch_count() - n0
     n0 = _abi.launch_count()
     feats.pitch_track(syn, SR, 256, continuous=False, lengths=ls)
