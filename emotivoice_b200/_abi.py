@@ -77,6 +77,8 @@ SIGNATURES = {
     "ev_eval_workspace_bytes": (_sz, [_i, _i, _i]),
     "ev_eval_compare": (_i, [_vp, _vp, ctypes.c_longlong, _vp, _i, _vp, _vp, ctypes.c_longlong, _vp, _i, _i, _vp, _vp, _vp, _vp,
                              ctypes.c_longlong, _vp, _sz, _vp]),
+    "ev_eval_align": (_i, [_vp, _vp, ctypes.c_longlong, _vp, _i, _vp, _vp, ctypes.c_longlong, _vp, _i, _i, _vp, _vp, _vp,
+                           ctypes.c_longlong, _vp, _sz, _vp]),
     "ev_flac_bound_bytes": (_sz, [ctypes.c_longlong]),
     "ev_flac_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
     "ev_flac_encode": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _vp, _sz, _vp]),
@@ -123,6 +125,8 @@ SIGNATURES = {
     "ev_stft_features": (_i, [_vp, ctypes.c_longlong, _vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "ev_pitch_workspace_bytes": (_sz, [_i, ctypes.c_longlong, _i, ctypes.c_double, _i]),
     "ev_pitch": (_i, [_vp, ctypes.c_longlong, _vp, _i, _i, ctypes.c_double, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ev_world_envelope": (_i, [_vp, ctypes.c_longlong, _vp, _i, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "ev_sp2mc": (_i, [_vp, ctypes.c_longlong, _i, _vp, _i, _vp, _vp]),
     "ev_style_create": (_i, [ctypes.POINTER(_vp), _i, ctypes.POINTER(EvStyleConfig)]),
     "ev_style_destroy": (None, [_vp]),
     "ev_style_bind_weights": (_i, [_vp, _vp, _sz, _vp, _i]),

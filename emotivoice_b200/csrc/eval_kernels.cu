@@ -80,9 +80,10 @@ __global__ void __launch_bounds__(EC_THREADS) eval_cep_kernel(const float* __res
   }
 }
 
-// cost[b * max_n * max_m + cell_index(i, j)] = d(i, j)
-__global__ void __launch_bounds__(ET_THREADS) eval_cost_kernel(const double* __restrict__ cep_syn, const int32_t* __restrict__ n_syn,
-                                                               int max_n, const double* __restrict__ cep_ref,
+// cost[b * max_n * max_m + cell_index(i, j)] = d(i, j); item b's cepstra start syn_rows / ref_rows frames apart
+__global__ void __launch_bounds__(ET_THREADS) eval_cost_kernel(const double* __restrict__ cep_syn, long long syn_rows,
+                                                               const int32_t* __restrict__ n_syn, int max_n,
+                                                               const double* __restrict__ cep_ref, long long ref_rows,
                                                                const int32_t* __restrict__ n_ref, int max_m,
                                                                double* __restrict__ cost) {
   pdl_entry();
@@ -91,8 +92,8 @@ __global__ void __launch_bounds__(ET_THREADS) eval_cost_kernel(const double* __r
   const int N = item_frames(n_syn, b, max_n), M = item_frames(n_ref, b, max_m);
   const int i0 = blockIdx.y * ET_TILE, j0 = blockIdx.x * ET_TILE;
   if (i0 >= N || j0 >= M) return;
-  const double* a = cep_syn + ((size_t)b * max_n + i0) * EV_CEPS;
-  const double* r = cep_ref + ((size_t)b * max_m + j0) * EV_CEPS;
+  const double* a = cep_syn + ((size_t)b * syn_rows + i0) * EV_CEPS;
+  const double* r = cep_ref + ((size_t)b * ref_rows + j0) * EV_CEPS;
   const int ni = min(ET_TILE, N - i0), nj = min(ET_TILE, M - j0);
   for (int e = threadIdx.x; e < ET_TILE * EV_CEPS; e += ET_THREADS) {
     const int row = e / EV_CEPS, k = e % EV_CEPS;
@@ -264,6 +265,41 @@ static bool eval_args_ok(int n_items, int max_n, int max_m) {
   return n_items >= 1 && n_items <= 65535 && max_n >= 1 && max_n <= EV_MAX_FRAMES && max_m >= 1 && max_m <= EV_MAX_FRAMES;
 }
 
+// the cost and DTW launches of ev_eval_compare and ev_eval_align, from cepstra (n_items, *_rows, 24) f64
+static int eval_align_tail(const double* cep_syn, long long syn_rows, const double* f0_syn, long long syn_frames, const int32_t* n_syn,
+                           int max_n, const double* cep_ref, long long ref_rows, const double* f0_ref, long long ref_frames,
+                           const int32_t* n_ref, int max_m, int n_items, double* stats, int32_t* counts, int32_t* path,
+                           long long path_stride, char* w, cudaStream_t st) {
+  w += align256((size_t)n_items * max_n * EV_CEPS * sizeof(double));
+  w += align256((size_t)n_items * max_m * EV_CEPS * sizeof(double));
+  double* cost = reinterpret_cast<double*>(w);
+  w += align256((size_t)n_items * max_n * max_m * sizeof(double));
+  unsigned char* codes = reinterpret_cast<unsigned char*>(w);
+  const size_t smem = 3 * EV_MAX_FRAMES * sizeof(double);
+  static std::atomic<uint64_t> attr_devs{0};
+  if (first_use_on_device(attr_devs))
+    cudaFuncSetAttribute(eval_dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  EV_TRY(launch("eval_cost_kernel", eval_cost_kernel, dim3((max_m + ET_TILE - 1) / ET_TILE, (max_n + ET_TILE - 1) / ET_TILE, n_items),
+                ET_THREADS, 0, st, cep_syn, syn_rows, n_syn, max_n, cep_ref, ref_rows, n_ref, max_m, cost));
+  return launch("eval_dtw_kernel", eval_dtw_kernel, dim3(n_items), ED_THREADS, smem, st, (const double*)cost, codes, n_syn, max_n, n_ref,
+                max_m, f0_syn, syn_frames, f0_ref, ref_frames, n_items, stats, counts, path, path_stride);
+}
+
+// the argument checks ev_eval_compare and ev_eval_align share
+static int eval_args_check(const char* what, int n_items, int max_n, int max_m, long long syn_frames, long long ref_frames,
+                           const int32_t* path, long long path_stride, size_t ws_bytes) {
+  EV_CHECK_ARG(n_items >= 1 && n_items <= 65535, "%s: n_items=%d must lie in [1, 65535]", what, n_items);
+  EV_CHECK_ARG(max_n >= 1 && max_n <= EV_MAX_FRAMES && max_m >= 1 && max_m <= EV_MAX_FRAMES,
+               "%s: max_n=%d, max_m=%d must lie in [1, %d]", what, max_n, max_m, EV_MAX_FRAMES);
+  EV_CHECK_ARG(syn_frames >= max_n && ref_frames >= max_m, "%s: %lld / %lld frames per row hold fewer than %d / %d", what,
+               syn_frames, ref_frames, max_n, max_m);
+  EV_CHECK_ARG(!path || path_stride >= (long long)max_n + max_m - 1, "%s: path_stride=%lld must be at least %d", what,
+               path_stride, max_n + max_m - 1);
+  const size_t need = eval_ws_bytes(n_items, max_n, max_m);
+  EV_CHECK_ARG(ws_bytes >= need, "%s: workspace of %zu bytes, %zu needed", what, ws_bytes, need);
+  return EV_OK;
+}
+
 }  // namespace ev
 
 using namespace ev;
@@ -280,36 +316,27 @@ int ev_eval_compare(const float* mel_syn, const double* f0_syn, long long syn_fr
                     size_t ws_bytes, void* stream) {
   EV_CHECK_ARG(mel_syn && f0_syn && n_syn && mel_ref && f0_ref && n_ref && table && stats && counts && ws,
                "ev_eval_compare: null argument");
-  EV_CHECK_ARG(n_items >= 1 && n_items <= 65535, "ev_eval_compare: n_items=%d must lie in [1, 65535]", n_items);
-  EV_CHECK_ARG(max_n >= 1 && max_n <= EV_MAX_FRAMES && max_m >= 1 && max_m <= EV_MAX_FRAMES,
-               "ev_eval_compare: max_n=%d, max_m=%d must lie in [1, %d]", max_n, max_m, EV_MAX_FRAMES);
-  EV_CHECK_ARG(syn_frames >= max_n && ref_frames >= max_m, "ev_eval_compare: %lld / %lld frames per row hold fewer than %d / %d",
-               syn_frames, ref_frames, max_n, max_m);
-  EV_CHECK_ARG(!path || path_stride >= (long long)max_n + max_m - 1, "ev_eval_compare: path_stride=%lld must be at least %d",
-               path_stride, max_n + max_m - 1);
-  const size_t need = eval_ws_bytes(n_items, max_n, max_m);
-  EV_CHECK_ARG(ws_bytes >= need, "ev_eval_compare: workspace of %zu bytes, %zu needed", ws_bytes, need);
+  EV_TRY(eval_args_check("ev_eval_compare", n_items, max_n, max_m, syn_frames, ref_frames, path, path_stride, ws_bytes));
   EV_TRY(use_device_of(mel_syn));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   char* w = static_cast<char*>(ws);
   double* cep_syn = reinterpret_cast<double*>(w);
-  w += align256((size_t)n_items * max_n * EV_CEPS * sizeof(double));
-  double* cep_ref = reinterpret_cast<double*>(w);
-  w += align256((size_t)n_items * max_m * EV_CEPS * sizeof(double));
-  double* cost = reinterpret_cast<double*>(w);
-  w += align256((size_t)n_items * max_n * max_m * sizeof(double));
-  unsigned char* codes = reinterpret_cast<unsigned char*>(w);
-  const size_t smem = 3 * EV_MAX_FRAMES * sizeof(double);
-  static std::atomic<uint64_t> attr_devs{0};
-  if (first_use_on_device(attr_devs))
-    cudaFuncSetAttribute(eval_dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  double* cep_ref = reinterpret_cast<double*>(w + align256((size_t)n_items * max_n * EV_CEPS * sizeof(double)));
   const int max_f = max_n > max_m ? max_n : max_m;
   EV_TRY(launch("eval_cep_kernel", eval_cep_kernel, dim3((max_f + EC_FRAMES - 1) / EC_FRAMES, n_items, 2), EC_THREADS, 0, st, mel_syn,
                 syn_frames, n_syn, max_n, mel_ref, ref_frames, n_ref, max_m, table, cep_syn, cep_ref));
-  EV_TRY(launch("eval_cost_kernel", eval_cost_kernel, dim3((max_m + ET_TILE - 1) / ET_TILE, (max_n + ET_TILE - 1) / ET_TILE, n_items),
-                ET_THREADS, 0, st, (const double*)cep_syn, n_syn, max_n, (const double*)cep_ref, n_ref, max_m, cost));
-  return launch("eval_dtw_kernel", eval_dtw_kernel, dim3(n_items), ED_THREADS, smem, st, (const double*)cost, codes, n_syn, max_n, n_ref,
-                max_m, f0_syn, syn_frames, f0_ref, ref_frames, n_items, stats, counts, path, path_stride);
+  return eval_align_tail(cep_syn, max_n, f0_syn, syn_frames, n_syn, max_n, cep_ref, max_m, f0_ref, ref_frames, n_ref, max_m, n_items,
+                         stats, counts, path, path_stride, w, st);
+}
+
+int ev_eval_align(const double* cep_syn, const double* f0_syn, long long syn_frames, const int32_t* n_syn, int max_n,
+                  const double* cep_ref, const double* f0_ref, long long ref_frames, const int32_t* n_ref, int max_m, int n_items,
+                  double* stats, int32_t* counts, int32_t* path, long long path_stride, void* ws, size_t ws_bytes, void* stream) {
+  EV_CHECK_ARG(cep_syn && f0_syn && n_syn && cep_ref && f0_ref && n_ref && stats && counts && ws, "ev_eval_align: null argument");
+  EV_TRY(eval_args_check("ev_eval_align", n_items, max_n, max_m, syn_frames, ref_frames, path, path_stride, ws_bytes));
+  EV_TRY(use_device_of(cep_syn));
+  return eval_align_tail(cep_syn, syn_frames, f0_syn, syn_frames, n_syn, max_n, cep_ref, ref_frames, f0_ref, ref_frames, n_ref, max_m,
+                         n_items, stats, counts, path, path_stride, static_cast<char*>(ws), reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -26,10 +26,14 @@ before anything is measured.  Definitions, per pair, at 16 kHz (other rates are 
    whose voicing differs.  voiced_pairs: the pairs voiced on both sides.  f0_rmse = sqrt(mean over those pairs of
    (1200 log2(f_syn / f_ref))^2) in cents, NaN when voiced_pairs = 0.
 
-This is not the SPTK / WORLD mel-cepstrum (mcep with alpha = 0.42) that many papers report MCD with: values are comparable
-between runs of this function, not with those papers.  The DTW is exact (no band, no fastdtw approximation), with the one step
-pattern above.  The cepstra, distances, DTW and path are bitwise ``oracle/eval_oracle.py``'s, and every pair's results are the
-same bits whatever else is in the batch and in which order.
+These cosine-series cepstra are this function's default (``cepstrum="mel"``); their values compare between runs of it.  For
+the MCD papers report, pass ``cepstrum="world"``: step 2 then takes c1..c24 of the SPTK mel-cepstrum of WORLD's spectral
+envelope, ``feats.sp2mc(feats.spectral_envelope(wav, 16000, 256, f0=F0), 24, alpha)`` with alpha = 0.42 by default (pyworld's
+CheapTrick and pysptk's sp2mc restated on the GPU in fp64; not checked against pyworld or pysptk), from the same F0 track.
+Steps 3 to 5 are unchanged.  The DTW is exact (no band, no fastdtw approximation), with the one step pattern above.  With
+``cepstrum="mel"`` the cepstra, distances, DTW and path are bitwise ``oracle/eval_oracle.py``'s; with ``"world"`` the
+distances, DTW and path are bitwise the oracle's on the GPU's mel-cepstra.  Every pair's results are the same bits whatever
+else is in the batch and in which order.
 
 Limits: each item holds at least ``feats.pitch_min_samples(16000)`` = 641 samples and at most 4096 frames at 16 kHz
 (4096 * 256 - 1 samples, about 65.5 s).  The workspace holds d and a predecessor code for every cell of every pair, sized by
@@ -38,7 +42,8 @@ pairs of 10 s.  One long item thus costs every pair of its batch its size: evalu
 similar length (sorted by length, say 32 to 128 pairs per call).  Forward only, no gradients.
 
 No call waits for the device: lengths and tables go up through pinned memory, and the results stay on the device.  The first
-call on a device builds its constant tables (the mel basis, the window, the cosine table) and allocates pinned host memory.
+call on a device builds its constant tables (the mel basis, the window, the cosine table; with ``"world"`` the sp2mc table of
+each alpha) and allocates pinned host memory.
 """
 import collections
 
@@ -53,6 +58,7 @@ N_MELS, N_CEPS = 80, 24
 MAX_FRAMES = 4096
 MIN_SAMPLES = feats.pitch_min_samples(SR)
 MAX_SAMPLES = MAX_FRAMES * HOP - 1
+WORLD_ALPHA = 0.42              # the all-pass constant MCD recipes use for 16 kHz speech
 
 Comparison = collections.namedtuple("Comparison", "mcd f0_rmse vuv_error voiced_pairs path_length path")
 Comparison.__doc__ = """Per-pair results of ``compare`` (device tensors of shape (B,)): mcd (dB), f0_rmse (cents) and vuv_error
@@ -80,18 +86,42 @@ def _features(wav, lens):
     return mel, f0
 
 
+def _check_cepstrum(cepstrum, alpha):
+    """-> the alpha of ``cepstrum="world"`` (None for "mel"); ValueError for an unknown kind, alpha with "mel", |alpha| >= 1."""
+    if cepstrum == "mel":
+        if alpha is not None:
+            raise ValueError("alpha applies to cepstrum='world' only")
+        return None
+    if cepstrum != "world":
+        raise ValueError("cepstrum must be 'mel' or 'world', got %r" % (cepstrum,))
+    alpha = WORLD_ALPHA if alpha is None else alpha
+    feats._check_sp2mc(N_CEPS, alpha)
+    return float(alpha)
+
+
+def _world_features(wav, lens, table):
+    """16 kHz (B, L) items -> (c1..c24 (B, F, 24) float64 of sp2mc(CheapTrick envelope), F0 (B, F) float64), F = L // 256 + 1:
+    one F0 track feeds both the envelope and the statistics."""
+    f0 = feats.pitch_track(wav, SR, HOP, continuous=False, lengths=lens)
+    _, cep = feats.envelope_features(wav, SR, HOP, f0=f0, lengths=lens, table=table, envelope=False)
+    return cep, f0
+
+
 @torch.no_grad()
-def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, return_path=False):
+def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, return_path=False, cepstrum="mel", alpha=None):
     """Compares row b of ``syn`` with row b of ``ref`` (see the module docstring for the definitions).
 
     ``syn``, ``ref``: CUDA (B, L_syn) and (B, L_ref) float32 tensors.  ``sample_rate``: the rate of both, one ``audio.plan``
     accepts; other rates than 16 kHz are resampled to 16 kHz first (``ev_format_audio``, as ``resample_poly``).
     ``syn_lengths``, ``ref_lengths``: the valid samples of each row (a sequence or a CPU tensor of B integers); None: the whole
     row.  Each item must hold 641 to 4096 * 256 - 1 samples once at 16 kHz.  ``return_path``: also return the DTW paths.
+    ``cepstrum``: "mel" (the log-mel's cosine series) or "world" (the SPTK mel-cepstrum of WORLD's envelope, warped by
+    ``alpha``, 0.42 by default, |alpha| < 1; alpha is for "world" only).
 
     Returns a ``Comparison`` of device tensors, with no host sync.  The workspace grows with B max(N) max(M): batch long
     test sets in chunks of similar lengths (module docstring).  Invalid arguments raise ValueError before anything is
     enqueued."""
+    alpha = _check_cepstrum(cepstrum, alpha)
     syn = recordings.recording_batch(syn, "syn")
     ref = recordings.recording_batch(ref, "ref")
     B = int(syn.shape[0])
@@ -120,8 +150,12 @@ def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, ret
         syn, ls = recordings.resample(syn, ls, rate, SR)
         ref, lr = recordings.resample(ref, lr, rate, SR)
     assert ls == ls16 and lr == lr16
-    mel_s, f0_s = _features(syn, ls)
-    mel_r, f0_r = _features(ref, lr)
+    if cepstrum == "world":
+        table = feats.mcep_table(feats.world_fft_size(SR), N_CEPS, alpha, dev, first=1)
+        (cep_s, f0_s), (cep_r, f0_r) = _world_features(syn, ls, table), _world_features(ref, lr, table)
+    else:
+        mel_s, f0_s = _features(syn, ls)
+        mel_r, f0_r = _features(ref, lr)
     ns = [n // HOP + 1 for n in ls]
     nr = [n // HOP + 1 for n in lr]
     counts_in, (p_ns, p_nr) = recordings.upload([ns, nr], dev, np.int32)
@@ -132,10 +166,15 @@ def compare(syn, ref, sample_rate=16000, syn_lengths=None, ref_lengths=None, ret
     path = torch.empty((B, p_max, 2), dtype=torch.int32, device=dev) if return_path else None
     nb = int(lib.ev_eval_workspace_bytes(B, max_n, max_m))
     ws = torch.empty((nb,), dtype=torch.uint8, device=dev)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    if cepstrum == "world":
+        _abi.check(lib.ev_eval_align(cep_s.data_ptr(), f0_s.data_ptr(), int(cep_s.shape[1]), p_ns, max_n, cep_r.data_ptr(),
+                                     f0_r.data_ptr(), int(cep_r.shape[1]), p_nr, max_m, B, stats.data_ptr(), counts.data_ptr(),
+                                     None if path is None else path.data_ptr(), p_max, ws.data_ptr(), nb, stream))
+        return Comparison(stats[0], stats[1], stats[2], counts[0], counts[1], path)
     table = recordings.device_table("cos_table", cos_table, dev)
     _abi.check(lib.ev_eval_compare(mel_s.data_ptr(), f0_s.data_ptr(), int(mel_s.shape[2]), p_ns, max_n,
                                    mel_r.data_ptr(), f0_r.data_ptr(), int(mel_r.shape[2]), p_nr, max_m, B,
                                    table.data_ptr(), stats.data_ptr(), counts.data_ptr(),
-                                   None if path is None else path.data_ptr(), p_max, ws.data_ptr(), nb,
-                                   torch.cuda.current_stream(dev).cuda_stream))
+                                   None if path is None else path.data_ptr(), p_max, ws.data_ptr(), nb, stream))
     return Comparison(stats[0], stats[1], stats[2], counts[0], counts[1], path)

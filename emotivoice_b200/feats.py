@@ -1,7 +1,9 @@
 """Log-mel spectrograms and frame energy of recordings on the GPU, with the reference's names and signatures:
 ``TacotronSTFT`` (models/prompt_tts_modified/tacotron_stft.py:46-80), ``mel_spectrogram_torch`` (mel_process.py:77-110),
 ``Energy`` (models/prompt_tts_modified/feats.py:159-213) and ``Pitch`` (feats.py:83-156), pyworld.dio + pyworld.stonemask
-restated on the GPU in fp64 (``ev_pitch``, csrc/pitch_kernels.cu).
+restated on the GPU in fp64 (``ev_pitch``, csrc/pitch_kernels.cu); and, with no reference counterpart, WORLD spectral
+envelopes (``spectral_envelope``, pyworld.cheaptrick) and SPTK mel-cepstra (``sp2mc``, pysptk.sp2mc) in fp64 (``ev_world_envelope``,
+``ev_sp2mc``, csrc/world_kernels.cu), the features of paper-style mel-cepstral distortion.
 
 These are the features the reference's data preparation computes per utterance on the CPU: the mel targets the acoustic model
 and the vocoder were trained on (prompt_dataset.py:29-49), the mel distance of its validation and training step
@@ -313,9 +315,8 @@ def _check_pitch_config(sr, hop):
         raise ValueError("hop length %r is not supported: it must be an integer in [%d, %d]" % ((hop,) + PITCH_HOP_RANGE))
 
 
-def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=False):
-    """One ev_pitch call on wav (B, N) CUDA float32/float64 -> pitch (B, F) float64 [, DIO's raw contour (B, F)],
-    F = pitch_frames(N, sr, hop); frames past an item's own count are 0."""
+def _pitch_input(wav, sr, hop, lengths):
+    """The checks of pitch_track and spectral_envelope -> host lengths."""
     _check(wav, "wav")
     _check_pitch_config(sr, hop)
     if wav.dim() != 2:
@@ -327,6 +328,14 @@ def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=Fals
     m = pitch_min_samples(sr)
     if any(v < m for v in ls):
         raise ValueError("an item of %d samples is too short to filter: at least %d at %d Hz" % (min(ls), m, int(sr)))
+    return ls
+
+
+def pitch_track(wav, sr, hop, continuous=True, log=False, lengths=None, raw=False):
+    """One ev_pitch call on wav (B, N) CUDA float32/float64 -> pitch (B, F) float64 [, DIO's raw contour (B, F)],
+    F = pitch_frames(N, sr, hop); frames past an item's own count are 0."""
+    ls = _pitch_input(wav, sr, hop, lengths)
+    B, N = wav.shape
     lib = _abi.load()
     dev = wav.device
     x = wav.detach().to(torch.float64).contiguous()
@@ -379,3 +388,104 @@ class Pitch:
         d = (d.detach() if torch.is_tensor(d) else torch.from_numpy(np.asarray(d))).to(device=pitch.device, dtype=torch.float32).reshape(1, -1)
         T, F = d.shape[1], pitch.shape[1]
         return align.average_by_duration(d, pitch, torch.tensor([T]), torch.tensor([F]))
+
+
+# ---- spectral envelope and mel-cepstrum -------------------------------------------------------------------------------------
+SP2MC_MAX_ORDER = 255
+
+
+def world_fft_size(sr):
+    """pyworld.cheaptrick's default FFT size at sr Hz: 2^(1 + int(log(3 sr / 71 + 1) / log 2)) (512 at 8 kHz, 1024 at 16 to
+    24 kHz, 2048 at 44.1 and 48 kHz)."""
+    return 2 ** (1 + int(np.log(3.0 * sr / 71.0 + 1.0) / np.log(2.0)))
+
+
+def sp2mc_table(n_fft, order, alpha):
+    """(order + 1, n_fft // 2 + 1) float64: the matrix of pysptk.sp2mc(sp, order, alpha) on log(sp), i.e. c = irfft(log sp),
+    c[0] /= 2, then SPTK's freqt(c, order, alpha) over all n_fft coefficients of c, its mirror half included.  Built by running
+    the freqt recursion on the columns of the irfft matrix in fp64."""
+    bins = n_fft // 2 + 1
+    c = np.fft.irfft(np.eye(bins), n=n_fft, axis=1).T          # (n_fft, bins): c = c_of_log @ log sp
+    c[0] /= 2.0
+    a, b = float(alpha), 1.0 - float(alpha) * float(alpha)
+    g = np.zeros((order + 1, bins))
+    for i in range(n_fft - 1, -1, -1):
+        d = g.copy()
+        g[0] = c[i] + a * d[0]
+        if order >= 1:
+            g[1] = b * d[0] + a * d[1]
+        for j in range(2, order + 1):
+            g[j] = d[j - 1] + a * (d[j] - g[j - 1])
+    return g
+
+
+def _check_sp2mc(order, alpha):
+    if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or not 0 <= int(order) <= SP2MC_MAX_ORDER:
+        raise ValueError("order must be an integer in [0, %d], got %r" % (SP2MC_MAX_ORDER, order))
+    if isinstance(alpha, bool) or not isinstance(alpha, (int, float, np.integer, np.floating)) or not abs(float(alpha)) < 1.0:
+        raise ValueError("alpha must be a number with |alpha| < 1, got %r" % (alpha,))
+
+
+def mcep_table(n_fft, order, alpha, dev, first=0):
+    """Rows first..order of sp2mc_table(n_fft, order, alpha) on dev, made once per device."""
+    key = ("sp2mc", int(n_fft), int(order), float(alpha), int(first))
+    return recordings.device_table(key, lambda: np.ascontiguousarray(sp2mc_table(int(n_fft), int(order), float(alpha))[first:]), dev)
+
+
+def envelope_features(wav, sr, hop, f0=None, lengths=None, table=None, envelope=True):
+    """One ev_world_envelope call -> (sp (B, F, bins) float64 or None, table @ log sp (B, F, rows) float64 or None).  The
+    arguments are spectral_envelope's; table: a device (rows, bins) float64 table or None."""
+    ls = _pitch_input(wav, sr, hop, lengths)
+    B, N = wav.shape
+    F = pitch_frames(N, sr, hop)
+    if f0 is None:
+        f0 = pitch_track(wav, sr, hop, continuous=False, lengths=lengths)
+    elif not (torch.is_tensor(f0) and f0.device == wav.device and f0.dtype == torch.float64 and tuple(f0.shape) == (B, F)):
+        raise ValueError("f0 must be a (%d, %d) float64 tensor on %s" % (B, F, wav.device))
+    lib = _abi.load()
+    dev = wav.device
+    x = wav.detach().to(torch.float64).contiguous()
+    f0 = f0.detach().contiguous()
+    bins = world_fft_size(int(sr)) // 2 + 1
+    sp = torch.empty((B, F, bins), dtype=torch.float64, device=dev) if envelope else None
+    mc = None if table is None else torch.empty((B, F, int(table.shape[0])), dtype=torch.float64, device=dev)
+    ns = None if lengths is None else recordings.upload([ls], dev)[0]
+    _abi.check(lib.ev_world_envelope(x.data_ptr(), N, None if ns is None else ns.data_ptr(), B, int(sr),
+                                     pitch_frame_period(int(sr), int(hop)), F, f0.data_ptr(), None if sp is None else sp.data_ptr(),
+                                     None if table is None else table.data_ptr(), 0 if table is None else int(table.shape[0]),
+                                     None if mc is None else mc.data_ptr(), None, torch.cuda.current_stream(dev).cuda_stream))
+    return sp, mc
+
+
+def spectral_envelope(wav, sample_rate, hop, f0=None, lengths=None):
+    """pyworld.cheaptrick at its defaults (q1 = -0.15, f0_floor 71, fft_size = world_fft_size(sample_rate)) on the GPU in fp64
+    (``ev_world_envelope``; oracle/world_oracle.py lists every assumed detail, not checked against pyworld).
+
+    wav (B, N) CUDA float32/float64 at ``sample_rate`` Hz with the frames of ``pitch_track(wav, sample_rate, hop)`` (frame
+    period 1000 hop / sample_rate ms); ``f0``: their F0, a (B, F) float64 tensor on wav's device, or None for
+    ``pitch_track(continuous=False)``; ``lengths`` as pitch_track's.  Returns the power envelope (B, F, fft_size // 2 + 1)
+    float64; frames past an item's own count are 0.  WORLD's random noise is replaced by a floor of 2^-52 on every power
+    bin, so each item's envelope is the same in any batch and silence gives finite values.  No host sync."""
+    return envelope_features(wav, sample_rate, hop, f0, lengths)[0]
+
+
+def sp2mc(sp, order, alpha):
+    """pysptk.sp2mc(sp, order, alpha) on the GPU (``ev_sp2mc``): sp a CUDA float64 (..., bins) power envelope, bins =
+    fft_size // 2 + 1 with fft_size a power of two in [4, 2048], every value > 0 -> (..., order + 1) float64 mel-cepstra.
+    order in [0, 255], |alpha| < 1.  The map is ``sp2mc_table`` (fp64, built once per (fft_size, order, alpha) and device)
+    applied to log(sp)."""
+    _check_sp2mc(order, alpha)
+    if not (torch.is_tensor(sp) and sp.is_cuda and sp.dtype == torch.float64 and sp.dim() >= 1):
+        raise ValueError("sp must be a CUDA float64 tensor (..., bins)")
+    bins = int(sp.shape[-1])
+    n_fft = 2 * (bins - 1)
+    if bins < 3 or n_fft > 2048 or n_fft & (n_fft - 1):
+        raise ValueError("sp has %d bins: it must have fft_size // 2 + 1 with fft_size a power of two in [4, 2048]" % bins)
+    lib = _abi.load()
+    dev = sp.device
+    x = sp.detach().contiguous()
+    table = mcep_table(n_fft, int(order), float(alpha), dev)
+    out = torch.empty(tuple(sp.shape[:-1]) + (int(order) + 1,), dtype=torch.float64, device=dev)
+    _abi.check(lib.ev_sp2mc(x.data_ptr(), x.numel() // bins, bins, table.data_ptr(), int(order) + 1, out.data_ptr(),
+                            torch.cuda.current_stream(dev).cuda_stream))
+    return out

@@ -389,6 +389,14 @@ EV_API int ev_eval_compare(const float* mel_syn, const double* f0_syn, long long
                            const float* mel_ref, const double* f0_ref, long long ref_frames, const int32_t* n_ref, int max_m,
                            int n_items, const double* table, double* stats, int32_t* counts, int32_t* path, long long path_stride,
                            void* ws, size_t ws_bytes, void* stream);
+/* The cost and DTW launches of ev_eval_compare from caller cepstra: cep_syn (n_items, syn_frames, 24) f64 DEVICE, row (k, f)
+ * holding c_1..c_24 of pair k's syn frame f; cep_ref likewise with ref_frames.  d, the DTW, the path and the statistics are
+ * ev_eval_compare's, with every other argument as there.  ws: ev_eval_workspace_bytes(n_items, max_n, max_m) bytes.  Two
+ * launches; each pair's results are bitwise the same in any batch or order.  No allocation, no sync. */
+EV_API int ev_eval_align(const double* cep_syn, const double* f0_syn, long long syn_frames, const int32_t* n_syn, int max_n,
+                         const double* cep_ref, const double* f0_ref, long long ref_frames, const int32_t* n_ref, int max_m,
+                         int n_items, double* stats, int32_t* counts, int32_t* path, long long path_stride, void* ws,
+                         size_t ws_bytes, void* stream);
 
 /* Number of kernel launches this library has enqueued in this process (bench.py's
  * `gpu_launches`). */
@@ -641,6 +649,30 @@ EV_API int ev_stft_features(const float* wav, long long item_stride, const int64
 EV_API size_t ev_pitch_workspace_bytes(int B, long long item_stride, int fs, double frame_period, int F);
 EV_API int ev_pitch(const double* x, long long item_stride, const int64_t* n_samples, int B, int fs, double frame_period, int F,
                     int flags, double* raw_f0, double* pitch, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Spectral envelopes of fp64 recordings: WORLD's CheapTrick at pyworld's defaults (q1 = -0.15, f0_floor 71), restated from the
+ * published algorithm (oracle/world_oracle.py lists every assumed detail, W1-W11; not checked against pyworld).  x, item_stride,
+ * n_samples, B, fs, frame_period, F and the frames F_b of each item are ev_pitch's.  f0 (B, F) f64 DEVICE: the F0 of each frame
+ * in Hz; a frame whose F0 is at or below 3 fs / (fft_size - 3), above fs / 4 or not finite is analysed at 500 Hz.  fft_size =
+ * 2^(1 + int(log(3 fs / 71 + 1) / log 2)): 512 at 8 kHz, 1024 at 16 to 24 kHz, 2048 at 44.1 and 48 kHz; bins = fft_size / 2 + 1.
+ * WORLD's random noise is replaced by a floor of 2^-52 on every smoothed power bin, so every frame depends on its own samples
+ * and digital silence gives finite output; the linear smoothing is summed over the bins it spans (what WORLD's difference of
+ * two running sums equals in exact arithmetic), so no smoothed bin is negative and every output is finite for finite input.
+ *   sp (B, F, bins) f64 or NULL: the power envelope (pyworld.cheaptrick's output).
+ *   mc (B, F, n_out) f64 or NULL: mc_table (n_out, bins) f64 DEVICE, 1 <= n_out <= 256, times the log envelope of the frame
+ *   (the log before the final exp): with the table of sp2mc (emotivoice_b200.feats.sp2mc_table) the mel-cepstrum.
+ * One of sp, mc is needed.  Frames f >= F_b are stored as 0.  status (i32, may be NULL): ev_pitch's bits (|= 1 a sample is not
+ * finite, |= 2 an item is shorter than 2 round(fs / 50) + 1 samples or longer than item_stride: its outputs are all 0).  fp64
+ * throughout; one launch.  Each output depends only on its own item: a batch is bitwise its items' single calls.  No
+ * workspace, no allocation, no sync. */
+EV_API int ev_world_envelope(const double* x, long long item_stride, const int64_t* n_samples, int B, int fs, double frame_period,
+                             int F, const double* f0, double* sp, const double* mc_table, int n_out, double* mc, int32_t* status,
+                             void* stream);
+/* Mel-cepstra of power envelopes (pysptk.sp2mc through a table): mc[r, k] = sum_j table[k, j] log(sp[r, j]), rows r < n_frames
+ * of sp (n_frames, bins) f64 DEVICE, bins = fft_size / 2 + 1 with fft_size a power of two in [4, 2048], sp > 0; table
+ * (n_out, bins) f64 DEVICE, 1 <= n_out <= 256; mc (n_frames, n_out) f64.  One launch (none for n_frames = 0); each row depends
+ * only on its own. */
+EV_API int ev_sp2mc(const double* sp, long long n_frames, int bins, const double* table, int n_out, double* mc, void* stream);
 
 #ifdef __cplusplus
 }
